@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- images/sec of Mask R-CNN R-50-FPN inference @ 3x800x1216, 1000 proposals, 100 detections
-(BASELINE.json `metric`, configs[2]: batch 8 per B200), one process per GPU.
+(BASELINE.json `metric`, configs[2]: batch 8 per GPU), one process per GPU.
 
-  python bench.py --gpus 1 --steps 20 --warmup 3            # our arm (sm_100a engine)
+  python bench.py --gpus 1 --steps 20 --warmup 3            # our arm (sm_90a engine)
+  python bench.py --steps 5 --dump-outputs /tmp/out         # + the detections of the last timed step as .npy files
   python bench.py --impl reference --steps 2 --warmup 1     # reference arm: the reference path on the host cores
 
 A "step" = one pass of the whole hot path (trunk, FPN, RPN, proposals, RoIAlign, box head, per-class NMS,
@@ -68,7 +69,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1400.0, "fallback"       # B200_PROFILING.md fallback figures
+    return 3350.0, 989.0, "H100 SXM data sheet (dense BF16, 700 W)"
 
 
 # ----------------------------------------------------------------------------- reference arm / cpu baseline
@@ -81,8 +82,8 @@ def cpu_reference_images_per_sec(steps, warmup, arch="resnet50"):
     """The reference's CPU path for this workload: its detector graph under torch-CPU fp32 + its RoIAlign loop +
     its greedy NMS + numpy post-processing, as restated in oracle/ (the reference tree does not exist on the GPU
     box; oracle/_ref holds its compiled RoIAlign loop when it was built here).  One step = one image (bounded sample).
-    Threads = what this process may really use (affinity mask capped by the cgroup quota), not os.cpu_count(): a 128-thread pool
-    inside a smaller quota was the 12x swing of the round-1 figure.  >= 1 warm-up, median of >= 3, per-stage break-out."""
+    Threads = what this process may really use (affinity mask capped by the cgroup quota), not os.cpu_count(): a pool larger than the
+    quota oversubscribes the cores.  `warmup` warm-up steps, median of `steps` timed steps, per-stage break-out."""
     import torch
     from oracle import network as net
     from oracle import usable_cpus
@@ -90,10 +91,10 @@ def cpu_reference_images_per_sec(steps, warmup, arch="resnet50"):
     torch.set_num_threads(n)
     P = net.synthetic_params(arch)
     img = net.synthetic_image(1, H, W)
-    for _ in range(max(1, warmup)):
+    for _ in range(warmup):
         net.detect_and_mask_fpn(img, P, arch=arch)
     times, stages = [], {}
-    for _ in range(max(3, steps)):
+    for _ in range(steps):
         t = {}
         t0 = time.perf_counter()
         net.detect_and_mask_fpn(img, P, arch=arch, timers=t)
@@ -139,8 +140,7 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    steps = max(3, min(args.steps, 5))
-    warm = max(1, min(args.warmup, 2))
+    steps, warm = args.steps, args.warmup
     ips, dt, n, stages, runs, raw = cpu_reference_images_per_sec(steps, warm, args.arch)
     line = {"impl": "reference", "metric": METRIC if args.arch == "resnet50" else METRIC.replace("R-50", "R-101"), "value": ips, "unit": "images/sec", "n_gpus": args.gpus,
             "steps": runs, "warmup": warm, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -165,8 +165,8 @@ MIRROR_KW = dict(conv_body_layers=['conv1', 'bn1', 'relu', 'maxpool', 'layer1', 
 
 def pin_to_gpu_numa_node(local):
     """Bind this process (the launch thread and, by first touch, the pinned host buffers it allocates next) to the CPUs of the GPU's NUMA
-    node: at N=8 eight processes otherwise share two sockets at random and the H2D streams / launch threads cross the socket link
-    (round-1: device-side scaling 0.998 but end-to-end 0.973).  Best effort; returns a description for the JSON line."""
+    node: at N=8 eight processes otherwise share two sockets at random and the H2D streams / launch threads cross the socket link.
+    Best effort; returns a description for the JSON line."""
     try:
         import torch
         pr = torch.cuda.get_device_properties(local)
@@ -206,7 +206,7 @@ def time_cuda(fn, torch, warm=2, reps=5, flush=None):
 def microbench_roialign(torch, dev, hbm_peak, which):
     """BASELINE.json configs[4]: 100 000 RoIs x 256 channels x 50x68 map, pooled 7x7 (and 14x14), sampling_ratio 2.  Algorithmic bytes =
     output write + map + RoIs (SURVEY.md 8d: 5 023 081 600 B for 7x7).  L2 is flushed between timed iterations.  The reference's own
-    CUDA kernel (lib/cppcuda_cffi/src/cuda/roi_align_forward_cuda_kernel.cu compiled unmodified for sm_100a into oracle/_ref) is timed on the
+    CUDA kernel (lib/cppcuda_cffi/src/cuda/roi_align_forward_cuda_kernel.cu compiled unmodified for sm_90a into oracle/_ref) is timed on the
     same inputs when that build exists."""
     import ctypes
     import numpy as np
@@ -323,6 +323,8 @@ def run_ours(args):
     eng.check_range()      # the kind::f16 conv path raises a device flag if an activation left the fp16 range (never on this workload)
     rois_per_image = float(eng.buffer("roi_counts").float().mean().item())
     dets_per_image = float(eng.buffer("det_counts").float().mean().item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, np)
 
     # ---- (B) end to end through the public call with HOST buffers: model.detect(pinned host batch) uploads through its two staging
     # buffers on a copy stream (H2D of step i+1 overlaps the compute of step i); every step's results are read back to pinned host memory
@@ -387,7 +389,7 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms, e2e_ms = t.tolist()
 
-    # ---- roofline of the dominant kernel family (conv_tcgen05_kernel), measured live with CUDA events on the launch stream
+    # ---- roofline of the dominant kernel family (conv_wgmma_kernel), measured live with CUDA events on the launch stream
     roof, roi_roof, roi_engine, micro, cpu_base = None, None, None, None, None
     if rank == 0:
         hbm_peak, bf16_peak, which = peaks()
@@ -401,17 +403,12 @@ def run_ours(args):
         for (m, f, st, bn) in prof:
             stage_ms[stage_names[st]] = round(stage_ms.get(stage_names[st], 0.0) + m, 4)
         f16_kind = eng.cfg.conv_kind == 0
-        # kind::f16 issues at the bf16 rate; kind::tf32 at half of it (B200_PROFILING.md nominal 2.25 vs 1.1 PF)
+        # fp16 wgmma issues at the bf16 rate; tf32 at half of it (H100 SXM data sheet: 989 vs 495 TFLOP/s dense)
         mma_peak = bf16_peak if f16_kind else bf16_peak / 2.0
         ach = conv_flops / (conv_ms * 1e-3) / 1e12
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "r02_dram_bytes.json")
-        if os.path.exists(tp):       # dram__bytes_read.sum + dram__bytes_write.sum of the conv launches of one step (an ncu pass of this very command)
-            td = json.load(open(tp))
-            traffic, traffic_src = td.get("conv_family_bytes_per_step"), td.get("source")
-        roof = {"bound": "tensor", "kernel": "conv_tcgen05_kernel (%d launches/step)" % len(conv), "achieved": ach, "peak": mma_peak, "unit": "TFLOP/s",
-                "frac": ach / mma_peak, "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": "%s bf16_tflops_sustained%s" % (which, " (kind::f16 MMA rate)" if f16_kind else "/2 (tf32 MMA rate is half of bf16)"),
+        roof = {"bound": "tensor", "kernel": "conv_wgmma_kernel (%d launches/step)" % len(conv), "achieved": ach, "peak": mma_peak, "unit": "TFLOP/s",
+                "frac": ach / mma_peak,
+                "peak_source": "%s%s" % (which, " (fp16 MMA rate)" if f16_kind else ", /2 (tf32 MMA rate is half of bf16)"),
                 "executed_tflops": 3.0 * ach, "frac_executed": 3.0 * ach / mma_peak,
                 "note": "achieved = algorithmic 2*MAC FLOPs of all conv/GEMM launches / their summed CUDA-event time; the kernel executes 3 %s MMAs "
                         "per algorithmic product (error-compensated hi/lo split, fp32-accurate), frac_executed counts those" % ("fp16" if f16_kind else "TF32"),
@@ -438,7 +435,7 @@ def run_ours(args):
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32 (%s tensor-core products, fp32 accumulate)" % ("3xFP16 hi/lo" if eng.cfg.conv_kind == 0 else "3xTF32"),
                 "data": "synthetic", "per_gpu_value": value / world,
                 "config": {"workload": WORKLOAD if args.arch == "resnet50" else WORKLOAD.replace("R-50", "R-101").replace("configs[2]", "configs[3] model"), "global_batch": BATCH * world, "parallelism": "dp%d (images sharded, no data-path collective)" % world,
-                           "l2": "inputs alternate between two 93 MB batches and every step streams ~11 GB of activations (>> 126 MB L2)",
+                           "l2": "inputs alternate between two 93 MB batches and every step streams ~11 GB of activations (>> 50 MB L2)",
                            "cuda_graph": True, "tflops_algorithmic": value * gflop_img / 1e3,
                            "rois_per_image": rois_per_image, "dets_per_image": dets_per_image, "numa": numa},
                 "clocks": clocks,
@@ -452,6 +449,24 @@ def run_ours(args):
         emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path, eng, np):
+    """What the timed path computed in its last step, as a caller of detector.detect() receives it: per image the detection count, and
+    per detection slot [image, slot] the box, score, class and 28x28 mask probabilities; slots past an image's count are zeroed (the
+    engine leaves them unwritten).  float32 / float64 .npy files, about 3 MB in all."""
+    os.makedirs(path, exist_ok=True)
+    counts = eng.buffer("det_counts").cpu().numpy().astype(np.int64)
+    B, cap = eng.buffer("det_scores").shape[:2]
+    live = np.arange(cap)[None, :] < counts[:, None]
+    m = eng.buffer("masks")
+    out = {"det_counts": counts.astype(np.float64), "det_boxes": eng.buffer("det_boxes").float().cpu().numpy(),
+           "det_scores": eng.buffer("det_scores").float().cpu().numpy(), "det_classes": eng.buffer("det_classes").cpu().numpy().astype(np.float64),
+           "masks": m.float().view(B, cap, m.shape[-2], m.shape[-1]).cpu().numpy()}
+    for name, a in out.items():
+        if name != "det_counts":
+            a = np.where(live.reshape(live.shape + (1,) * (a.ndim - 2)), a, 0).astype(a.dtype)
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 _json_out = None
@@ -472,13 +487,14 @@ def main():
     os.dup2(2, 1)
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100, help="timed steps (both arms; the reference arm times one image per step)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-microbench", action="store_true", help="skip the configs[4] RoIAlign microbench keys")
     ap.add_argument("--no-reference-flow", action="store_true", help="skip the batch-1 notebook-shaped end-to-end figure")
     ap.add_argument("--no-config1", action="store_true", help="reference arm: skip the Fast R-CNN R-50-C4 (configs[0]) CPU timing")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the detections of the last timed step to DIR/<name>.npy")
     ap.add_argument("--arch", default="resnet50", choices=["resnet50", "resnet101"],
                     help="resnet101 = BASELINE.json configs[3] model (not the headline metric)")
     args = ap.parse_args()

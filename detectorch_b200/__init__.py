@@ -1,3 +1,3 @@
-"""detectorch_b200 -- B200-native (sm_100a) two-stage detector inference hot path behind the
+"""detectorch_b200 -- H100-native (sm_90a) two-stage detector inference hot path behind the
 reference's own operator / model interface (ignacio-rocco/detectorch lib/model, lib/utils)."""
 __version__ = "0.1"

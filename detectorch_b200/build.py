@@ -1,5 +1,5 @@
-"""Builds the sm_100a CUDA library IN-TREE (detectorch_b200/csrc/libdetectorch_b200.so) with nvcc.
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot."""
+"""Builds the sm_90a CUDA library IN-TREE (detectorch_b200/csrc/libdetectorch_b200.so) with nvcc.
+The .so is a build product (git-ignored); build() recreates it whenever a CUDA source is newer."""
 import os
 import subprocess
 import sys
@@ -8,16 +8,22 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libdetectorch_b200.so")
 SOURCES = ["capi_ops.cu", "capi_engine.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DNDEBUG"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DNDEBUG"]
+
+
+STAMP = LIB + ".flags"       # the nvcc command line the library was built with (a library built for another target is rebuilt)
 
 
 def needs_build():
-    if not os.path.exists(LIB):
+    if not os.path.exists(LIB) or not os.path.exists(STAMP):
         return True
+    with open(STAMP) as f:
+        if f.read() != " ".join(NVCC_FLAGS + SOURCES):
+            return True
     t = os.path.getmtime(LIB)
     for root, _, files in os.walk(CSRC):
         for f in files:
-            if f.endswith((".cu", ".cuh", ".h")) and os.path.getmtime(os.path.join(root, f)) > t:
+            if f.endswith((".cu", ".cuh", ".inc", ".h")) and os.path.getmtime(os.path.join(root, f)) > t:
                 return True
     hdr = os.path.join(HERE, "..", "include", "detectorch_b200.h")
     return os.path.exists(hdr) and os.path.getmtime(hdr) > t
@@ -32,6 +38,8 @@ def build(force=False, verbose=False):
         cmd.insert(1, "-Xptxas=-v")
         print(" ".join(cmd))
     subprocess.check_call(cmd, cwd=CSRC)
+    with open(STAMP, "w") as f:
+        f.write(" ".join(NVCC_FLAGS + SOURCES))
     return LIB
 
 

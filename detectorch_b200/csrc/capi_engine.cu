@@ -126,7 +126,7 @@ __global__ void scale16_kernel(const float* __restrict__ scale, const MatInfo* _
 }
 inline int grid_for(long long n, int threads = 256) {
     long long g = (n + threads - 1) / threads;
-    return (int)(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g));
+    return (int)(g < 1 ? 1 : (g > num_sms() * 16 ? num_sms() * 16 : g));
 }
 
 // ---------------------------------------------------------------------------------- engine
@@ -448,8 +448,6 @@ struct ProgBuilder {
         s.Cout = c.cout; s.kh = c.k; s.kw = c.k; s.pad = kpad; s.stride = stride;
         s.shift = zero_shift ? e->wvec((*cw)["__zeros"].shift) : e->wvec(c.shift);
         s.tap0 = tap0; s.ntaps = ntaps;
-        // mask head: the long-K layers keep the cross terms in their own accumulator (mask logits: 1e-4 absolute bar)
-        s.no_merge = (stage == ST_MASK_HEAD && (ntaps > 0 ? ntaps : c.k * c.k) * (c.cin / 32) > 16) ? 1 : 0;
         if (e->cfg.conv_kind == 0) {
             // kind::f16 three-term product: fp16 halves of w * multiplier(matrix); the multiplier is undone through a per-op scale vector
             const size_t n16 = align_up((size_t)c.cout, 64);
@@ -579,10 +577,10 @@ cudaError_t fn_roi_box(Engine* e, cudaStream_t s) {
     const int R = e->cfg.batch * e->cfg.post_nms_top_n;
     // per-image counts: padded rows carry zero boxes (collect_kernel) -> harmless, fully defined output
     if (e->cfg.exact_roialign)
-        roi_align_nhwc_kernel<<<R < 148 * 64 ? R : 148 * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), nullptr, R, 256, 7, 7,
+        roi_align_nhwc_kernel<<<R < num_sms() * 64 ? R : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), nullptr, R, 256, 7, 7,
                                                                           2, e->buf("roi_feat"));
     else
-        roi_align_fast_nhwc_kernel<<<R < 148 * 64 ? R : 148 * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), R, 256, 7, 7,
+        roi_align_fast_nhwc_kernel<<<R < num_sms() * 64 ? R : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), R, 256, 7, 7,
                                                                                e->buf("roi_feat"));
     return cudaGetLastError();
 }
@@ -611,10 +609,10 @@ cudaError_t fn_mask_rois(Engine* e, cudaStream_t s) {
 cudaError_t fn_mask_roi_feat(Engine* e, cudaStream_t s) {
     const int D = e->cfg.batch * e->cfg.det_cap;
     if (e->cfg.exact_roialign)
-        roi_align_nhwc_kernel<<<D < 148 * 64 ? D : 148 * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), nullptr, D, 256, 14,
+        roi_align_nhwc_kernel<<<D < num_sms() * 64 ? D : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), nullptr, D, 256, 14,
                                                                           14, 2, e->buf("mask_feat"));
     else
-        roi_align_fast_nhwc_kernel<<<D < 148 * 64 ? D : 148 * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), D, 256, 14, 14,
+        roi_align_fast_nhwc_kernel<<<D < num_sms() * 64 ? D : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), D, 256, 14, 14,
                                                                                e->buf("mask_feat"));
     return cudaGetLastError();
 }
@@ -808,9 +806,8 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
         // The mask logits carry the tightest parity bar (1e-4 absolute) and sit behind four K = 2304 convolutions, where the tensor
         // core's truncating fp32 accumulate is the error floor.  precise_mask shortens the chains by SPLITTING K: each 3x3 convolution
         // runs as two launches over filter taps [0,5) and [5,9); the second adds the first's fp32 result in its epilogue (RES_TILE on the
-        // output buffer itself, round-to-nearest) before the ReLU.  That halves the error like the former 128-wide / 3-accumulator
-        // tiles did, but keeps the 256-wide 2-SM tiles (converted A tiles are shared by all 256 output channels): 2 x ~205 us instead
-        // of 640 us per layer.  precise_mask = 2 selects the old 128-wide rotating-accumulator tiles.
+        // output buffer itself, round-to-nearest) before the ReLU.  precise_mask = 2 instead runs 64-wide tiles with 3 rotating
+        // main-term accumulators.
         const int mbn = c.precise_mask == 2 ? 128 : 0;
         pb.fn(ST_MASK_ROIS, fn_mask_rois);
         pb.fn(ST_MASK_ROI_FEAT, fn_mask_roi_feat);

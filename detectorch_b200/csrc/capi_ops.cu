@@ -10,7 +10,7 @@
 
 using namespace dt;
 
-extern "C" const char* dt_version(void) { return "detectorch_b200 0.1 (sm_100a)"; }
+extern "C" const char* dt_version(void) { return "detectorch_b200 0.1 (sm_90a)"; }
 
 // ================================================================================== RoIAlign
 extern "C" int dt_roi_align_forward_nchw(const float* features, const float* rois, int64_t num_rois, int roi_cols, int channels,
@@ -21,7 +21,7 @@ extern "C" int dt_roi_align_forward_nchw(const float* features, const float* roi
         fprintf(stderr, "[detectorch_b200] roi_align: rois must have 4 or 5 columns\n");
         return 0;
     }
-    const int grid = (int)(num_rois < (int64_t)kNumSMs * 64 ? num_rois : (int64_t)kNumSMs * 64);
+    const int grid = (int)(num_rois < (int64_t)num_sms() * 64 ? num_rois : (int64_t)num_sms() * 64);
     roi_align_nchw_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(features, rois, (long long)num_rois, roi_cols, channels, height, width,
                                                                   pooled_height, pooled_width, spatial_scale, sampling_ratio, out);
     DT_CHECK_CUDA(cudaGetLastError());
@@ -47,7 +47,7 @@ extern "C" int launch_roi_align_backward_cuda(const int nthreads, const float* t
     (void)nthreads;
     if (num_rois <= 0 || channels <= 0) return 1;
     if (roi_cols != 4 && roi_cols != 5) { fprintf(stderr, "[detectorch_b200] roi_align backward: rois must have 4 or 5 columns\n"); return 0; }
-    const int grid = num_rois < kNumSMs * 8 ? num_rois : kNumSMs * 8;
+    const int grid = num_rois < num_sms() * 8 ? num_rois : num_sms() * 8;
     roi_align_backward_nchw_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(top_diff, bottom_rois, (long long)num_rois, roi_cols, channels, height,
                                                                           width, pooled_height, pooled_width, spatial_scale, sampling_ratio,
                                                                           bottom_diff);
@@ -116,7 +116,7 @@ extern "C" int dt_roi_align_backward_deterministic(const float* top_diff, const 
                                                                        w.v0, w.src, w.wgt, w.cnt);
     roi_bwd_sort_kernel<<<1, 1024, 0, st>>>(w.k0, w.v0, w.k1, w.v1, (int)total_contributions);
     const long long cells = (long long)batch * height * width;
-    const int grid = (int)(cells < (long long)kNumSMs * 16 ? cells : (long long)kNumSMs * 16);
+    const int grid = (int)(cells < (long long)num_sms() * 16 ? cells : (long long)num_sms() * 16);
     roi_bwd_reduce_kernel<<<grid, 256, 0, st>>>(w.k0, w.v0, (long long)total_contributions, w.src, w.wgt, w.cnt, top_diff, channels, height * width,
                                                cells, pooled_height * pooled_width, bottom_diff);
     DT_CHECK_CUDA(cudaGetLastError());
@@ -135,7 +135,7 @@ extern "C" int dt_roi_align_forward_nhwc(const float* const* feats, const int* h
     RoiLevels lv;
     lv.num_levels = num_levels;
     for (int i = 0; i < num_levels; ++i) { lv.feat[i] = feats[i]; lv.H[i] = heights[i]; lv.W[i] = widths[i]; lv.scale[i] = scales[i]; }
-    const int grid = max_rois < kNumSMs * 64 ? max_rois : kNumSMs * 64;
+    const int grid = max_rois < num_sms() * 64 ? max_rois : num_sms() * 64;
     roi_align_nhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(lv, rois, level, num_rois_dev, max_rois, channels, pooled_height,
                                                                   pooled_width, sampling_ratio, out);
     DT_CHECK_CUDA(cudaGetLastError());
@@ -178,9 +178,9 @@ bool smem_map_plan(int batch, int channels, int height, int width, int64_t num_r
     pl->smem = map_bytes + (size_t)pl->nwarps * pl->group * (ph + pw) * 32;
     if (pl->smem > 227 * 1024) return false;
     const int slabs = batch * (channels / kSlabC);
-    int a = kNumSMs, b = slabs;
+    int a = num_sms(), b = slabs;
     while (b) { const int t = a % b; a = b; b = t; }
-    int chunks = kNumSMs / a;                                        // slabs * chunks is a multiple of the SM count
+    int chunks = num_sms() / a;                                        // slabs * chunks is a multiple of the SM count
     const int64_t per_pass = (int64_t)pl->nwarps * pl->group;       // RoIs one CTA covers per sweep of its warps
     const int64_t max_chunks = (num_rois + per_pass - 1) / per_pass;
     if (chunks > max_chunks) chunks = (int)max_chunks;
@@ -202,8 +202,8 @@ extern "C" int dt_roi_align_forward_nchw_fast(const float* features, int batch, 
                                               int sampling_ratio, float* out, void* workspace, dt_stream_t stream) {
     if (num_rois <= 0) return 1;
     // channel slab: the largest divisor of C (multiple of 4) whose [CS][ph*pw] fp32 tile fits ~50 KB of shared memory
-    // smaller tiles = more resident CTAs and more L1 left for the gathers; measured on B200: 28 KB (128 channels x 49 bins)
-    // beats 56 / 14 / 7 KB (tunable: DT_ROI_TILE_KB)
+    // smaller tiles = more resident CTAs and more L1 left for the gathers; default 28 KB (128 channels x 49 bins)
+    // (tunable: DT_ROI_TILE_KB)
     static int tile_kb = 0;
     if (!tile_kb) { const char* e = getenv("DT_ROI_TILE_KB"); tile_kb = e ? atoi(e) : 28; if (tile_kb < 4) tile_kb = 4; if (tile_kb > 100) tile_kb = 100; }
     int cs = 0;
@@ -226,7 +226,7 @@ extern "C" int dt_roi_align_forward_nchw_fast(const float* features, int batch, 
         roi_tables_kernel<<<(unsigned)((ents + 255) / 256), 256, 0, st>>>(rois, (long long)num_rois, roi_cols, spatial_scale, height, width,
                                                                          pooled_height, pooled_width, batch, tab);
         DT_CHECK_CUDA(cudaGetLastError());
-        const int grid = pl.num_items < kNumSMs ? pl.num_items : kNumSMs;
+        const int grid = pl.num_items < num_sms() ? pl.num_items : num_sms();
 #define DT_LAUNCH_SMEM_MAP(PHW, BATCHED)                                                                                                   \
     {                                                                                                                                      \
         static bool attr = false;                                                                                                          \
@@ -254,7 +254,7 @@ extern "C" int dt_roi_align_forward_nchw_fast(const float* features, int batch, 
         attr_set = true;
     }
     const int per_sm = (int)(200 * 1024 / (tile_bytes + 2048)) < 8 ? (int)(200 * 1024 / (tile_bytes + 2048)) : 8;
-    const int grid = (int)(num_rois < (int64_t)kNumSMs * per_sm ? num_rois : (int64_t)kNumSMs * per_sm);
+    const int grid = (int)(num_rois < (int64_t)num_sms() * per_sm ? num_rois : (int64_t)num_sms() * per_sm);
     roi_align_fast_nchw_out_kernel<<<grid, 256, tile_bytes, st>>>(nhwc, rois, (long long)num_rois, roi_cols, channels, cs, height, width, pooled_height,
                                                                   pooled_width, spatial_scale, out);
     DT_CHECK_CUDA(cudaGetLastError());
@@ -487,7 +487,7 @@ __global__ void tf32_residual_kernel(const float* __restrict__ w, float* __restr
 
 extern "C" int dt_tf32_residual(const float* w, float* w_lo, int64_t n, dt_stream_t stream) {
     if (n <= 0) return 1;
-    const int grid = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+    const int grid = (int)((n + 255) / 256 < num_sms() * 8 ? (n + 255) / 256 : num_sms() * 8);
     tf32_residual_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, w_lo, (long long)n);
     DT_CHECK_CUDA(cudaGetLastError());
     return 1;
@@ -516,7 +516,7 @@ int conv2d_nhwc_impl(int kind, const float* x, int N, int H, int W, int Cin, int
     s.residual = residual; s.res_pix_stride = Cout; s.up_src = up_src; s.up_h = up_h; s.up_w = up_w;
     s.res_mode = res_mode; s.relu = relu; s.sigmoid_ch = sigmoid_ch; s.passes = passes; s.force_block_n = force_block_n;
     s.precise = force_block_n < 0;
-    if (force_block_n < 0) s.force_block_n = 128;        // -1: the precise 128-wide tile (3 rotating accumulators)
+    if (force_block_n < 0) s.force_block_n = 0;          // -1: the precise tile (64 wide, 3 rotating accumulators; conv_build)
     ConvLayer L;
     if (!conv_build(s, &L)) return 0;
     DT_CHECK_CUDA(conv_launch(L, (cudaStream_t)stream));
@@ -526,7 +526,7 @@ int conv2d_nhwc_impl(int kind, const float* x, int N, int H, int W, int Cin, int
 
 extern "C" int dt_fp16_split(const float* w, int64_t n, float multiplier, void* w_hi16, void* w_lo16, dt_stream_t stream) {
     if (n <= 0) return 1;
-    const int grid = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+    const int grid = (int)((n + 255) / 256 < num_sms() * 8 ? (n + 255) / 256 : num_sms() * 8);
     fp16_split_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, multiplier, reinterpret_cast<__half*>(w_hi16), reinterpret_cast<__half*>(w_lo16),
                                                              (long long)n);
     DT_CHECK_CUDA(cudaGetLastError());

@@ -1,11 +1,11 @@
-// detectorch_b200 -- host side of the tcgen05 conv/GEMM engine: TMA descriptor construction,
+// detectorch_b200 -- host side of the wgmma conv/GEMM engine: TMA descriptor construction,
 // tile-geometry selection and launch.  No torch types; raw device pointers only.
 #pragma once
 #include <cudaTypedefs.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include "conv_tcgen05.cuh"
+#include "conv_wgmma.cuh"
 
 namespace dt {
 
@@ -109,13 +109,8 @@ inline bool make_tmap_4d_f16(CUtensorMap* tm, const void* base, uint64_t d0, uin
 struct ConvLayer {
     ConvParams p;
     int block_n;
-    int nmain = 1;      // rotating main-term accumulators (3 = precise: shorter truncating accumulation chains)
-    bool two_sm = true; // cta_group::2 MMA (default) vs 1-SM MMA + multicast (DT_CONV_1SM=1)
+    int nmain = 1;      // rotating main-term accumulators (3 = shorter truncating accumulation chains; 64-wide tiles)
     int kind = KIND_TF32X3;
-    int ring = 0;       // residual prefetch ring (short-K RES_TILE layers)
-    int slots = 1;      // epilogue staging slots per group (2 = the TMA store of a chunk drains while the next chunk is computed)
-    bool ws = false;    // weight-stationary halo kernel (64-wide, one N tile): the whole weight matrix stays resident in shared memory
-    int halo = 0;       // 1 = 3x3 halo variant: one (8 + 2)-pixel-wide A box per filter row serves its three taps; 2 = stem row-parity halo
     dim3 grid;
     bool valid = false;
 };
@@ -140,9 +135,8 @@ struct ConvSpec {
     // x_lo / y_lo at the LOW plane, each [N,H,W,C] fp16
     const void* x_lo; void* y_lo;
     int tap0, ntaps;                              // K-split: only filter taps [tap0, tap0+ntaps) (ntaps == 0: all kh*kw)
-    int force_block_n;                            // 0 = auto
-    int precise;                                  // BLOCK_N == 128 only: 3 rotating accumulators instead of TMEM double-buffering
-    int no_merge;                                 // keep the cross terms in their own accumulator whatever K is (mask head: tightest parity bar)
+    int force_block_n;                            // 0 = auto (64 or 128)
+    int precise;                                  // 64-wide tiles with 3 rotating main-term accumulators (shorter accumulation chains)
 };
 
 inline void choose_box(int Wo, int Ho, int N, int max_w, int* wbox, int* hbox, int* nbox) {
@@ -162,61 +156,13 @@ inline void choose_box(int Wo, int Ho, int N, int max_w, int* wbox, int* hbox, i
     *wbox = bw; *hbox = bh; *nbox = bn;
 }
 
-// MMA mode per layer.  cta_group::2 (each SM keeps half of the weight tile: smaller stages, half the B-operand ingest and shared-memory
-// reads per SM) measured 1-22 % faster on every 128- and 256-wide layer once the cluster-scope fences were gone from the per-k-block
-// signalling; the 64-wide layers (stem, 64-channel stage, RPN heads) are a wash or up to 5 % slower, so they stay on 1-SM MMAs with
-// multicast weights.  DT_CONV_MMA=1sm|2sm forces one mode everywhere (tests exercise both).
-inline bool conv_use_two_sm(int block_n, int num_kb) {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("DT_CONV_MMA");
-        v = (e && e[0] == '1') ? 1 : ((e && e[0] == '2') ? 2 : 0);
-    }
-    if (v == 1) return false;
-    if (v == 2) return true;
-    (void)num_kb;
-    return block_n > 64;
-}
-
-inline bool conv_merge_acc(int num_kb) {
-    static int thr = -1;
-    if (thr < 0) { const char* e = getenv("DT_CONV_MERGE_KB"); thr = e ? atoi(e) : 72; }
-    return num_kb <= thr;
-}
-
-// DT_CONV_HALO=0 switches the halo variant of the 64 / 128-wide 3x3 plane-input layers off (A/B, tests)
-inline bool conv_use_halo() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("DT_CONV_HALO"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v == 1;
-}
-
-// weight-stationary form of the 64-wide halo kernels: DT_CONV_WS=0 off, 1 (default) the stem only, 2 also the 64-channel 3x3 layers
-inline int conv_ws_mode() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("DT_CONV_WS"); v = e ? atoi(e) : 1; }
-    return v;
-}
-
-// DT_CONV_NARROW1=0: 64-wide short-K layers and the stem keep 3 rotating accumulators (A/B, tests)
-inline bool conv_narrow_one_acc() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("DT_CONV_NARROW1"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v == 1;
-}
-
-// Persistent launch geometry: work items = (pairs of M-tiles) x (N-tiles); one 2-CTA cluster per SM pair (74 on B200),
-// each looping over items pair, pair + num_pairs, ...  An odd M-tile count gets one all-out-of-range surplus tile (TMA
-// zero-fills its loads and clips its stores) so that both CTAs of a pair always run the same multicast protocol.
+// Persistent launch geometry: work items = M-tiles x N-tiles; one CTA per SM, each looping over items blockIdx.x, + gridDim.x, ...
 inline void finish_grid(ConvLayer* L, int n_tiles) {
     ConvParams& p = L->p;
-    const int mtiles = p.tiles_w * p.tiles_h * p.tiles_n;
-    p.m_pairs = (mtiles + 1) / 2;
+    p.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
     p.n_tiles = n_tiles;
-    const int items = p.m_pairs * p.n_tiles;
-    const int pairs = items < kNumSMs / 2 ? items : kNumSMs / 2;
-    L->two_sm = conv_use_two_sm(L->block_n, p.kh * p.kw * p.cin_blocks);
-    L->grid = dim3((unsigned)(2 * pairs), 1, 1);
+    const int items = p.m_tiles * p.n_tiles;
+    L->grid = dim3((unsigned)(items < num_sms() ? items : num_sms()), 1, 1);
     L->valid = true;
 }
 
@@ -231,44 +177,33 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     const int Wo = (s.W + 2 * s.pad - s.kw) / s.stride + 1;
     int wbox, hbox, nbox;
     choose_box(Wo, Ho, s.N, 256 / s.stride, &wbox, &hbox, &nbox);
+    // Tiles are at most 128 channels wide: the main and cross accumulators of a 64 x 128 warpgroup tile are 128 registers per thread,
+    // which is what the register file leaves with two MMA warpgroups per SM.  A wider request (256) runs as 128-wide tiles.
     int bn = s.force_block_n;
-    if (bn == 0) bn = s.Cout > 128 ? 256 : (s.Cout > 64 ? 128 : 64);
+    if (bn == 0 || bn > 128) bn = s.Cout > 64 ? 128 : 64;
+    // tf32 k-steps are half as long as fp16 ones: a long-K tf32 layer's accumulation chain is twice as long, and the 3xTF32 engine met the
+    // 1e-4 mask-logit bar only with the main term rotated over three accumulators (64-wide tiles)
+    if (s.precise || (s.kind != KIND_F16X3 && s.kh * s.kw * (s.Cin / 32) > 16)) bn = 64;
+    if (bn != 64 && bn != 128) { fprintf(stderr, "[detectorch_b200] conv_build: unsupported tile width %d\n", bn); return false; }
     L->block_n = bn;
-    // Halo variant (conv_tcgen05.cuh): 3x3 / stride 1 / pad 1 over fp16 planes, tiles up to 128 channels wide in the two instantiations
-    // the engine uses for them (64: 1-SM MMA, 3 rotating accumulators; 128: 2-SM MMA, 1 accumulator).  Tiles are 8 pixels wide and
-    // (hbox x nbox) = 16 rows high; the A box is 10 pixels wide.
-    L->halo = conv_use_halo() && s.x_lo && s.kind == KIND_F16X3 && s.kh == 3 && s.kw == 3 && s.stride == 1 && s.pad == 1 && s.ntaps == 0 &&
-              s.passes != 1 && s.W >= 10 && ((bn == 64 && !conv_use_two_sm(64, 0)) || (bn == 128 && conv_use_two_sm(128, 0) && !s.precise));
-    if (L->halo) {
-        long best = -1;
-        for (int h = 16; h >= 1; h >>= 1) {
-            const int n = 16 / h;
-            if (h > s.H || n > s.N) continue;
-            const long tiles = (long)ceil_div(Wo, 8) * ceil_div(Ho, h) * ceil_div(s.N, n);
-            if (best < 0 || tiles < best) { best = tiles; hbox = h; nbox = n; }
-        }
-        if (best < 0) L->halo = 0; else wbox = 8;
-    }
-    const int abox_w = L->halo ? wbox + 2 : wbox * s.stride;
     const int K = s.kh * s.kw * s.Cin;
     const uint64_t xs = (uint64_t)s.x_pix_stride * 4;
     if (s.x_lo) {
         if (s.kind != KIND_F16X3 || s.x_pix_stride != s.Cin) { fprintf(stderr, "[detectorch_b200] conv_build: fp16 input planes need the f16 kind and a dense layout\n"); return false; }
         const uint64_t hs = (uint64_t)s.Cin * 2;
-        if (!make_tmap_4d_f16(&p.tm_a, s.x, s.Cin, s.W, s.H, s.N, hs, hs * s.W, hs * s.W * s.H, 32, abox_w, hbox * s.stride, nbox, s.stride, s.stride) ||
-            !make_tmap_4d_f16(&p.tm_a2, s.x_lo, s.Cin, s.W, s.H, s.N, hs, hs * s.W, hs * s.W * s.H, 32, abox_w, hbox * s.stride, nbox, s.stride, s.stride))
+        if (!make_tmap_4d_f16(&p.tm_a, s.x, s.Cin, s.W, s.H, s.N, hs, hs * s.W, hs * s.W * s.H, 32, wbox * s.stride, hbox * s.stride, nbox, s.stride, s.stride) ||
+            !make_tmap_4d_f16(&p.tm_a2, s.x_lo, s.Cin, s.W, s.H, s.N, hs, hs * s.W, hs * s.W * s.H, 32, wbox * s.stride, hbox * s.stride, nbox, s.stride, s.stride))
             return false;
         p.a_planes = 1;
     } else if (!make_tmap_4d(&p.tm_a, s.x, s.Cin, s.W, s.H, s.N, xs, xs * s.W, xs * s.W * s.H, 32, wbox * s.stride, hbox * s.stride, nbox,
                              s.stride, s.stride))
         return false;
-    // each CTA of a pair fetches half of the BLOCK_N weight rows and multicasts them
     if (s.kind == KIND_F16X3) {
-        if (!make_tmap_2d_f16(&p.tm_bhi, s.w_hi, K, s.Cout, (uint64_t)K * 2, 32, bn / 2)) return false;
-        if (!make_tmap_2d_f16(&p.tm_blo, s.w_lo ? s.w_lo : s.w_hi, K, s.Cout, (uint64_t)K * 2, 32, bn / 2)) return false;
+        if (!make_tmap_2d_f16(&p.tm_bhi, s.w_hi, K, s.Cout, (uint64_t)K * 2, 32, bn)) return false;
+        if (!make_tmap_2d_f16(&p.tm_blo, s.w_lo ? s.w_lo : s.w_hi, K, s.Cout, (uint64_t)K * 2, 32, bn)) return false;
     } else {
-        if (!make_tmap_2d(&p.tm_bhi, s.w_hi, K, s.Cout, (uint64_t)K * 4, 32, bn / 2)) return false;
-        if (!make_tmap_2d(&p.tm_blo, s.w_lo ? s.w_lo : s.w_hi, K, s.Cout, (uint64_t)K * 4, 32, bn / 2)) return false;
+        if (!make_tmap_2d(&p.tm_bhi, s.w_hi, K, s.Cout, (uint64_t)K * 4, 32, bn)) return false;
+        if (!make_tmap_2d(&p.tm_blo, s.w_lo ? s.w_lo : s.w_hi, K, s.Cout, (uint64_t)K * 4, 32, bn)) return false;
     }
     L->kind = s.kind == KIND_F16X3 ? KIND_F16X3 : KIND_TF32X3;
     p.range_flag = s.range_flag;
@@ -307,52 +242,12 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     p.wo = Wo; p.ho = Ho; p.nimg = s.N;
     p.cout = s.Cout;
     p.a_tile_bytes = wbox * hbox * nbox * 128;
-    p.a_halo_bytes = L->halo ? (wbox + 2) * hbox * nbox * 64 : 0;
     p.relu = s.relu; p.sigmoid_ch = s.sigmoid_ch; p.res_mode = s.res_mode;
     p.passes = s.passes == 1 ? 1 : 3;
-    // 256-wide tiles: (main + cross) accumulators fill the 512 TMEM columns, so the epilogue cannot overlap the next tile's MMAs.  One
-    // merged accumulator leaves room for two tiles (measured: -0.7 ms per step when applied to every layer up to K = 2304); the price is
-    // a 3x longer truncating-accumulate chain (main and both cross terms in one accumulator), which the trunk / FPN / RPN / box-head
-    // activations can afford (they sit at 1e-5 of their 1e-4 bar) and the mask-head layers cannot (no_merge).
-    // 64-wide tiles rotate the main term over 3 accumulators (short truncating-accumulate chains at no TMEM cost) -- except at K <= 256, where
-    // one accumulator already is a chain of at most 16 steps and the two extra TMEM reads + RN adds per chunk only lengthen the epilogue
-    const bool narrow1 = bn == 64 && s.kind == KIND_F16X3 && !L->halo && p.ntaps * p.cin_blocks <= 8 && conv_narrow_one_acc();
-    L->nmain = (bn == 64) ? (narrow1 ? 1 : 3) : ((bn == 128 && s.precise) ? 3 : ((bn == 256 && !s.no_merge && conv_merge_acc(p.ntaps * p.cin_blocks)) ? 0 : 1));
+    // 64-wide tiles rotate the main term over 3 accumulators (same register budget as one 128-wide pair) -- except at K <= 256, where
+    // one accumulator already is a chain of at most 16 k-blocks
+    L->nmain = (bn == 64 && (s.precise || p.ntaps * p.cin_blocks > 8)) ? 3 : 1;
     finish_grid(L, ceil_div(s.Cout, bn));
-    {
-        // Residual prefetch ring for the conv3 + residual layers (K <= 512): -15..26 % at K <= 256 when it was introduced; K = 512 (16 k-blocks
-        // per tile) was 11 % slower with it while a ring kernel had two 48 KB pipeline stages -- with in-place 32 KB stages it gains 15 %
-        // with 3 ring tiles / 3 stages and 23 % with 2 ring tiles / 4 stages (same-box sweep over DT_CONV_RING_KB / DT_CONV_RING2_KB).
-        static int use_ring = -1, ring_kb = 16, ring2_kb = 16;
-        if (use_ring < 0) {
-            const char* e = getenv("DT_CONV_RES_RING"); use_ring = e ? atoi(e) : 1;
-            const char* e1 = getenv("DT_CONV_RING_KB"); if (e1) ring_kb = atoi(e1);             // ring for at most this many k-blocks per tile
-            const char* e2 = getenv("DT_CONV_RING2_KB"); if (e2) ring2_kb = atoi(e2);           // from this many k-blocks on: 2 ring tiles (one more stage)
-        }
-        L->ring = (use_ring && L->nmain == 0 && L->two_sm && L->kind == KIND_F16X3 && s.res_mode == RES_TILE && p.ntaps * p.cin_blocks <= ring_kb) ? 1 : 0;
-        if (L->ring && ring2_kb > 0 && p.ntaps * p.cin_blocks >= ring2_kb) L->ring = 2;
-    }
-    {
-        // Two staging slots per epilogue group (the TMA store of a chunk drains while the next chunk is computed) for tiles up to 128 wide,
-        // where the extra 32 KB do not cost a pipeline stage.  256-wide tiles take ONE slot = one more pipeline stage: since the store warps
-        // decoupled the stores from the workers, the second slot no longer pays for itself there (same-box sweep, profiles/r02_summary.md:
-        // short-K 256-wide layers -5..20 % with one slot, long-K +15 % with two; with the stores still issued by worker thread 0 the
-        // short-K layers had been 10-16 % faster with two).  DT_CONV_SLOTS=1|2 forces one setting (A/B, tests).
-        static int force = -1;
-        if (force < 0) { const char* e = getenv("DT_CONV_SLOTS"); force = e ? atoi(e) : 0; }
-        L->slots = bn <= 128 ? 2 : 1;
-        if (force == 1 || force == 2) L->slots = force;
-        if (L->halo) L->slots = 2;
-    }
-    // weight-stationary form of the 64-wide 3x3 halo layer (one N tile, all 18 k-blocks resident, 2-SM MMA): measured a wash to +4 % slower
-    // than the streaming form (167 -> 175 us; the stem gains 17 %), so it is opt-in here (DT_CONV_WS=2)
-    L->ws = L->halo == 1 && bn == 64 && conv_ws_mode() == 2 && s.Cout <= 64 && s.kh * s.kw * p.cin_blocks <= 18;
-    if (L->ws) L->two_sm = true;
-    if (L->nmain == 1 && bn == 64 && L->slots != 2) L->nmain = 3;       // the one-accumulator 64-wide kernel exists with two staging slots only
-    if (L->halo && (L->nmain != (bn == 64 ? 3 : 1) || L->two_sm != (bn == 128 || L->ws) || L->ring)) {
-        fprintf(stderr, "[detectorch_b200] conv_build: halo layer ended up in an instantiation the halo kernel does not cover\n");
-        return false;
-    }
     return true;
 }
 
@@ -370,7 +265,6 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
     choose_box(W1, H1, B, 256, &wbox, &hbox, &nbox);
     const int bn = 64;
     L->block_n = bn;
-    L->halo = 0;
     const uint64_t row = (uint64_t)Wp * 16;
     if (x4_planes) {
         // x4 holds two fp16 planes [B, Hp, Wp, 4] back to back (hi, lo): same overlapping-stride window, 16 bytes (2 pixels) per step
@@ -378,22 +272,17 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
         const __half* xh = reinterpret_cast<const __half*>(x4);
         const __half* xl = xh + (size_t)B * Hp * Wp * 4;
         const uint64_t rowh = (uint64_t)Wp * 8;
-        // row-parity halo (conv_tcgen05.cuh, HALO == 2): tiles of 8 x 16 pixels of one image, A boxes of 16 + 3 stride-2 row slabs
-        L->halo = (conv_use_halo() && H1 >= 16 && W1 >= 8 && !conv_use_two_sm(64, 0)) ? 2 : 0;
-        if (L->halo) { wbox = 8; hbox = 16; nbox = 1; }
-        const int abox_h = L->halo ? (hbox + 3) * 2 : hbox * 2;
-        if (!make_tmap_4d_f16(&p.tm_a, xh, 32, W1, Hp, B, 16, rowh, rowh * Hp, 32, wbox, abox_h, nbox, 1, 2) ||
-            !make_tmap_4d_f16(&p.tm_a2, xl, 32, W1, Hp, B, 16, rowh, rowh * Hp, 32, wbox, abox_h, nbox, 1, 2))
+        if (!make_tmap_4d_f16(&p.tm_a, xh, 32, W1, Hp, B, 16, rowh, rowh * Hp, 32, wbox, hbox * 2, nbox, 1, 2) ||
+            !make_tmap_4d_f16(&p.tm_a2, xl, 32, W1, Hp, B, 16, rowh, rowh * Hp, 32, wbox, hbox * 2, nbox, 1, 2))
             return false;
         p.a_planes = 1;
-        p.a_halo_bytes = L->halo ? wbox * (hbox + 3) * 64 : 0;
     } else if (!make_tmap_4d(&p.tm_a, x4, 32, W1, Hp, B, 32, row, row * Hp, 32, wbox, hbox * 2, nbox, 1, 2)) return false;
     if (kind == KIND_F16X3) {
-        if (!make_tmap_2d_f16(&p.tm_bhi, w_hi, 224, 64, 224 * 2, 32, bn / 2)) return false;
-        if (!make_tmap_2d_f16(&p.tm_blo, w_lo, 224, 64, 224 * 2, 32, bn / 2)) return false;
+        if (!make_tmap_2d_f16(&p.tm_bhi, w_hi, 224, 64, 224 * 2, 32, bn)) return false;
+        if (!make_tmap_2d_f16(&p.tm_blo, w_lo, 224, 64, 224 * 2, 32, bn)) return false;
     } else {
-        if (!make_tmap_2d(&p.tm_bhi, w_hi, 224, 64, 224 * 4, 32, bn / 2)) return false;
-        if (!make_tmap_2d(&p.tm_blo, w_lo, 224, 64, 224 * 4, 32, bn / 2)) return false;
+        if (!make_tmap_2d(&p.tm_bhi, w_hi, 224, 64, 224 * 4, 32, bn)) return false;
+        if (!make_tmap_2d(&p.tm_blo, w_lo, 224, 64, 224 * 4, 32, bn)) return false;
     }
     L->kind = kind == KIND_F16X3 ? KIND_F16X3 : KIND_TF32X3;
     p.range_flag = range_flag;
@@ -407,12 +296,8 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
     p.wo = W1; p.ho = H1; p.nimg = B; p.cout = 64;
     p.a_tile_bytes = wbox * hbox * nbox * 128;
     p.relu = 1; p.sigmoid_ch = 0; p.res_mode = RES_NONE; p.passes = passes == 1 ? 1 : 3;
-    L->nmain = 3;
-    L->slots = 2;
+    L->nmain = 1;       // K = 7 k-blocks: one main accumulator (see conv_build)
     finish_grid(L, 1);
-    L->ws = L->halo == 2 && conv_ws_mode() >= 1;
-    if (L->ws) L->two_sm = true;
-    if (L->ws && conv_narrow_one_acc()) L->nmain = 1;       // K = 7 k-blocks: one main accumulator (see conv_build)
     return true;
 }
 
@@ -424,12 +309,12 @@ inline bool conv_use_pdl() {
     return v == 1;
 }
 
-template <int BN, int NM, bool TWO, int KIND, int RING = 0, int SLOTS = 1, int HALO = 0, bool WS = false>
+template <int BN, int NM, int KIND>
 inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
-    using Cfg = ConvCfg<BN, NM, TWO, KIND, RING, SLOTS, HALO, WS>;
+    using Cfg = ConvCfg<BN, NM, KIND>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tcgen05_kernel<BN, NM, TWO, KIND, RING, SLOTS, HALO, WS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
@@ -443,63 +328,22 @@ inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, conv_tcgen05_kernel<BN, NM, TWO, KIND, RING, SLOTS, HALO, WS>, prm);
+        return cudaLaunchKernelEx(&cfg, conv_wgmma_kernel<BN, NM, KIND>, prm);
     }
-    conv_tcgen05_kernel<BN, NM, TWO, KIND, RING, SLOTS, HALO, WS><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
+    conv_wgmma_kernel<BN, NM, KIND><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
     return cudaGetLastError();
 }
 
-template <bool TWO, int KIND>
-inline cudaError_t conv_launch_sm(const ConvLayer& L, cudaStream_t stream) {
-    // two staging slots only in the kind::f16 kernels (the engine default): the tf32 kind's stages are 64-96 KB
-    constexpr bool kCan2 = KIND == KIND_F16X3;
-    const bool s2 = kCan2 && L.slots == 2;
-    constexpr int S2 = kCan2 ? 2 : 1;
-    if constexpr (KIND == KIND_F16X3) {
-        if (L.halo) {
-            if constexpr (TWO) {
-                if (L.block_n == 128 && L.halo == 1) return conv_launch_cfg<128, 1, true, KIND_F16X3, 0, 2, 1>(L, stream);
-                if (L.block_n == 64 && L.halo == 1 && L.ws) return conv_launch_cfg<64, 3, true, KIND_F16X3, 0, 2, 1, true>(L, stream);
-                if (L.block_n == 64 && L.halo == 2 && L.ws)
-                    return L.nmain == 1 ? conv_launch_cfg<64, 1, true, KIND_F16X3, 0, 2, 2, true>(L, stream)
-                                        : conv_launch_cfg<64, 3, true, KIND_F16X3, 0, 2, 2, true>(L, stream);
-            } else {
-                if (L.block_n == 64 && L.halo == 1) return conv_launch_cfg<64, 3, false, KIND_F16X3, 0, 2, 1>(L, stream);
-                if (L.block_n == 64 && L.halo == 2) return conv_launch_cfg<64, 3, false, KIND_F16X3, 0, 2, 2>(L, stream);
-            }
-            return cudaErrorInvalidValue;
-        }
-    }
-    switch (L.block_n) {
-        case 64:
-            if constexpr (kCan2) { if (L.nmain == 1 && s2) return conv_launch_cfg<64, 1, TWO, KIND, 0, 2>(L, stream); }
-            return s2 ? conv_launch_cfg<64, 3, TWO, KIND, 0, S2>(L, stream) : conv_launch_cfg<64, 3, TWO, KIND, 0, 1>(L, stream);
-        case 128:
-            if (L.nmain == 3) return s2 ? conv_launch_cfg<128, 3, TWO, KIND, 0, S2>(L, stream) : conv_launch_cfg<128, 3, TWO, KIND, 0, 1>(L, stream);
-            return s2 ? conv_launch_cfg<128, 1, TWO, KIND, 0, S2>(L, stream) : conv_launch_cfg<128, 1, TWO, KIND, 0, 1>(L, stream);
-        case 256:
-            if (L.nmain == 0) {
-                if constexpr (TWO && KIND == KIND_F16X3) {
-                    if (L.ring) {
-                        // residual prefetch ring: 2 tiles in flight per epilogue group with two staging slots (3 with one slot);
-                        // ring 3 + 2 slots (possible with 32 KB stages) measured 8-11 % slower than ring 2 + 2 slots
-                        if (!s2) return L.ring == 2 ? conv_launch_cfg<256, 0, TWO, KIND, 2, 1>(L, stream) : conv_launch_cfg<256, 0, TWO, KIND, 3, 1>(L, stream);
-                        return conv_launch_cfg<256, 0, TWO, KIND, 2, 2>(L, stream);
-                    }
-                    if (s2) return conv_launch_cfg<256, 0, TWO, KIND, 0, 2>(L, stream);
-                }
-                return conv_launch_cfg<256, 0, TWO, KIND, 0, 1>(L, stream);
-            }
-            if constexpr (TWO && KIND == KIND_F16X3) { if (s2) return conv_launch_cfg<256, 1, TWO, KIND, 0, 2>(L, stream); }
-            return conv_launch_cfg<256, 1, TWO, KIND>(L, stream);
-        default: return cudaErrorInvalidValue;
-    }
+template <int KIND>
+inline cudaError_t conv_launch_kind(const ConvLayer& L, cudaStream_t stream) {
+    if (L.block_n == 64) return L.nmain == 3 ? conv_launch_cfg<64, 3, KIND>(L, stream) : conv_launch_cfg<64, 1, KIND>(L, stream);
+    if (L.block_n == 128 && L.nmain == 1) return conv_launch_cfg<128, 1, KIND>(L, stream);
+    return cudaErrorInvalidValue;
 }
 
 inline cudaError_t conv_launch(const ConvLayer& L, cudaStream_t stream) {
     if (!L.valid) return cudaErrorInvalidValue;
-    if (L.kind == KIND_F16X3) return L.two_sm ? conv_launch_sm<true, KIND_F16X3>(L, stream) : conv_launch_sm<false, KIND_F16X3>(L, stream);
-    return L.two_sm ? conv_launch_sm<true, KIND_TF32X3>(L, stream) : conv_launch_sm<false, KIND_TF32X3>(L, stream);
+    return L.kind == KIND_F16X3 ? conv_launch_kind<KIND_F16X3>(L, stream) : conv_launch_kind<KIND_TF32X3>(L, stream);
 }
 
 }  // namespace dt

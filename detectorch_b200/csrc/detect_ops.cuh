@@ -961,7 +961,7 @@ static __global__ void __launch_bounds__(256) det_class_kernel(const __grid_cons
 // grid B, 1024 threads: limit to max_dets over all classes (result_utils.py:152-168) and emit.
 // The kept flags of a class are swept by ONE WARP (ballot + popc over 32 RoIs at a time, no block barriers): class counts -> exclusive
 // class offsets -> ordered writes.  Two such sweeps (gather keys, emit) replace two block-wide scans of the NC*R flags (79 iterations x 3
-// __syncthreads each in round 1: 148 us at batch 8).  Order and arithmetic are unchanged: class-major, ascending RoI index.
+// __syncthreads each).  Order and arithmetic are unchanged: class-major, ascending RoI index.
 static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_constant__ DetParams P) {
     __shared__ uint32_t hist[32 * 256];
     __shared__ int cls_cnt[128], cls_off[129];

@@ -254,10 +254,6 @@ __device__ __forceinline__ AxisBin axis_bin2(float start, int p, float bin, int 
 
 static constexpr int kMaxPooled = 16;     // pooled_height / pooled_width supported by the fast path (7 and 14 in practice)
 
-// Measured and rejected (round 2, profiles/r02_summary.md): requesting 2 tap rows x 4 tap columns before the first FMA (8 loads in flight, 61
-// registers, 4 CTAs/SM) made the box-head launch 447 -> 510 us and the mask launch 200 -> 237 us, like round 1's fully unrolled 4x4 variant:
-// the kernel is bound by what the L2 delivers to the SMs (ncu: 1.1 GB DRAM read + 0.75 GB written by the two launches, 2.9 TB/s), not by
-// loads in flight per thread; the plain loop with 8 resident CTAs per SM stays.
 // NHWC features (multi-level), out [R, PH, PW, C]; one CTA per RoI (grid-stride), threads over (bin, 4-channel group)
 static __global__ void __launch_bounds__(256) roi_align_fast_nhwc_kernel(RoiLevels lv, const float* __restrict__ rois, const int* __restrict__ level,
                                                                          int max_rois, int C, int PH, int PW, float* __restrict__ out) {

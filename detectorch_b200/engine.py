@@ -136,7 +136,7 @@ class Engine:
         cfg.num_classes, cfg.score_thresh, cfg.det_nms_thresh = num_classes, score_thresh, det_nms_thresh
         cfg.max_dets, cfg.det_cap = max_dets, det_cap
         cfg.use_mask, cfg.output_prob, cfg.emit_full_masks, cfg.passes = int(use_mask), int(output_prob), int(emit_full_masks), passes
-        cfg.precise_mask = int(precise_mask)          # 1/True = K-split mask convs, 2 = 128-wide rotating accumulators, 0 = plain
+        cfg.precise_mask = int(precise_mask)          # 1/True = K-split mask convs, 2 = 64-wide tiles with 3 rotating accumulators, 0 = plain
         cfg.stem_im2col = int(stem_im2col)
         cfg.exact_roialign = int(exact_roialign)
         cfg.model_type = 1 if model == "c4" else 0

@@ -1,7 +1,7 @@
 """Drop-in mirror of the reference model API (lib/model/detector.py:130-286): same constructor
 kwargs, same forward signature / return tuple, same attribute names (`model`, `conv_body`,
 `conv_head`, `rpn`, `bbox_head`, `classif_head`, `mask_head`), same state_dict names and the same
-Detectron-pkl loader entry point -- but forward() runs the fused sm_100a engine
+Detectron-pkl loader entry point -- but forward() runs the fused sm_90a engine
 (detectorch_b200/csrc/capi_engine.cu) instead of torch.nn ops + host numpy.
 
 The torch modules below are PARAMETER CONTAINERS ONLY (so state_dict()/load_state_dict()/the pkl

@@ -1,5 +1,5 @@
 """Drop-in mirror of the reference op wrapper lib/model/roi_align.py (RoIAlignFunction :23-145,
-RoIAlign :150-169, preprocess_rois :172-188) over the sm_100a kernel.  Same names, argument order
+RoIAlign :150-169, preprocess_rois :172-188) over the sm_90a kernel.  Same names, argument order
 and error behaviour; CUDA only (the reference's CPU branch is the parity oracle, not a product path)."""
 import os
 

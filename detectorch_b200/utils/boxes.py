@@ -1,5 +1,5 @@
 """Mirror of the hot-path part of the reference lib/utils/boxes.py: nms (:332-336) backed by the
-sm_100a NMS kernel, numpy in / numpy out like the reference."""
+sm_90a NMS kernel, numpy in / numpy out like the reference."""
 import numpy as np
 import torch
 

@@ -1,5 +1,5 @@
 /*
- * detectorch_b200 -- C ABI of the B200-native two-stage-detector inference hot path.
+ * detectorch_b200 -- C ABI of the H100-native two-stage-detector inference hot path.
  *
  * Plain pointers and sizes only (no torch types).  Every pointer is a DEVICE pointer unless
  * stated otherwise; every call is asynchronous on `stream` (a cudaStream_t passed as void*),
@@ -128,7 +128,7 @@ int dt_prep_image(const uint8_t* image_hwc, int height, int width, const double*
                   float* blob_chw, int blob_height, int blob_width, dt_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Convolution / GEMM on tcgen05 tensor cores (3xTF32, fp32-accurate), NHWC activations.
+ * Convolution / GEMM on wgmma tensor cores (3xTF32 or 3xFP16, fp32-accurate), NHWC activations.
  * Replaces the torch.nn.Conv2d / Linear / ConvTranspose2d calls of lib/model/detector.py
  * (:17-27 FPN, :58-59 FC6/FC7, :71-74 mask convs, :89-90 deconv + mask logits, :119-121 RPN, :170-183 trunk).
  *   x        [N,H,W,Cin]   (Cin % 32 == 0), x_pix_stride floats between pixels
@@ -136,8 +136,8 @@ int dt_prep_image(const uint8_t* image_hwc, int height, int width, const double*
  *   y        [N,Ho,Wo,Cout] (Cout % 4 == 0), y = act( conv(x,w)*scale[c] + shift[c] (+ residual) )
  *   res_mode 0 none | 1 residual [N,Ho,Wo,Cout] | 2 nearest-2x-upsampled up_src [N,up_h,up_w,Cout]
  *   relu     0/1 ; sigmoid_ch: channels [0,sigmoid_ch) get a sigmoid ; passes 3 (3xTF32) or 1 (TF32)
- *   force_block_n 0 = auto | 64 | 128 | 256 | -1 = 128 with 3 rotating accumulators (shortest truncating-accumulate chains)
- * dt_conv2d_nhwc_f16x3 is the same product on the kind::f16 pipe (twice the tf32 issue rate): w_hi16 / w_lo16 are the fp16 halves of
+ *   force_block_n 0 = auto | 64 | 128 (256 runs as 128-wide tiles) | -1 = 64 with 3 rotating accumulators (shortest truncating-accumulate chains)
+ * dt_conv2d_nhwc_f16x3 is the same product with fp16 MMAs (twice the tf32 rate): w_hi16 / w_lo16 are the fp16 halves of
  * w * multiplier from dt_fp16_split (multiplier a power of two that keeps the low half a normal fp16 number; the caller folds
  * 1/multiplier into `scale`); the fp32 activations are split in shared memory.  *range_flag (device int, may be NULL) is set
  * to 1 if an activation does not fit fp16 (|x| >= 65504); the result is then not meaningful and the tf32 entry must be used.
@@ -158,7 +158,7 @@ int dt_conv2d_nhwc(const float* x, int N, int H, int W, int Cin, int x_pix_strid
  * Fused Mask R-CNN (ResNet-50/101 + FPN) inference engine: the whole of
  *   lib/model/detector.py:233-286 (detector.forward), lib/utils/result_utils.py:76-168
  *   (postprocess_output) and lib/model/detector.py:99-112 (mask_head.forward)
- * as one static, sync-free program of sm_100a kernels.  The caller owns two flat device buffers
+ * as one static, sync-free program of sm_90a kernels.  The caller owns two flat device buffers
  * (weights, workspace); named intermediate / output tensors are exposed as (offset, shape) into the
  * workspace so the host language wraps them without copies.
  */

@@ -1,6 +1,6 @@
 """`cppcuda_cffi.roialign` with the reference's cffi calling convention (caller allocates and zeroes `output`,
 lib/cppcuda_cffi/src/roi_align_forward_cuda.h:1-7) so that the UNMODIFIED reference lib/model/roi_align.py
-(which imports this module on torch != 0.4, roi_align.py:20) runs on the sm_100a kernel."""
+(which imports this module on torch != 0.4, roi_align.py:20) runs on the sm_90a kernel."""
 import ctypes
 import os
 import sys

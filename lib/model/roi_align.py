@@ -1,4 +1,4 @@
-"""Overlay of lib/model/roi_align.py: RoIAlignFunction / RoIAlign / preprocess_rois over the sm_100a kernel."""
+"""Overlay of lib/model/roi_align.py: RoIAlignFunction / RoIAlign / preprocess_rois over the sm_90a kernel."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))

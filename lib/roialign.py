@@ -1,7 +1,7 @@
 """The reference's torch-0.4 flavour of the native op: a module named `roialign` with the pybind11 entry points of
 lib/cppcuda/roi_align_binding.cpp:7-12 / roi_align_cuda.h:4-22 (JIT-loaded by lib/model/roi_align.py:11-18 when torch is 0.4) --
 callee-allocates convention, argument order and AT_CHECK conditions (-> RuntimeError) as in
-lib/cppcuda/roi_align_forward_cuda.cu:162-212 and roi_align_backward_cuda.cu:210-260, over the sm_100a kernels."""
+lib/cppcuda/roi_align_forward_cuda.cu:162-212 and roi_align_backward_cuda.cu:210-260, over the sm_90a kernels."""
 import os
 import sys
 

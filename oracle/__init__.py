@@ -4,8 +4,8 @@ import os
 
 def usable_cpus():
     """Host threads this process may really use: the scheduler affinity mask, capped by the cgroup CPU quota (cpu.max) when there is one.
-    os.cpu_count() alone counts every core of the machine, and a torch thread pool of that size inside a smaller cgroup quota runs an
-    order of magnitude slower than a right-sized one (the 12x swing of the round-1 cpu_baseline)."""
+    os.cpu_count() alone counts every core of the machine, and a torch thread pool of that size inside a smaller cgroup quota
+    oversubscribes the cores it may use."""
     try:
         n = len(os.sched_getaffinity(0))
     except Exception:

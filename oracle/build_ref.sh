@@ -1,13 +1,13 @@
 #!/usr/bin/env bash
 # Builds the REFERENCE's own sources for the hot path, from where they lie under
-# /root/reference (read-only), into oracle/_ref/ (git-ignored, travels to the GPU box).
+# $REF (read-only), into oracle/_ref/ (git-ignored).
 # No reference source is copied into the repo: the Cython NMS needs a 2-token numpy-2
 # patch (np.int_t -> np.intp_t, np.int -> np.intp; SURVEY.md 8c), which is applied by
 # sed into a temp dir at build time.
 #   _ref/libroialign_ref.so       <- lib/cppcuda_cffi/src/cpp/roi_align_cpu_loop.cpp   (CPU loop)
 #   _ref/libroialign_ref_cuda.so  <- lib/cppcuda_cffi/src/cuda/roi_align_forward_cuda_kernel.cu
-#                                     (the reference CUDA kernel, compiled unmodified for sm_100a:
-#                                      the on-box "kernel to beat")
+#                                     (the reference CUDA kernel, compiled unmodified for sm_90a:
+#                                      the kernel to beat)
 #   _ref/cython_nms*.so           <- lib/utils_cython/cython_nms.pyx (patched as above)
 #   _ref/libroialign_bwd_ref.so   <- lib/cppcuda/roi_align_backward_cpu.cpp: the file is ATen-0.4 flavoured and does not compile against
 #                                     torch 2.x, but its templates bilinear_interpolate_gradient / add / roi_align_backward_loop
@@ -26,7 +26,7 @@ if [ ! -d "$REF/lib" ]; then echo "build_ref: $REF not present (GPU box) - using
 mkdir -p "$OUT"
 g++ -O2 -fPIC -shared -o "$OUT/libroialign_ref.so" "$REF/lib/cppcuda_cffi/src/cpp/roi_align_cpu_loop.cpp"
 if command -v nvcc >/dev/null; then
-  nvcc -O3 -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC -shared \
+  nvcc -O3 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -shared \
        -o "$OUT/libroialign_ref_cuda.so" "$REF/lib/cppcuda_cffi/src/cuda/roi_align_forward_cuda_kernel.cu"
 fi
 TMPB=$(mktemp -d)

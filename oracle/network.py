@@ -4,7 +4,7 @@ ORACLE -- test infrastructure only (never imported by detectorch_b200/).
 Torch-CPU fp32 restatement of the reference detector graph, written functionally
 over a flat {reference-parameter-name: tensor} dict so that the same weights load
 into the reference `detector` (state_dict names), into this oracle, and into the
-B200 engine.
+H100 engine.
 
   trunk (torchvision Bottleneck, stride on conv1 of layer{2,3,4}[0])   detector.py:170-183
   BN in eval mode with running stats (0,1): y = x*g/sqrt(1+1e-5) + b     detector.py:231,301

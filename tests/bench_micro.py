@@ -1,6 +1,6 @@
-"""RoIAlign + NMS microbench (BASELINE.json configs[4]): 100k boxes x 256-ch 50x68 feature map on 1 B200,
+"""RoIAlign + NMS microbench (BASELINE.json configs[4]): 100k boxes x 256-ch 50x68 feature map on 1 H100,
 achieved HBM GB/s vs the measured roofline, next to the reference's own CUDA kernel (compiled unmodified for
-sm_100a into oracle/_ref/libroialign_ref_cuda.so) and the reference's CPU loop / Cython NMS on a bounded sample.
+sm_90a into oracle/_ref/libroialign_ref_cuda.so) and the reference's CPU loop / Cython NMS on a bounded sample.
 
   python tests/bench_micro.py            -> one JSON line per measurement
 """

@@ -1,5 +1,5 @@
-"""One engine run under the kernel switches of the calling environment (DT_CONV_HALO, DT_CONV_WS, DT_CONV_SLOTS, DT_CONV_NARROW1,
-DT_PLANE_HANDOVER, DT_CONV_PDL, DT_CONV_MMA ...: they are read once per process), compared with the oracle: prints one JSON line with the
+"""One engine run under the kernel switches of the calling environment (DT_CONV_KIND, DT_PLANE_HANDOVER, DT_CONV_PDL, DT_RPN_SPLIT,
+DT_RPN_NMS_SPLIT: they are read once per process), compared with the oracle: prints one JSON line with the
 worst relative error over C2..C5 / P2..P6, the worst absolute error of the RPN maps and of the teacher-forced mask logits.
 Run by tests/test_gpu_engine.py::test_conv_kernel_variants in a subprocess per setting."""
 import json

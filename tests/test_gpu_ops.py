@@ -262,7 +262,7 @@ def test_nms_large_properties(dev):
     assert again.numel() == keep.numel()
 
 
-# ------------------------------------------------------------------------------- conv / GEMM (tcgen05, 3xTF32)
+# ------------------------------------------------------------------------------- conv / GEMM (wgmma, 3xTF32 / 3xFP16)
 def _conv_case(dev, N, Hh, Ww, Cin, Cout, k, pad, stride, res=False, up=False, relu=False, sig=0, passes=3, kind="tf32", force_block_n=0):
     from detectorch_b200 import ops
     g = torch.Generator().manual_seed(N * 1000 + Hh * 10 + Cin + Cout + k)
@@ -314,9 +314,9 @@ def test_conv_f16_epilogues_tiles_and_range_flag(dev):
     assert _conv_case(dev, 2, 13, 19, 128, 64, 3, 1, 1, res=True, relu=True, kind="f16") < 1e-4
     assert _conv_case(dev, 1, 26, 38, 64, 256, 1, 0, 1, up=True, kind="f16") < 1e-4
     assert _conv_case(dev, 1, 25, 38, 256, 16, 1, 0, 1, sig=3, kind="f16") < 1e-4
-    assert _conv_case(dev, 5, 14, 14, 256, 256, 3, 1, 1, kind="f16", force_block_n=-1) < 1e-4      # precise 128-wide tile
+    assert _conv_case(dev, 5, 14, 14, 256, 256, 3, 1, 1, kind="f16", force_block_n=-1) < 1e-4      # precise tile (3 rotating accumulators)
     assert _conv_case(dev, 5, 14, 14, 256, 256, 3, 1, 1, kind="f16", force_block_n=128) < 1e-4
-    assert _conv_case(dev, 1, 1, 512, 2048, 256, 1, 0, 1, kind="f16") < 1e-4                         # K = 2048: cta_group::2 variant
+    assert _conv_case(dev, 1, 1, 512, 2048, 256, 1, 0, 1, kind="f16") < 1e-4                         # K = 2048
     assert 1e-5 < _conv_case(dev, 1, 1, 256, 1024, 128, 1, 0, 1, passes=1, kind="f16") < 5e-3       # single fp16 pass: not fp32-accurate
     # fp16 has a 5-bit exponent: an activation of 1e5 raises the range flag, ordinary data does not
     x = torch.randn((1, 4, 32, 64), device=dev)
@@ -328,24 +328,6 @@ def test_conv_f16_epilogues_tiles_and_range_flag(dev):
     x[0, 1, 7, 3] = 1.0e5
     ops.conv2d_nhwc(x, w, one, zero, 1, 1, 0, 1, kind="f16", range_flag=flag)
     assert int(flag.item()) == 1
-
-
-def test_conv_both_mma_modes(built):
-    """The 1-SM (multicast) and 2-SM (cta_group::2) variants of the conv kernel are both exercised over every tile
-    configuration in fresh processes (the mode is latched per process from DT_CONV_MMA)."""
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for mode in ("1sm", "2sm"):
-        env = dict(os.environ, DT_CONV_MMA=mode)
-        out = subprocess.run([sys.executable, os.path.join(root, "tests", "gpu_probe.py"), "conv_basic", "conv_spatial", "conv_epilogue"],
-                             env=env, capture_output=True, text=True, timeout=600)
-        assert out.returncode == 0, out.stderr[-2000:]
-        lines = [l for l in out.stdout.splitlines() if l.startswith("CONV")]
-        assert len(lines) == 17
-        for l in lines:
-            rel = float(l.split(" rel ")[1].split()[0])
-            assert rel < (5e-3 if "passes1" in l else 1e-4), (mode, l)
 
 
 def test_conv_epilogues(dev):

@@ -1,4 +1,4 @@
-"""CPU tests of the host side: the C-ABI library builds for sm_100a without a GPU, loads, and exports
+"""CPU tests of the host side: the C-ABI library builds for sm_90a without a GPU, loads, and exports
 every symbol include/detectorch_b200.h declares; the engine's parameter table equals the reference's
 state_dict names; the product path refuses to run without CUDA (no CPU fallback)."""
 import ctypes
@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol(built):
     assert "dt_segm_rle" in names and "dt_prep_image" in names and "dt_conv2d_nhwc_f16x3" in names and len(names) >= 33
     for n in names:
         assert hasattr(L, n), "library does not export %s" % n
-    assert b"sm_100a" in _lib.lib().dt_version()
+    assert b"sm_90a" in _lib.lib().dt_version()
 
 
 def test_ctypes_signatures_cover_operator_api(built):

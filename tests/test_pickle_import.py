@@ -2,86 +2,44 @@
 reference's own blob names loads identically into the reference detector and into the detectorch_b200 mirror, for the
 constructor kwargs of every eval_*.ipynb notebook (Fast / Faster / Mask R-CNN on the C4 and on the FPN body: the loader
 branches on use_rpn_head / use_fpn_body / mask_head_type / two_layer_mlp exactly like detector.py:317-374).
-Needs the reference tree (its utils.utils.parse_th_to_caffe2 name mapping), so it is skipped on the GPU box."""
+The reference side (its utils.utils.parse_th_to_caffe2 name mapping, its detector's trunk keys, and what its loader read from the
+pickle) is stored in tests/golden/ref_golden.npz by tests/golden/make_ref_golden.py."""
 import os
-import pickle
 
 import numpy as np
 import pytest
 import torch
 
+import ref_cases as rc
 from oracle import network as net
-from oracle import reference_shim as rs
 
-FPN = dict(arch='resnet50', conv_body_layers=['conv1', 'bn1', 'relu', 'maxpool', 'layer1', 'layer2', 'layer3', 'layer4'],
-           conv_head_layers='two_layer_mlp', fpn_layers=['layer1', 'layer2', 'layer3', 'layer4'],
-           roi_height=7, roi_width=7, roi_spatial_scale=[0.25, 0.125, 0.0625, 0.03125], roi_sampling_ratio=2)
-# name -> (constructor kwargs as the notebook passes them, oracle parameter-set flags)
-CONFIGS = {
-    "eval_fast": (dict(arch='resnet50'), dict(fpn=False, rpn=False, mask=False)),
-    "eval_faster": (dict(arch='resnet50', use_rpn_head=True), dict(fpn=False, rpn=True, mask=False)),
-    "eval_mask": (dict(arch='resnet50', use_rpn_head=True, use_mask_head=True), dict(fpn=False, rpn=True, mask=True)),
-    "eval_fast_FPN": (dict(FPN), dict(fpn=True, rpn=False, mask=False)),
-    "eval_faster_FPN": (dict(FPN, fpn_extra_lvl=True, use_rpn_head=True), dict(fpn=True, rpn=True, mask=False)),
-    "eval_mask_FPN": (dict(FPN, fpn_extra_lvl=True, use_rpn_head=True, use_mask_head=True, mask_head_type='1up4convs'), dict(fpn=True, rpn=True, mask=True)),
-}
+GOLD = os.path.join(os.path.dirname(__file__), "golden", "ref_golden.npz")
 
 
-def write_detectron_pickle(path, ref_model, P, flags):
-    """A pickle in the published checkpoints' format ({'blobs': {caffe2 name: ndarray}}), filled from the flat parameter dict P."""
-    from utils.utils import parse_th_to_caffe2
-    blobs = {}
-    for k in ref_model.model.state_dict().keys():                            # trunk: torchvision name -> caffe2 blob name
-        if 'running' in k or 'fc' in k:
-            continue
-        if 'num_batches' in k:
-            # torch >= 0.4.1 adds this buffer; the reference's loader (detector.py:300-304) does not skip it, so a blob must exist
-            blobs[parse_th_to_caffe2(k.split('.'))] = np.zeros((), np.float32)
-            continue
-        w = P["model." + k].numpy()
-        blobs[parse_th_to_caffe2(k.split('.'))] = w[:, (2, 1, 0), :, :].copy() if k == 'conv1.weight' else w     # pickles hold BGR
-
-    def put(wn, bn, name):
-        blobs[wn], blobs[bn] = P[name + ".weight"].numpy(), P[name + ".bias"].numpy()
-    put('bbox_pred_w', 'bbox_pred_b', 'bbox_head'); put('cls_score_w', 'cls_score_b', 'classif_head')
-    if flags["rpn"]:
-        sfx = '_fpn2' if flags["fpn"] else ''
-        put('conv_rpn%s_w' % sfx, 'conv_rpn%s_b' % sfx, 'rpn.conv_rpn')
-        put('rpn_cls_logits%s_w' % sfx, 'rpn_cls_logits%s_b' % sfx, 'rpn.rpn_cls_prob')
-        put('rpn_bbox_pred%s_w' % sfx, 'rpn_bbox_pred%s_b' % sfx, 'rpn.rpn_bbox_pred')
-    if flags["mask"]:
-        put('conv5_mask_w', 'conv5_mask_b', 'mask_head.transposed_conv'); put('mask_fcn_logits_w', 'mask_fcn_logits_b', 'mask_head.classif_logits')
-        if flags["fpn"]:
-            for i in range(1, 5):
-                put('_[mask]_fcn%d_w' % i, '_[mask]_fcn%d_b' % i, 'mask_head.conv_head.fcn%d' % i)
-    if flags["fpn"]:
-        for i, l in enumerate(FPN['fpn_layers']):
-            kc = parse_th_to_caffe2((l + '.' + list(getattr(ref_model.model, l).state_dict().keys())[-1]).split('.'))
-            kc = kc[:kc.rfind("_")]
-            suffix = '_sum_lateral' if i < 3 else '_sum'
-            put('fpn_inner_' + kc + suffix + '_w', 'fpn_inner_' + kc + suffix + '_b', 'conv_body.fpn_lateral.%d' % i)
-            put('fpn_' + kc + '_sum_w', 'fpn_' + kc + '_sum_b', 'conv_body.fpn_output.%d' % i)
-        put('fc6_w', 'fc6_b', 'conv_head.fc6'); put('fc7_w', 'fc7_b', 'conv_head.fc7')
-    with open(path, "wb") as f:
-        pickle.dump({'blobs': blobs}, f, protocol=2)
+@pytest.fixture(scope="module")
+def G():
+    return np.load(GOLD)
 
 
-@pytest.mark.skipif(not rs.available(), reason="reference tree not present")
-@pytest.mark.parametrize("name", sorted(CONFIGS))
-def test_detectron_pickle_loads_like_the_reference(tmp_path, built, name):
-    rs.install()
-    from model.detector import detector as ref_detector                 # the reference
+@pytest.mark.parametrize("name", sorted(rc.CONFIGS))
+def test_detectron_pickle_loads_like_the_reference(tmp_path, built, G, name):
     from detectorch_b200.model.detector import detector as b200_detector
-    kw, flags = CONFIGS[name]
+    kw, flags = rc.CONFIGS[name]
     P = net.synthetic_params("resnet50", **flags)
-    ref_kw = dict(kw, roi_feature_channels=1024) if flags["fpn"] else kw   # the FPN notebooks rely on the pickle to resize the 2048-wide default heads
+    trunk = [str(k) for k in G["pkl_%s_trunk" % name]]
+    layout = {"trunk": trunk, "c2": dict(zip(trunk, [str(c) for c in G["pkl_%s_trunk_c2" % name]])), "fpn": [str(c) for c in G["pkl_%s_fpn" % name]]}
     pkl = os.path.join(str(tmp_path), "model_final.pkl")
-    write_detectron_pickle(pkl, ref_detector(**ref_kw), P, flags)
-    ref = ref_detector(detector_pkl_file=pkl, **kw)                     # exactly the notebook's cell 7
-    mine = b200_detector(detector_pkl_file=pkl, **kw)
-    sr, sm = ref.state_dict(), mine.state_dict()
-    for k, v in P.items():
-        assert torch.equal(sr[k], v), "reference loader: " + k           # the synthetic pickle round-trips through the reference
+    rc.write_detectron_pickle(pkl, layout, P, flags)
+    mine = b200_detector(detector_pkl_file=pkl, **kw)                   # exactly the notebook's cell 7
+    sm = mine.state_dict()
+    # the reference loader read the same pickle into exactly these parameters (names, shapes, bit-pattern sums, leading values)
+    keys = [str(k) for k in G["pkl_%s_keys" % name]]
+    assert keys == sorted(P)
+    for i, k in enumerate(keys):
+        v = P[k]
+        assert list(G["pkl_%s_shapes" % name][i][:v.dim()]) == list(v.shape), "reference loader: " + k
+        assert int(G["pkl_%s_bitsums" % name][i]) == rc.bitsum(v), "reference loader: " + k
+        assert np.array_equal(G["pkl_%s_head" % name][i], rc.head8(v), equal_nan=True), "reference loader: " + k
         assert torch.equal(sm[k], v), "mirror loader: " + k
     # and the engine's parameter table accepts exactly these names
     from detectorch_b200 import engine
@@ -89,15 +47,12 @@ def test_detectron_pickle_loads_like_the_reference(tmp_path, built, name):
     assert set(t) == set(P) and all(t[k] == int(np.prod(P[k].shape)) for k in P)
 
 
-@pytest.mark.skipif(not rs.available(), reason="reference tree not present")
-def test_caffe2_blob_names_match_the_reference_helper():
+def test_caffe2_blob_names_match_the_reference_helper(G):
     """The mirror's own torchvision-name -> caffe2-blob-name mapping equals utils/utils.py:44-71 (parse_th_to_caffe2) on every trunk key."""
-    rs.install()
     import torchvision.models as models
-    from utils.utils import parse_th_to_caffe2
     from detectorch_b200.model.detector import caffe2_blob_name
     for arch in ("resnet50", "resnet101"):
         keys = [k for k in getattr(models, arch)().state_dict().keys() if not ('running' in k or 'fc' in k or 'num_batches' in k)]
-        assert len(keys) > 150
-        for k in keys:
-            assert caffe2_blob_name(k) == parse_th_to_caffe2(k.split('.')), k
+        assert len(keys) > 150 and keys == [str(k) for k in G["name_%s_th" % arch]]
+        for k, want in zip(keys, G["name_%s_c2" % arch]):
+            assert caffe2_blob_name(k) == str(want), k

@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# pre-commit gate used during development: the library must build for sm_100a and the CPU suite must pass
+# pre-commit check: the library must build for sm_90a and the CPU suite must pass
 set -e
 cd "$(dirname "$0")/.."
 python -m detectorch_b200.build --force > /dev/null
