@@ -16,10 +16,12 @@
 //                written next to the A tile by the MMA warpgroups, B_l is precomputed once per weight tensor.
 //   KIND_F16X3 (the engine default, twice the tf32 rate): A_h = fp16(A), A_l = fp16(A - A_h) (22 mantissa bits, like the two tf32
 //                pieces); B_h / B_l likewise, precomputed and pre-scaled by a power of two so that B_l stays a normal fp16 number
-//                (the epilogue scale undoes it exactly).  The fp32 A tile arrives by TMA and each MMA warpgroup splits its own 64 rows
-//                into two 64-byte-row (SWIZZLE_64B) fp16 tiles -- unless the producing layer already wrote the activation as two fp16
-//                planes (a_planes / out_planes), in which case TMA delivers the operand tiles directly.  fp16 has a 5-bit exponent:
-//                |A| >= 65504 raises a device flag (the engine then reports it; the tf32 kind has no such limit).
+//                (the epilogue scale undoes it exactly).  A is a register operand of the wgmma: the fp32 A tile arrives by TMA and each
+//                MMA warpgroup loads its own 64 rows straight into m64k16 fragments and splits them into A_h / A_l in registers -- or,
+//                when the producing layer already wrote the activation as two fp16 planes (a_planes / out_planes), TMA delivers two
+//                64-byte-row (SWIZZLE_64B) fp16 tiles and ldmatrix loads the fragments.  Only B is read by the tensor core from shared
+//                memory.  fp16 has a 5-bit exponent: |A| >= 65504 raises a device flag (the engine then reports it; the tf32 kind has
+//                no such limit).
 // `passes` == 1 runs the plain single-pass product (speed-of-light reference; not fp32-accurate).
 //
 // Tile: BLOCK_M = 128 output pixels (a wbox x hbox x nbox box of the NHWC output, so the same TMA box geometry loads A for any
@@ -31,7 +33,8 @@
 //   warpgroup 0    TMA producer (one thread; the warpgroup gives its registers up to the MMA warpgroups)
 //   warpgroups 1-2 MMA + epilogue, rows [0, 64) and [64, 128) of the tile: operand split, wgmma, then scale/shift [+residual]
 //                  [ReLU|sigmoid] -> swizzled staging area -> TMA store.  The producer runs ahead into the next tile while a tile
-//                  drains, and the stores of a tile overlap the main loop of the next.
+//                  drains, and the stores of a tile overlap the main loop of the next.  A RES_TILE layer loads the residual tile into the
+//                  staging area during the main loop, as soon as the previous tile's stores have read it.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -82,8 +85,9 @@ struct ConvCfg {
     static constexpr int A_BYTES = BLOCK_M * 128;                     // 16 KB: the fp32 A tile as TMA delivers it
     static constexpr int B_ROW_BYTES = KIND == KIND_F16X3 ? 64 : 128; // 32 k-elements per row
     static constexpr int B_BYTES = BLOCK_N * B_ROW_BYTES;
-    // tf32: A | A_lo (16 KB each); f16: A (fp32 as delivered) | A_h | A_l (8 KB each; with a_planes TMA fills A_h | A_l).  Then B_h | B_l.
-    static constexpr int A_STAGE_BYTES = 2 * A_BYTES;
+    // tf32: A | A_lo (16 KB each); f16: A (16 KB: the fp32 tile as delivered, or with a_planes the fp16 planes A_h | A_l, 8 KB each).
+    // Then B_h | B_l.  f16 stages are 32 KB at BLOCK_N = 128 (5 stages) and 24 KB at BLOCK_N = 64 (6).
+    static constexpr int A_STAGE_BYTES = KIND == KIND_F16X3 ? A_BYTES : 2 * A_BYTES;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + 2 * B_BYTES;
     // epilogue staging: one 16 KB swizzled 128 x 32-channel chunk per 32 output channels (the layout of a tm_d box)
     static constexpr int NCHUNK = BLOCK_N / 32;
@@ -100,15 +104,30 @@ struct ConvCfg {
     static constexpr int KSTEPS = KIND == KIND_F16X3 ? 2 : 4;         // instructions per 32-element k-block (32 bytes of a row each)
     static_assert(SMEM_BYTES <= SMEM_LIMIT, "exceeds the 227 KB shared-memory limit");
     static_assert(8 * NUM_BARS <= 256, "barrier area");
+    static_assert(STAGE_BYTES % 1024 == 0, "stages start on a SWIZZLE_128B atom");
 };
 
-template <int BLOCK_N, int KIND>
-__device__ __forceinline__ void conv_mma(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db) {
-    if constexpr (KIND == KIND_F16X3) {
-        if constexpr (BLOCK_N == 64) wgmma_f16_n64(d, da, db, 1u); else wgmma_f16_n128(d, da, db, 1u);
-    } else {
-        if constexpr (BLOCK_N == 64) wgmma_tf32_n64(d, da, db, 1u); else wgmma_tf32_n128(d, da, db, 1u);
-    }
+// tf32: A and B from shared memory
+template <int BLOCK_N>
+__device__ __forceinline__ void conv_mma_tf32(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db) {
+    if constexpr (BLOCK_N == 64) wgmma_tf32_n64(d, da, db, 1u); else wgmma_tf32_n128(d, da, db, 1u);
+}
+// f16: A from registers, B from shared memory
+template <int BLOCK_N>
+__device__ __forceinline__ void conv_mma_f16(float (&d)[BLOCK_N / 2], const uint32_t (&a)[4], uint64_t db) {
+    if constexpr (BLOCK_N == 64) wgmma_f16_rs_n64(d, a, db, 1u); else wgmma_f16_rs_n128(d, a, db, 1u);
+}
+
+template <int I>
+struct IntC { static constexpr int value = I; };
+
+// (hi, lo) = (fp16(x), fp16(x - hi)) for two consecutive k elements, packed as fragment registers (the lower k in the low half)
+__device__ __forceinline__ void split_f16x2(float2 v, uint32_t& hi, uint32_t& lo) {
+    const __half2 h = __float22half2_rn(v);
+    const float2 hf = __half22float2(h);
+    const __half2 l = __float22half2_rn(make_float2(v.x - hf.x, v.y - hf.y));
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
 template <int BLOCK_N, int NMAIN, int KIND>
@@ -186,9 +205,9 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
                     const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
                     mbar_arrive_expect_tx(bar_full(s), tx_bytes);
                     if (KIND == KIND_F16X3 && p.a_planes) {
-                        // fp16 planes: the two operand tiles land where the split would have written them
-                        tma_load_4d(st + Cfg::A_BYTES, &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
-                        tma_load_4d(st + Cfg::A_BYTES + Cfg::A_BYTES / 2, &p.tm_a2, bar_full(s), cb * 32, xw, xh, n0img);
+                        // fp16 planes: the two operand tiles land where the fp32 tile would have landed
+                        tma_load_4d(st, &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
+                        tma_load_4d(st + Cfg::A_BYTES / 2, &p.tm_a2, bar_full(s), cb * 32, xw, xh, n0img);
                     } else {
                         tma_load_4d(st, &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
                     }
@@ -205,57 +224,131 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
     const int cw = wg - 1;                  // rows [64 cw, 64 cw + 64) of the tile
     const int t = threadIdx.x & 127;        // thread within the warpgroup
     const int ct = threadIdx.x - 128;       // thread within the two MMA warpgroups
+    // A thread holds accumulator rows 16 (warp % 4) + l / 4 (+ 8) of its warpgroup's 64 (and, in the f16 kind, the same A fragment rows).
+    // In the f16 kind those rows are free to be any permutation of the tile's pixels, as long as the A load and the epilogue agree:
+    // fragment row i of each group of 8 is tile row 2 (i % 4) + i / 4.  The four rows of a half-warp then differ in (row mod 8) / 2, so
+    // the 64-bit A loads from the 128B-swizzled tile, and the epilogue's 64-bit staging writes, hit 32 distinct banks.
+    const int i8 = lane >> 2;
+    const int rsub = KIND == KIND_F16X3 ? (((i8 & 3) << 1) | (i8 >> 2)) : i8;
+    const int trow = 64 * cw + 16 * (warp & 3) + rsub;   // tile row of fragment row l / 4; row + 8 is trow + 8
+    const bool live0 = trow * 128 < p.a_tile_bytes, live1 = (trow + 8) * 128 < p.a_tile_bytes;   // rows inside the TMA box
+    // fp32 A tile: the float2 of channels 8 j + 2 (l % 4) of row trow is 16-byte piece 2 j + (l % 4) / 2, XOR (trow mod 8) = rsub
+    const uint32_t a32_off = (uint32_t)trow * 128u + ((lane & 1) << 3);
+    const int a32_x = ((lane & 3) >> 1) ^ rsub;
+    // fp16 plane tiles: ldmatrix row address of lane l = row l % 8 (tile row rsub-permuted like above) of 8 x 8 matrix l / 8; matrices
+    // 0..3 = (rows 0-7, k 0-7), (rows 8-15, k 0-7), (rows 0-7, k 8-15), (rows 8-15, k 8-15) = fragment registers 0..3
+    const int lm_sub = (((lane & 3) << 1) | ((lane >> 2) & 1));
+    const uint32_t lm_off = (uint32_t)(64 * cw + 16 * (warp & 3) + 8 * ((lane >> 3) & 1) + lm_sub) * 64u;
+    const int lm_x = (lm_sub >> 1) & 3, lm_k = lane >> 4;   // SWIZZLE_64B: 16-byte piece XOR ((row / 2) mod 4)
     float acc[NMAIN][R];
     float accx[R];
+    uint32_t fh[2][Cfg::KSTEPS][4], fl[2][Cfg::KSTEPS][4];  // f16 A fragments (hi, lo), double-buffered across k-blocks
+    bool bad = false;                                       // an fp32 activation in a live row does not fit fp16
     uint32_t it = 0, tcount = 0;
     for (int item = blockIdx.x; item < num_tiles; item += gridDim.x, ++tcount) {
         int w0, h0, n0img, n0;
         tile_of(item, w0, h0, n0img, n0);
+        int nlive = (p.cout - n0 + 31) / 32;       // chunks past the true Cout are neither computed nor stored
+        nlive = nlive > Cfg::NCHUNK ? Cfg::NCHUNK : nlive;
 #pragma unroll
         for (int i = 0; i < R; ++i) {
             accx[i] = 0.f;
 #pragma unroll
             for (int a = 0; a < NMAIN; ++a) acc[a][i] = 0.f;
         }
+        // RES_TILE: the residual tile goes to the staging area while the main loop runs, once the previous tile's stores have read it.
+        // Called after the first k-block's MMAs are issued, so that waiting for those stores overlaps tensor-core work.
+        auto prefetch_residual = [&]() {
+            if (p.res_mode == RES_TILE && ct == 0) {
+                tma_store_wait_read0();
+                mbar_arrive_expect_tx(bar_res, (uint32_t)(nlive * p.a_tile_bytes));
+                for (int c = 0; c < nlive; ++c) tma_load_4d(epi_base + c * Cfg::A_BYTES, &p.tm_r, bar_res, n0 + c * 32, w0, h0, n0img);
+            }
+        };
         int prev_s = -1;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-            const int s = it % STAGES;
-            mbar_wait(bar_full(s), (it / STAGES) & 1u);
-            const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
-            uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
-            if constexpr (KIND == KIND_F16X3) {
+        if constexpr (KIND == KIND_F16X3) {
+            // one k-block into fragment buffer B: wait for the stage, load A into registers, one uninterrupted batch of wgmmas, then
+            // retire the previous k-block's batch (whose fragment buffer the next k-block rewrites) and hand its stage back
+            auto kblock = [&](auto B, int kb) {
+                constexpr int b = decltype(B)::value;
+                const int s = it % STAGES;
+                mbar_wait(bar_full(s), (it / STAGES) & 1u);
+                const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+                const uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
                 if (!p.a_planes) {
-                    // A_h = fp16(A), A_l = fp16(A - A_h): thread -> (row, two 8-channel groups); two 16-byte pieces of the 128B-swizzled
-                    // fp32 row in, one 16-byte piece of each 64B-swizzled fp16 row out, per group
-                    const int r = 64 * cw + (t & 63);
-                    uint8_t* ah = st_gen + Cfg::A_BYTES;
-                    uint8_t* al = ah + Cfg::A_BYTES / 2;
-                    bool bad = false;
+                    // fragment register (hr + 2 (j % 2)) of k-step j / 2 = the float2 of channels 8 j + 2 (l % 4) of row trow + 8 hr
+                    float2 v[2][4];
 #pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int c8 = (t >> 6) * 2 + i;
-                        const float4 v0 = *reinterpret_cast<const float4*>(st_gen + r * 128 + (((2 * c8) ^ (r & 7)) << 4));
-                        const float4 v1 = *reinterpret_cast<const float4*>(st_gen + r * 128 + (((2 * c8 + 1) ^ (r & 7)) << 4));
-                        const float f[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-                        __half2 hh[4], ll[4];
+                    for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            v[hr][j] = *reinterpret_cast<const float2*>(st_gen + a32_off + hr * 1024 + (((2 * j) ^ a32_x) << 4));
+#pragma unroll
+                    for (int hr = 0; hr < 2; ++hr) {
+                        bool b_hr = false;
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
-                            const __half x0 = __float2half_rn(f[2 * j]), x1 = __float2half_rn(f[2 * j + 1]);
-                            bad = bad || !(fabsf(f[2 * j]) < 65504.f) || !(fabsf(f[2 * j + 1]) < 65504.f);
-                            hh[j] = __halves2half2(x0, x1);
-                            ll[j] = __halves2half2(__float2half_rn(f[2 * j] - __half2float(x0)), __float2half_rn(f[2 * j + 1] - __half2float(x1)));
+                            split_f16x2(v[hr][j], fh[b][j >> 1][hr + 2 * (j & 1)], fl[b][j >> 1][hr + 2 * (j & 1)]);
+                            b_hr = b_hr || !(fabsf(v[hr][j].x) < 65504.f) || !(fabsf(v[hr][j].y) < 65504.f);
                         }
-                        const int off = r * 64 + ((c8 ^ ((r >> 1) & 3)) << 4);
-                        *reinterpret_cast<uint4*>(ah + off) = *reinterpret_cast<const uint4*>(hh);
-                        if (p.passes == 3) *reinterpret_cast<uint4*>(al + off) = *reinterpret_cast<const uint4*>(ll);
+                        // rows past the TMA box (boxes smaller than 128 pixels) hold stale data: their accumulator rows are never stored,
+                        // and they must not raise the range flag
+                        bad = bad || (b_hr && (hr == 0 ? live0 : live1));
                     }
-                    // rows past the TMA box (boxes smaller than 128 pixels) hold stale data: their accumulator rows are never stored, and
-                    // they must not trip the range flag
-                    if (bad && r * 128 < p.a_tile_bytes && p.range_flag) *p.range_flag = 1;
-                    fence_proxy_async_smem();      // generic-proxy writes -> visible to the tensor core (async proxy)
-                    named_bar_sync(2 + cw, 128);
+                } else {
+#pragma unroll
+                    for (int k = 0; k < Cfg::KSTEPS; ++k) {
+                        const uint32_t a = st + lm_off + ((uint32_t)((2 * k + lm_k) ^ lm_x) << 4);
+                        ldmatrix_x4(fh[b][k], a);
+                        ldmatrix_x4(fl[b][k], a + Cfg::A_BYTES / 2);
+                    }
                 }
-            } else {
+                const uint64_t dbh = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES);
+                const uint64_t dbl = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
+                // the same MMA sequence per k-step as the three-term product always ran: cross terms A_l B_h, A_h B_l, then the main term
+                auto batch = [&](float (&am)[R]) {
+                    if (p.passes == 3) {
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < Cfg::KSTEPS; ++k) {
+                            const uint64_t koff = (uint64_t)(k * 32 >> 4);
+                            conv_mma_f16<BLOCK_N>(accx, fl[b][k], dbh + koff);
+                            conv_mma_f16<BLOCK_N>(accx, fh[b][k], dbl + koff);
+                            conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + koff);
+                        }
+                        wgmma_commit();
+                    } else {
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < Cfg::KSTEPS; ++k) conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + (uint64_t)(k * 32 >> 4));
+                        wgmma_commit();
+                    }
+                };
+                // NMAIN == 3 rotates the main term over three accumulators by k-block (see the tf32 loop)
+                if constexpr (NMAIN == 1) {
+                    batch(acc[0]);
+                } else {
+                    const int sel = kb % 3;
+                    if (sel == 0) batch(acc[0]);
+                    else if (sel == 1) batch(acc[NMAIN > 1 ? 1 : 0]);
+                    else batch(acc[NMAIN > 2 ? 2 : 0]);
+                }
+                wgmma_wait<1>();
+                if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
+                prev_s = s;
+                ++it;
+            };
+            for (int kb = 0; kb < num_kb; kb += 2) {
+                kblock(IntC<0>{}, kb);
+                if (kb == 0) prefetch_residual();
+                if (kb + 1 < num_kb) kblock(IntC<1>{}, kb + 1);
+            }
+        } else {
+            for (int kb = 0; kb < num_kb; ++kb, ++it) {
+                const int s = it % STAGES;
+                mbar_wait(bar_full(s), (it / STAGES) & 1u);
+                const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+                uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
                 if (p.passes == 3) {
                     // A_lo = A - trunc_tf32(A), element-wise, so the swizzled placement is preserved verbatim
                     const float4* a = reinterpret_cast<const float4*>(st_gen) + 512 * cw;
@@ -273,43 +366,36 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
                     fence_proxy_async_smem();
                     named_bar_sync(2 + cw, 128);
                 }
-            }
-            uint64_t da, dal, dbh, dbl;      // "hi" A, "lo" A, "hi" B, "lo" B
-            if constexpr (KIND == KIND_F16X3) {
-                da = gmma_desc_sw64(st + Cfg::A_BYTES + cw * 64 * 64);
-                dal = gmma_desc_sw64(st + Cfg::A_BYTES + Cfg::A_BYTES / 2 + cw * 64 * 64);
-                dbh = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES);
-                dbl = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
-            } else {
-                da = gmma_desc_sw128(st + cw * 64 * 128);
-                dal = gmma_desc_sw128(st + Cfg::A_BYTES + cw * 64 * 128);
-                dbh = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES);
-                dbl = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
-            }
-            wgmma_fence();
+                const uint64_t da = gmma_desc_sw128(st + cw * 64 * 128);
+                const uint64_t dal = gmma_desc_sw128(st + Cfg::A_BYTES + cw * 64 * 128);
+                const uint64_t dbh = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES);
+                const uint64_t dbl = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
+                wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < Cfg::KSTEPS; ++k) {
-                const uint64_t koff = (uint64_t)(k * 32 >> 4);
-                if (p.passes == 3) {
-                    conv_mma<BLOCK_N, KIND>(accx, dal + koff, dbh + koff);
-                    conv_mma<BLOCK_N, KIND>(accx, da + koff, dbl + koff);
+                for (int k = 0; k < Cfg::KSTEPS; ++k) {
+                    const uint64_t koff = (uint64_t)(k * 32 >> 4);
+                    if (p.passes == 3) {
+                        conv_mma_tf32<BLOCK_N>(accx, dal + koff, dbh + koff);
+                        conv_mma_tf32<BLOCK_N>(accx, da + koff, dbl + koff);
+                    }
+                    // The tensor core accumulates in fp32 with truncation, so every accumulate step costs up to 1 ulp of the running sum.
+                    // NMAIN == 3 rotates the main term over three accumulators by k-block (summed with RN adds in the epilogue): shorter chains.
+                    if constexpr (NMAIN == 1) {
+                        conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
+                    } else {
+                        const int sel = kb % 3;
+                        if (sel == 0) conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
+                        else if (sel == 1) conv_mma_tf32<BLOCK_N>(acc[NMAIN > 1 ? 1 : 0], da + koff, dbh + koff);
+                        else conv_mma_tf32<BLOCK_N>(acc[NMAIN > 2 ? 2 : 0], da + koff, dbh + koff);
+                    }
                 }
-                // The tensor core accumulates in fp32 with truncation, so every accumulate step costs up to 1 ulp of the running sum.
-                // NMAIN == 3 rotates the main term over three accumulators by k-block (summed with RN adds in the epilogue): shorter chains.
-                if constexpr (NMAIN == 1) {
-                    conv_mma<BLOCK_N, KIND>(acc[0], da + koff, dbh + koff);
-                } else {
-                    const int sel = kb % 3;
-                    if (sel == 0) conv_mma<BLOCK_N, KIND>(acc[0], da + koff, dbh + koff);
-                    else if (sel == 1) conv_mma<BLOCK_N, KIND>(acc[NMAIN > 1 ? 1 : 0], da + koff, dbh + koff);
-                    else conv_mma<BLOCK_N, KIND>(acc[NMAIN > 2 ? 2 : 0], da + koff, dbh + koff);
-                }
+                wgmma_commit();
+                if (kb == 0) prefetch_residual();
+                // the MMAs of the previous k-block have retired: its stage goes back to the producer
+                wgmma_wait<1>();
+                if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
+                prev_s = s;
             }
-            wgmma_commit();
-            // the MMAs of the previous k-block have retired: its stage goes back to the producer
-            wgmma_wait<1>();
-            if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
-            prev_s = s;
         }
         wgmma_wait<0>();
         if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
@@ -318,21 +404,13 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
         for (int a = 0; a < NMAIN; ++a) reg_fence(acc[a]);
 
         // ---------------------------------------------------------------- epilogue
-        int nlive = (p.cout - n0 + 31) / 32;       // chunks past the true Cout are neither computed nor stored
-        nlive = nlive > Cfg::NCHUNK ? Cfg::NCHUNK : nlive;
-        if (ct == 0) {
-            tma_store_wait_read0();                // the previous tile's stores have read the staging area
-            if (p.res_mode == RES_TILE) {
-                mbar_arrive_expect_tx(bar_res, (uint32_t)(nlive * p.a_tile_bytes));
-                for (int c = 0; c < nlive; ++c) tma_load_4d(epi_base + c * Cfg::A_BYTES, &p.tm_r, bar_res, n0 + c * 32, w0, h0, n0img);
-            }
-        }
+        if (ct == 0 && p.res_mode != RES_TILE) tma_store_wait_read0();   // the previous tile's stores have read the staging area
         named_bar_sync(1, 256);
         if (p.res_mode == RES_TILE) mbar_wait(bar_res, tcount & 1u);
-        // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1)
-        const int rbase = 64 * cw + 16 * (warp & 3) + (lane >> 2);
+        // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1);
+        // its rows are tile rows trow (+ 8)
+        const int rbase = trow;
         const int cq = 2 * (lane & 3);
-        bool bad = false;
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int row = rbase + 8 * hr;
