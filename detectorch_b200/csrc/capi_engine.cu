@@ -183,6 +183,7 @@ struct Engine {
     const float* image = nullptr;
     float scaling_factor = 1.f;
     float orig_h = 0.f, orig_w = 0.f;   // original image size for the final clip (0 = network size / scaling_factor)
+    bool use_image_info = false;        // per-image sizes / scales from the "im_info" buffer (dt_engine_use_image_info)
     // static geometry
     int H1, W1, H2, W2;                 // stem out, pool out
     int Hp, Wp;                         // padded NHWC4 stem input
@@ -220,6 +221,8 @@ struct Engine {
         if (it == bufs.end()) { fprintf(stderr, "[detectorch_b200] engine: unknown buffer %s\n", n.c_str()); return nullptr; }
         return reinterpret_cast<T*>(ws + it->second.off);
     }
+    // the per-image table the kernels read (image_info), or null when every image fills the canvas
+    const float* im_info() { return use_image_info ? buf("im_info") : nullptr; }
 };
 
 // ---- parameter table ---------------------------------------------------------------------------
@@ -415,6 +418,7 @@ void plan_buffers(Engine* e) {
     add_buf(e, "det_boxes", {B, cap, 4}); add_buf(e, "det_scores", {B, cap}); add_buf(e, "det_classes", {B, cap}, 1);
     add_buf(e, "det_roi_idx", {B, cap}, 1); add_buf(e, "det_counts", {B}, 1);
     add_buf(e, "range_flag", {1}, 1);     // raised by a kind::f16 conv when an activation does not fit fp16
+    add_buf(e, "im_info", {B, 5});        // per-image (net_h, net_w, scaling_factor, orig_h, orig_w), read when dt_engine_use_image_info is on
     if (c.use_mask) {
         const long long D = (long long)B * cap;
         add_buf(e, "mask_rois", {D, 5}); add_buf(e, "mask_levels", {D}, 1);
@@ -435,6 +439,7 @@ struct ProgBuilder {
     Engine* e;
     std::map<std::string, ConvW>* cw;
     bool ok = true;
+    int img_stride = 0;     // > 0: the following convs write image-shaped maps at this stride (masked per image when the table is on)
 
     void conv(int stage, const std::string& wname, const float* x, int N, int H, int W, int xstride, float* y, int ystride, int kpad,
               int stride, bool relu, int res_mode = RES_NONE, const float* res = nullptr, const float* up = nullptr, int up_h = 0,
@@ -478,6 +483,7 @@ struct ProgBuilder {
         s.out_h = out_h; s.out_w = out_w; s.out_step = out_step; s.out_y0 = oy; s.out_x0 = ox;
         s.residual = res; s.res_pix_stride = c.cout; s.up_src = up; s.up_h = up_h; s.up_w = up_w;
         s.res_mode = res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = sigmoid_ch; s.passes = e->cfg.passes; s.force_block_n = force_bn; s.precise = (force_bn == 128) ? 1 : 0;
+        s.im_stride = img_stride;
         op.stage = stage; op.kind = 0; op.fn = -1;
         {
             const int Ho = (H + 2 * kpad - c.k) / stride + 1, Wo = (W + 2 * kpad - c.k) / stride + 1;
@@ -499,30 +505,30 @@ struct ProgBuilder {
 
 cudaError_t fn_stem_im2col(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->H1 * e->W1 * 40;
-    stem_im2col_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->H1, e->W1, e->buf("stem_col"));
+    stem_im2col_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->H1, e->W1, e->buf("stem_col"), e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_stem_pack(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->Hp * e->Wp;
-    stem_pack_nhwc4_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->Hp, e->Wp, e->buf("stem_x4"));
+    stem_pack_nhwc4_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->Hp, e->Wp, e->buf("stem_x4"), e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_stem_pack_planes(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->Hp * e->Wp;
     uint2* xh = reinterpret_cast<uint2*>(e->buf("stem_x4"));
     stem_pack_nhwc4_planes_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->Hp, e->Wp, xh, xh + n,
-                                                             e->buf<int>("range_flag"));
+                                                             e->buf<int>("range_flag"), e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_maxpool(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->H2 * e->W2 * 16;
-    maxpool3x3s2_nhwc_kernel<false><<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"), nullptr);
+    maxpool3x3s2_nhwc_kernel<false><<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"), nullptr, e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_maxpool_planes(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->H2 * e->W2 * 16;
     maxpool3x3s2_nhwc_kernel<true><<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"),
-                                                              e->buf<int>("range_flag"));
+                                                              e->buf<int>("range_flag"), e->im_info());
     return cudaGetLastError();
 }
 
@@ -548,6 +554,7 @@ void rpn_modes(Engine* e, int levels) {
 cudaError_t launch_proposals(Engine* e, cudaStream_t s, int levels) {
     RpnParams& P = e->rpn;
     P.scaling_factor = e->scaling_factor;
+    P.im_info = e->im_info();
     rpn_modes(e, levels);
     int max_n = 0;
     for (int l = 0; l < levels; ++l) max_n = std::max(max_n, P.lv[l].n);
@@ -575,6 +582,7 @@ cudaError_t fn_collect(Engine* e, cudaStream_t s) {
 }
 cudaError_t fn_roi_box(Engine* e, cudaStream_t s) {
     const int R = e->cfg.batch * e->cfg.post_nms_top_n;
+    e->roi_lv.im_info = e->im_info();
     // per-image counts: padded rows carry zero boxes (collect_kernel) -> harmless, fully defined output
     if (e->cfg.exact_roialign)
         roi_align_nhwc_kernel<<<R < num_sms() * 64 ? R : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), nullptr, R, 256, 7, 7,
@@ -594,6 +602,7 @@ cudaError_t fn_detect(Engine* e, cudaStream_t s) {
     e->det.scaling_factor = e->scaling_factor;
     e->det.im_h = e->orig_h > 0.f ? e->orig_h : (float)e->cfg.height / e->scaling_factor;
     e->det.im_w = e->orig_w > 0.f ? e->orig_w : (float)e->cfg.width / e->scaling_factor;
+    e->det.im_info = e->im_info();
     det_class_kernel<<<dim3(e->cfg.num_classes - 1, e->cfg.batch), 256, 0, s>>>(e->det);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
@@ -603,11 +612,12 @@ cudaError_t fn_detect(Engine* e, cudaStream_t s) {
 cudaError_t fn_mask_rois(Engine* e, cudaStream_t s) {
     const int n = e->cfg.batch * e->cfg.det_cap;
     mask_rois_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->buf("det_boxes"), e->buf<int>("det_counts"), e->cfg.batch, e->cfg.det_cap, e->scaling_factor, 2, 5,
-                                                    e->buf("mask_rois"), e->buf<int>("mask_levels"));
+                                                    e->buf("mask_rois"), e->buf<int>("mask_levels"), e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_mask_roi_feat(Engine* e, cudaStream_t s) {
     const int D = e->cfg.batch * e->cfg.det_cap;
+    e->roi_lv.im_info = e->im_info();
     if (e->cfg.exact_roialign)
         roi_align_nhwc_kernel<<<D < num_sms() * 64 ? D : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), nullptr, D, 256, 14,
                                                                           14, 2, e->buf("mask_feat"));
@@ -669,6 +679,7 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
         }
         if (e->stem_fused) {
             pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
+            op.conv.p.im_stride = 2;        // c1 is image-shaped (the im2col stem's GEMM-shaped output is not: the pool bounds its reads)
             e->ops.push_back(op);
         } else {
             if (!c.stem_im2col) fprintf(stderr, "[detectorch_b200] engine: fused stem descriptor rejected, using the im2col stem\n");
@@ -685,6 +696,7 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
     int h = e->H2, w = e->W2, cin = 64;
     for (int li = 1; li <= 4; ++li) {
         const int planes = 64 << (li - 1);
+        pb.img_stride = 4 << (li - 1);
         for (int b = 0; b < c.arch_blocks[li - 1]; ++b) {
             const std::string p = "l" + std::to_string(li) + "b" + std::to_string(b);
             const std::string wp = "model.layer" + std::to_string(li) + "." + std::to_string(b) + ".";
@@ -718,6 +730,7 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
     const int cins[4] = {256, 512, 1024, 2048};
     for (int i = 3; i >= 0; --i) {
         const std::string ln = "conv_body.fpn_lateral." + std::to_string(i);
+        pb.img_stride = 4 << i;
         const float* src = e->buf("C" + std::to_string(i + 2));
         if (i == 3)
             pb.conv(ST_FPN, ln, src, B, e->LH[i], e->LW[i], cins[i], e->buf("inner5"), 256, 0, 1, false);
@@ -725,17 +738,21 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
             pb.conv(ST_FPN, ln, src, B, e->LH[i], e->LW[i], cins[i], e->buf("inner" + std::to_string(i + 2)), 256, 0, 1, false, RES_UPSAMPLE2X,
                     nullptr, e->buf("inner" + std::to_string(i + 3)), e->LH[i + 1], e->LW[i + 1]);
     }
-    for (int i = 0; i < 4; ++i)
+    for (int i = 0; i < 4; ++i) {
+        pb.img_stride = 4 << i;
         pb.conv(ST_FPN, "conv_body.fpn_output." + std::to_string(i), e->buf("inner" + std::to_string(i + 2)), B, e->LH[i], e->LW[i], 256,
                 e->buf("P" + std::to_string(i + 2)), 256, 1, 1, false);
+    }
     pb.fn(ST_FPN, fn_p6);
     // ---- RPN head on P2..P6 (detector.py:251)
     for (int i = 0; i < 5 && c.use_rpn; ++i) {
         const std::string L = std::to_string(i + 2);
+        pb.img_stride = 4 << i;
         pb.conv(ST_RPN, "rpn.conv_rpn", e->buf("P" + L), B, e->LH[i], e->LW[i], 256, e->buf("rpn_t" + L), 256, 1, 1, true);
         pb.conv(ST_RPN, "rpn.head", e->buf("rpn_t" + L), B, e->LH[i], e->LW[i], 256, e->buf("rpn_out" + L), 16, 0, 1, false, RES_NONE, nullptr,
                 nullptr, 0, 0, 3);
     }
+    pb.img_stride = 0;      // everything below is RoI-shaped
     // ---- proposals (generate_proposals.py) + collect (collect_and_distribute...py)
     if (c.use_rpn) {
         RpnParams& P = e->rpn;
@@ -778,6 +795,7 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
         e->roi_lv.feat[i] = e->buf("P" + std::to_string(i + 2));
         e->roi_lv.H[i] = e->LH[i]; e->roi_lv.W[i] = e->LW[i];
         e->roi_lv.scale[i] = 1.f / (float)(4 << i);
+        e->roi_lv.stride[i] = 4 << i;
     }
     pb.fn(ST_ROI_BOX, fn_roi_box);
     // ---- box head (detector.py:61-64,277-284)
@@ -901,6 +919,12 @@ int64_t dt_engine_weight_bytes(dt_engine_t h) {
 }
 int64_t dt_engine_workspace_bytes(dt_engine_t h) { return (int64_t)reinterpret_cast<Engine*>(h)->ws_bytes; }
 
+// the image-shaped conv launches read the table (or not) -- the other kernels take e->im_info() when they are launched
+static void apply_image_info(Engine* e) {
+    for (Op& op : e->ops)
+        if (op.kind == 0 && op.conv.p.im_stride > 0) op.conv.p.im_info = e->im_info();
+}
+
 static int bind_impl(Engine* e, void* weights, void* workspace, cudaStream_t st, bool fresh) {
     e->wbase = reinterpret_cast<float*>(weights);
     e->ws = reinterpret_cast<uint8_t*>(workspace);
@@ -921,6 +945,7 @@ static int bind_impl(Engine* e, void* weights, void* workspace, cudaStream_t st,
         if (e->cfg.model_type == 1) build_param_table_c4(&tmp, &cw); else build_param_table(&tmp, &cw);
     }
     if (!(e->cfg.model_type == 1 ? build_program_c4(e, &cw) : build_program(e, &cw))) return 0;
+    apply_image_info(e);
     e->bound = true;
     return 1;
 }
@@ -1012,6 +1037,17 @@ int dt_engine_param_info(dt_engine_t h, int i, char* name_out, int name_cap, int
 int dt_engine_set_original_size(dt_engine_t h, float orig_h, float orig_w) {
     Engine* e = reinterpret_cast<Engine*>(h);
     e->orig_h = orig_h; e->orig_w = orig_w;
+    return 1;
+}
+
+int dt_engine_use_image_info(dt_engine_t h, int enabled) {
+    Engine* e = reinterpret_cast<Engine*>(h);
+    if (enabled && (e->cfg.model_type != 0 || e->bufs.find("im_info") == e->bufs.end())) {
+        fprintf(stderr, "[detectorch_b200] engine: per-image sizes are built for the FPN engine only\n");
+        return 0;
+    }
+    e->use_image_info = enabled != 0;
+    apply_image_info(e);
     return 1;
 }
 

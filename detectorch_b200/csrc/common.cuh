@@ -37,6 +37,34 @@ inline int num_sms() {
 __host__ __device__ __forceinline__ int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ __forceinline__ long long ceil_div64(long long a, long long b) { return (a + b - 1) / b; }
 
+// ---------------------------------------------------------------------------------- per-image geometry of a padded batch
+// A batch of differently-sized images shares one canvas: image b occupies the top-left net_h x net_w of its slot.  The engine's
+// im_info table [batch, 5] = (net_h, net_w, scaling_factor, orig_h, orig_w) describes them; kernels read it at run time (a captured
+// graph replays for any size mix).  orig_h / orig_w <= 0 stand for net / scaling_factor.
+struct ImageInfo {
+    int h, w;                 // extent at the requested stride, ceil(net / stride), clamped to the map
+    float scale;              // scaling_factor
+    float orig_h, orig_w;     // original image size (the detection clip)
+};
+// image b at `stride` on a map_h x map_w canvas map.  Without a table (im_info == null) the image fills the canvas and the scalar
+// arguments hold.
+__device__ __forceinline__ ImageInfo image_info(const float* im_info, int b, int stride, int map_h, int map_w, float scale = 1.f,
+                                                float orig_h = 0.f, float orig_w = 0.f) {
+    ImageInfo g;
+    g.h = map_h; g.w = map_w; g.scale = scale; g.orig_h = orig_h; g.orig_w = orig_w;
+    if (im_info) {
+        const float* r = im_info + 5 * (size_t)b;
+        const float nh = r[0], nw = r[1];
+        const int ih = nh > 0.f ? (int)fminf(nh, 1e9f) : 0, iw = nw > 0.f ? (int)fminf(nw, 1e9f) : 0;   // NaN / negative -> 0
+        g.h = max(1, min(ceil_div(ih, stride), map_h));      // never past the map, never empty (RoIAlign clamps to extent - 1)
+        g.w = max(1, min(ceil_div(iw, stride), map_w));
+        g.scale = r[2];
+        g.orig_h = r[3] > 0.f ? r[3] : __fdiv_rn(nh, r[2]);
+        g.orig_w = r[4] > 0.f ? r[4] : __fdiv_rn(nw, r[2]);
+    }
+    return g;
+}
+
 // ---------------------------------------------------------------------------------- smem / mbarrier
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

@@ -137,6 +137,7 @@ struct ConvSpec {
     int tap0, ntaps;                              // K-split: only filter taps [tap0, tap0+ntaps) (ntaps == 0: all kh*kw)
     int force_block_n;                            // 0 = auto (64 or 128)
     int precise;                                  // 64-wide tiles with 3 rotating main-term accumulators (shorter accumulation chains)
+    int im_stride;                                // image-shaped output at this stride: pixels outside each image can be zeroed (ConvParams::im_info)
 };
 
 inline void choose_box(int Wo, int Ho, int N, int max_w, int* wbox, int* hbox, int* nbox) {
@@ -244,6 +245,7 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     p.a_tile_bytes = wbox * hbox * nbox * 128;
     p.relu = s.relu; p.sigmoid_ch = s.sigmoid_ch; p.res_mode = s.res_mode;
     p.passes = s.passes == 1 ? 1 : 3;
+    p.im_stride = s.out_step == 0 ? s.im_stride : 0;
     // 64-wide tiles rotate the main term over 3 accumulators (same register budget as one 128-wide pair) -- except at K <= 256, where
     // one accumulator already is a chain of at most 16 k-blocks
     L->nmain = (bn == 64 && (s.precise || p.ntaps * p.cin_blocks > 8)) ? 3 : 1;
@@ -309,12 +311,12 @@ inline bool conv_use_pdl() {
     return v == 1;
 }
 
-template <int BN, int NM, int KIND>
+template <int BN, int NM, int KIND, bool MASK>
 inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
     using Cfg = ConvCfg<BN, NM, KIND>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
@@ -328,22 +330,24 @@ inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, conv_wgmma_kernel<BN, NM, KIND>, prm);
+        return cudaLaunchKernelEx(&cfg, conv_wgmma_kernel<BN, NM, KIND, MASK>, prm);
     }
-    conv_wgmma_kernel<BN, NM, KIND><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
+    conv_wgmma_kernel<BN, NM, KIND, MASK><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
     return cudaGetLastError();
 }
 
-template <int KIND>
+template <int KIND, bool MASK>
 inline cudaError_t conv_launch_kind(const ConvLayer& L, cudaStream_t stream) {
-    if (L.block_n == 64) return L.nmain == 3 ? conv_launch_cfg<64, 3, KIND>(L, stream) : conv_launch_cfg<64, 1, KIND>(L, stream);
-    if (L.block_n == 128 && L.nmain == 1) return conv_launch_cfg<128, 1, KIND>(L, stream);
+    if (L.block_n == 64) return L.nmain == 3 ? conv_launch_cfg<64, 3, KIND, MASK>(L, stream) : conv_launch_cfg<64, 1, KIND, MASK>(L, stream);
+    if (L.block_n == 128 && L.nmain == 1) return conv_launch_cfg<128, 1, KIND, MASK>(L, stream);
     return cudaErrorInvalidValue;
 }
 
 inline cudaError_t conv_launch(const ConvLayer& L, cudaStream_t stream) {
     if (!L.valid) return cudaErrorInvalidValue;
-    return L.kind == KIND_F16X3 ? conv_launch_kind<KIND_F16X3>(L, stream) : conv_launch_kind<KIND_TF32X3>(L, stream);
+    if (L.p.im_info)
+        return L.kind == KIND_F16X3 ? conv_launch_kind<KIND_F16X3, true>(L, stream) : conv_launch_kind<KIND_TF32X3, true>(L, stream);
+    return L.kind == KIND_F16X3 ? conv_launch_kind<KIND_F16X3, false>(L, stream) : conv_launch_kind<KIND_TF32X3, false>(L, stream);
 }
 
 }  // namespace dt

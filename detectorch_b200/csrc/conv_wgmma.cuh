@@ -75,6 +75,10 @@ struct ConvParams {
     int out_planes;        // KIND_F16X3: write the output as a pair of fp16 planes (hi = fp16(y), lo = fp16(y - hi)) instead of fp32
     int* range_flag;       // KIND_F16X3: set to 1 when an activation does not fit fp16 (|x| >= 65504 or NaN); may be null
     int pdl;               // launched with programmatic stream serialization: release the next launch early, wait for the previous one
+    // image-shaped maps of a batch of differently-sized images: output pixels outside image n's extent at im_stride (image_info) are
+    // written as exact zeros, so the next 3x3 conv reads what a batch-1 run of that image reads through TMA zero fill.  Null = off.
+    const float* im_info;
+    int im_stride;         // output stride relative to the network input (0: not an image-shaped launch)
 };
 
 template <int BLOCK_N, int NMAIN, int KIND>
@@ -130,7 +134,9 @@ __device__ __forceinline__ void split_f16x2(float2 v, uint32_t& hi, uint32_t& lo
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-template <int BLOCK_N, int NMAIN, int KIND>
+// MASK: the launch zeroes pixels outside each image (p.im_info non-null); a separate instantiation, so that the epilogue of every other
+// launch is the plain one
+template <int BLOCK_N, int NMAIN, int KIND, bool MASK>
 __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     using Cfg = ConvCfg<BLOCK_N, NMAIN, KIND>;
     constexpr int STAGES = Cfg::STAGES;
@@ -414,6 +420,15 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int row = rbase + 8 * hr;
+            bool outside = false;           // past its image's extent: the row is written as zeros below, and never raises the range flag
+            if constexpr (MASK) {
+                int r = row;
+                const int pw_ = r % p.wbox; r /= p.wbox;
+                const int ph_ = r % p.hbox; r /= p.hbox;
+                const ImageInfo g = image_info(p.im_info, min(n0img + r, p.nimg - 1), p.im_stride, p.ho, p.wo);
+                outside = h0 + ph_ >= g.h || w0 + pw_ >= g.w;
+            }
+            const bool flag_row = row * 128 < p.a_tile_bytes && !outside;
             const float* up_row = nullptr;
             if (p.res_mode == RES_UPSAMPLE2X) {
                 int r = row;
@@ -463,12 +478,28 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
                     const __half2 h = __floats2half2_rn(o0, o1);
                     const float2 hf = __half22float2(h);
                     const __half2 l = __floats2half2_rn(o0 - hf.x, o1 - hf.y);
-                    bad = bad || ((!(fabsf(o0) < 65504.f) || !(fabsf(o1) < 65504.f)) && row * 128 < p.a_tile_bytes);
+                    bad = bad || ((!(fabsf(o0) < 65504.f) || !(fabsf(o1) < 65504.f)) && flag_row);
                     const int off16 = row * 64 + ((((col & 31) >> 3) ^ ((row >> 1) & 3)) << 4) + ((col & 7) << 1);
                     *reinterpret_cast<__half2*>(slot + off16) = h;
                     *reinterpret_cast<__half2*>(slot + Cfg::A_BYTES / 2 + off16) = l;
                 } else {
                     *reinterpret_cast<float2*>(slot + off32) = make_float2(o0, o1);
+                }
+            }
+            if (MASK && outside) {
+                // rare (per-image sizes only): overwrite the row's staged values instead of testing every element above
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int col = 8 * j + cq, c = j >> 2;
+                    if (c >= nlive) continue;
+                    uint8_t* slot = epi_gen + c * Cfg::A_BYTES;
+                    if (KIND == KIND_F16X3 && p.out_planes) {
+                        const int off16 = row * 64 + ((((col & 31) >> 3) ^ ((row >> 1) & 3)) << 4) + ((col & 7) << 1);
+                        *reinterpret_cast<uint32_t*>(slot + off16) = 0u;
+                        *reinterpret_cast<uint32_t*>(slot + Cfg::A_BYTES / 2 + off16) = 0u;
+                    } else {
+                        *reinterpret_cast<float2*>(slot + row * 128 + (((((col & 31) >> 2)) ^ (row & 7)) << 4) + ((col & 3) << 2)) = make_float2(0.f, 0.f);
+                    }
                 }
             }
         }

@@ -18,8 +18,9 @@ static constexpr float kBBoxXformClip = 4.135166556742356f;   // log(1000/16), b
 
 // ---------------------------------------------------------------------------------- stem im2col
 // image NCHW [B,3,H,W] -> col [B*Ho*Wo, 160], k = c*49 + ky*7 + kx (torch weight order), k >= 147 zero.
-// 7x7 stride 2 pad 3 (torchvision resnet conv1).
-static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int Wo, float* __restrict__ col) {
+// 7x7 stride 2 pad 3 (torchvision resnet conv1).  im_info (may be null): pixels outside image b read as zero (image_info).
+static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int Wo, float* __restrict__ col,
+                                          const float* __restrict__ im_info) {
     const long long total = (long long)B * Ho * Wo * 40;   // float4 granules
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int k4 = (int)(i % 40);
@@ -27,6 +28,7 @@ static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, 
         const int wo = (int)(m % Wo); m /= Wo;
         const int ho = (int)(m % Ho);
         const int b = (int)(m / Ho);
+        const ImageInfo g = image_info(im_info, b, 1, H, W);
         float v[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -35,7 +37,7 @@ static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, 
             if (k < 147) {
                 const int c = k / 49, r = k - c * 49, ky = r / 7, kx = r - ky * 7;
                 const int y = ho * 2 - 3 + ky, xx = wo * 2 - 3 + kx;
-                if (y >= 0 && y < H && xx >= 0 && xx < W) x = __ldg(img + (((size_t)b * 3 + c) * H + y) * W + xx);
+                if (y >= 0 && y < g.h && xx >= 0 && xx < g.w) x = __ldg(img + (((size_t)b * 3 + c) * H + y) * W + xx);
             }
             v[j] = x;
         }
@@ -43,16 +45,19 @@ static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, 
     }
 }
 
-// image NCHW [B,3,H,W] -> zero-bordered NHWC4 [B,Hp,Wp,4] (3-pixel border = the conv1 padding; channel 3 = 0)
-static __global__ void stem_pack_nhwc4_kernel(const float* __restrict__ img, int B, int H, int W, int Hp, int Wp, float* __restrict__ x4) {
+// image NCHW [B,3,H,W] -> zero-bordered NHWC4 [B,Hp,Wp,4] (3-pixel border = the conv1 padding; channel 3 = 0).  im_info (may be null):
+// everything outside image b is written as zero, whatever the canvas holds there (NaN included)
+static __global__ void stem_pack_nhwc4_kernel(const float* __restrict__ img, int B, int H, int W, int Hp, int Wp, float* __restrict__ x4,
+                                              const float* __restrict__ im_info) {
     const long long total = (long long)B * Hp * Wp;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int xp = (int)(i % Wp);
         const int yp = (int)((i / Wp) % Hp);
         const int b = (int)(i / ((long long)Wp * Hp));
         const int x = xp - 3, y = yp - 3;
+        const ImageInfo g = image_info(im_info, b, 1, H, W);
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (x >= 0 && x < W && y >= 0 && y < H) {
+        if (x >= 0 && x < g.w && y >= 0 && y < g.h) {
             const size_t o = ((size_t)b * 3 * H + y) * W + x;
             v.x = __ldg(img + o); v.y = __ldg(img + o + (size_t)H * W); v.z = __ldg(img + o + 2 * (size_t)H * W);
         }
@@ -77,7 +82,7 @@ __device__ __forceinline__ void split_planes4(float4 v, uint2* hi, uint2* lo, bo
 
 // stem_pack_nhwc4_kernel emitting the two fp16 planes [B, Hp, Wp, 4] the kind::f16 stem loads straight into its operand tiles
 static __global__ void stem_pack_nhwc4_planes_kernel(const float* __restrict__ img, int B, int H, int W, int Hp, int Wp, uint2* __restrict__ xh,
-                                                     uint2* __restrict__ xl, int* __restrict__ range_flag) {
+                                                     uint2* __restrict__ xl, int* __restrict__ range_flag, const float* __restrict__ im_info) {
     const long long total = (long long)B * Hp * Wp;
     bool bad = false;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -85,8 +90,9 @@ static __global__ void stem_pack_nhwc4_planes_kernel(const float* __restrict__ i
         const int yp = (int)((i / Wp) % Hp);
         const int b = (int)(i / ((long long)Wp * Hp));
         const int x = xp - 3, y = yp - 3;
+        const ImageInfo g = image_info(im_info, b, 1, H, W);
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (x >= 0 && x < W && y >= 0 && y < H) {
+        if (x >= 0 && x < g.w && y >= 0 && y < g.h) {
             const size_t o = ((size_t)b * 3 * H + y) * W + x;
             v.x = __ldg(img + o); v.y = __ldg(img + o + (size_t)H * W); v.z = __ldg(img + o + 2 * (size_t)H * W);
         }
@@ -97,10 +103,11 @@ static __global__ void stem_pack_nhwc4_planes_kernel(const float* __restrict__ i
     if (bad && range_flag) *range_flag = 1;
 }
 
-// NHWC 3x3 stride-2 pad-1 max pool (torchvision maxpool); PLANES: the result leaves as two fp16 planes (hi, lo) for plane-input convs
+// NHWC 3x3 stride-2 pad-1 max pool (torchvision maxpool); PLANES: the result leaves as two fp16 planes (hi, lo) for plane-input convs.
+// im_info (may be null): the window ends at image b's extent (the input is the stride-2 map), and outputs past it are zero.
 template <bool PLANES>
 static __global__ void maxpool3x3s2_nhwc_kernel(const float* __restrict__ x, int B, int H, int W, int C, int Ho, int Wo, float* __restrict__ y,
-                                                int* __restrict__ range_flag) {
+                                                int* __restrict__ range_flag, const float* __restrict__ im_info) {
     const int C4 = C >> 2;
     const long long total = (long long)B * Ho * Wo * C4;
     bool bad = false;
@@ -110,17 +117,19 @@ static __global__ void maxpool3x3s2_nhwc_kernel(const float* __restrict__ x, int
         const int wo = (int)(m % Wo); m /= Wo;
         const int ho = (int)(m % Ho);
         const int b = (int)(m / Ho);
+        const ImageInfo g = image_info(im_info, b, 2, H, W);
         float4 best = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
         for (int dy = 0; dy < 3; ++dy) {
             const int yy = ho * 2 - 1 + dy;
-            if (yy < 0 || yy >= H) continue;
+            if (yy < 0 || yy >= g.h) continue;
             for (int dx = 0; dx < 3; ++dx) {
                 const int xx = wo * 2 - 1 + dx;
-                if (xx < 0 || xx >= W) continue;
+                if (xx < 0 || xx >= g.w) continue;
                 const float4 v = __ldg(reinterpret_cast<const float4*>(x + (((size_t)b * H + yy) * W + xx) * C) + c4);
                 best.x = fmaxf(best.x, v.x); best.y = fmaxf(best.y, v.y); best.z = fmaxf(best.z, v.z); best.w = fmaxf(best.w, v.w);
             }
         }
+        if (ho * 2 >= g.h || wo * 2 >= g.w) best = make_float4(0.f, 0.f, 0.f, 0.f);
         if constexpr (PLANES) {
             uint2 h, l;
             split_planes4(best, &h, &l, &bad);
@@ -133,7 +142,9 @@ static __global__ void maxpool3x3s2_nhwc_kernel(const float* __restrict__ x, int
     if (PLANES && bad && range_flag) *range_flag = 1;
 }
 
-// P6 = max_pool2d(P5, kernel 1, stride 2) == stride-2 subsample (detector.py:250)
+// P6 = max_pool2d(P5, kernel 1, stride 2) == stride-2 subsample (detector.py:250).  With per-image sizes no mask is needed: output
+// (ho, wo) reads P5 at (2 ho, 2 wo), which lies inside image b's P5 extent exactly when (ho, wo) lies inside its P6 extent
+// ceil(H5 / 2), and P5 is zero outside (the conv epilogue).
 static __global__ void subsample2_nhwc_kernel(const float* __restrict__ x, int B, int H, int W, int C, int Ho, int Wo, float* __restrict__ y) {
     const int C4 = C >> 2;
     const long long total = (long long)B * Ho * Wo * C4;
@@ -248,6 +259,7 @@ struct RpnParams {
     int pre_nms, post_nms;
     float nms_thresh, min_size, scaling_factor;
     float im_h, im_w;
+    const float* im_info;    // per-image sizes and scales (image_info), null = every image fills the canvas
     long long ws_per_image;  // elements of sort workspace per image (sum over levels)
     uint32_t *k0, *k1;       // [B * ws_per_image]
     int *v0, *v1;
@@ -274,6 +286,17 @@ static constexpr int kRpnMaxChunks = 64;      // >= ceil(largest level / kRpnChu
 
 __host__ __device__ __forceinline__ bool rpn_level_selects(int n, int K) { return n > 4 * K && n > 8192; }
 
+// Image b's anchors on level lv: the ceil(net / stride) rows and columns of its valid region, n = h * w * A of them, numbered
+// (y * w + x) * A + a like those of a batch-1 run at that size (the top-k tie order and dbg_order follow this image-local index).
+struct RpnImageLevel { int n, w; };
+__device__ __forceinline__ RpnImageLevel rpn_image_level(const RpnParams& P, const RpnLevel& lv, int b) {
+    if (!P.im_info) return {lv.n, lv.W};
+    const ImageInfo g = image_info(P.im_info, b, (int)lv.stride, lv.H, lv.W);
+    return {g.h * g.w * lv.A, g.w};
+}
+// canvas cell (row-major over the level's W columns) of image-local cell `cell` of an image w cells wide
+__device__ __forceinline__ size_t rpn_canvas_cell(int cell, int w, int W) { return (size_t)(cell / w) * W + (cell % w); }
+
 // first bin with c0 + prefix >= K among 2048 bins (warp-collective, all 32 lanes of ONE warp must call); h may be global or shared
 __device__ __forceinline__ void rpn_find_bin(const uint32_t* h, uint32_t c0, uint32_t K, uint32_t* out_bin, uint32_t* out_c) {
     const int lane = threadIdx.x & 31;
@@ -299,7 +322,8 @@ static __global__ void __launch_bounds__(1024) rpn_select_keys_kernel(const __gr
     __shared__ uint32_t hist[2048];
     const int l = blockIdx.y, b = blockIdx.z;
     const RpnLevel& lv = P.lv[l];
-    const int n = lv.n, i0 = blockIdx.x * kRpnChunk;
+    const RpnImageLevel il = rpn_image_level(P, lv, b);
+    const int n = il.n, i0 = blockIdx.x * kRpnChunk;
     if (i0 >= n) return;
     const int K = (P.pre_nms <= 0 || P.pre_nms >= n) ? n : P.pre_nms;
     const bool select = rpn_level_selects(n, K);
@@ -314,7 +338,7 @@ static __global__ void __launch_bounds__(1024) rpn_select_keys_kernel(const __gr
         const int i = i0 + j * 1024 + threadIdx.x;
         valid[j] = i < n;
         k[j] = 0u;
-        if (valid[j]) { const int a = i % lv.A, cell = i / lv.A; k[j] = float_desc_key(base[(size_t)cell * lv.ch_stride + a]); }
+        if (valid[j]) { const int a = i % lv.A, cell = i / lv.A; k[j] = float_desc_key(base[rpn_canvas_cell(cell, il.w, lv.W) * lv.ch_stride + a]); }
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -341,7 +365,8 @@ static __global__ void __launch_bounds__(1024) rpn_select_hist2_kernel(const __g
     __shared__ uint32_t sel[2];
     const int l = blockIdx.y, b = blockIdx.z;
     const RpnLevel& lv = P.lv[l];
-    const int n = lv.n, i0 = blockIdx.x * kRpnChunk;
+    const RpnImageLevel il = rpn_image_level(P, lv, b);
+    const int n = il.n, i0 = blockIdx.x * kRpnChunk;
     if (i0 >= n) return;
     const int K = (P.pre_nms <= 0 || P.pre_nms >= n) ? n : P.pre_nms;
     if (!rpn_level_selects(n, K)) return;
@@ -378,7 +403,8 @@ static __global__ void __launch_bounds__(1024) rpn_select_count_kernel(const __g
     __shared__ uint32_t hh[4096];
     const int l = blockIdx.y, b = blockIdx.z;
     const RpnLevel& lv = P.lv[l];
-    const int n = lv.n, i0 = blockIdx.x * kRpnChunk;
+    const RpnImageLevel il = rpn_image_level(P, lv, b);
+    const int n = il.n, i0 = blockIdx.x * kRpnChunk;
     if (i0 >= n) return;
     const int K = (P.pre_nms <= 0 || P.pre_nms >= n) ? n : P.pre_nms;
     if (!rpn_level_selects(n, K)) return;
@@ -415,7 +441,8 @@ static __global__ void __launch_bounds__(1024) rpn_select_scatter_kernel(const _
     __shared__ int offset;
     const int l = blockIdx.y, b = blockIdx.z;
     const RpnLevel& lv = P.lv[l];
-    const int n = lv.n, i0 = blockIdx.x * kRpnChunk;
+    const RpnImageLevel il = rpn_image_level(P, lv, b);
+    const int n = il.n, i0 = blockIdx.x * kRpnChunk;
     if (i0 >= n) return;
     const int K = (P.pre_nms <= 0 || P.pre_nms >= n) ? n : P.pre_nms;
     if (!rpn_level_selects(n, K)) return;
@@ -459,7 +486,8 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
     __shared__ int scratch[33];
     const int l = blockIdx.x, b = blockIdx.y;
     const RpnLevel& lv = P.lv[l];
-    const int n = lv.n;
+    const RpnImageLevel il = rpn_image_level(P, lv, b);
+    const int n = il.n;
     uint32_t* k0 = P.k0 + (size_t)b * P.ws_per_image + lv.ws_off;
     uint32_t* k1 = P.k1 + (size_t)b * P.ws_per_image + lv.ws_off;
     int* v0 = P.v0 + (size_t)b * P.ws_per_image + lv.ws_off;
@@ -504,7 +532,7 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
                 k[j] = 0u;
                 if (valid[j]) {
                     const int a = i % lv.A, cell = i / lv.A;
-                    k[j] = float_desc_key(base[(size_t)cell * lv.ch_stride + a]);
+                    k[j] = float_desc_key(base[rpn_canvas_cell(cell, il.w, lv.W) * lv.ch_stride + a]);
                 }
             }
     #pragma unroll
@@ -610,7 +638,10 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
     float4* cand = P.cand + ((size_t)b * P.num_levels + l) * P.pre_nms;
     float* cscore = P.cand_score + ((size_t)b * P.num_levels + l) * P.pre_nms;
     int nc = 0;
-    const float min_size = P.min_size * P.scaling_factor;
+    // clip and centre filter against this image's network-input size
+    const ImageInfo img = image_info(P.im_info, b, 1, (int)P.im_h, (int)P.im_w, P.scaling_factor);
+    const float im_h = (float)img.h, im_w = (float)img.w;
+    const float min_size = P.min_size * img.scale;
     for (int base_i = 0; base_i < K; base_i += blockDim.x) {
         const int i = base_i + threadIdx.x;
         bool keep = false;
@@ -620,17 +651,18 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
             const int idx = vs[i];
             if (P.dbg_order) P.dbg_order[((size_t)b * P.num_levels + l) * P.pre_nms + i] = idx;
             const int a = idx % lv.A, cell = idx / lv.A;
-            const int x = cell % lv.W, y = cell / lv.W;
+            const int x = cell % il.w, y = cell / il.w;
+            const size_t ccell = (size_t)y * lv.W + x;
             const float sx = (float)x * lv.stride, sy = (float)y * lv.stride;
             const float4 anc = make_float4(lv.anchors[a * 4 + 0] + sx, lv.anchors[a * 4 + 1] + sy, lv.anchors[a * 4 + 2] + sx,
                                            lv.anchors[a * 4 + 3] + sy);
-            const float* d = base + (size_t)cell * lv.ch_stride + lv.A + a * 4;
-            sc = base[(size_t)cell * lv.ch_stride + a];
-            box = clip_box(decode_box(anc, d[0], d[1], d[2], d[3]), P.im_w - 1.f, P.im_h - 1.f);
+            const float* d = base + ccell * lv.ch_stride + lv.A + a * 4;
+            sc = base[ccell * lv.ch_stride + a];
+            box = clip_box(decode_box(anc, d[0], d[1], d[2], d[3]), im_w - 1.f, im_h - 1.f);
             // filter_boxes (:151-163)
             const float ws = __fadd_rn(__fsub_rn(box.z, box.x), 1.f), hs = __fadd_rn(__fsub_rn(box.w, box.y), 1.f);
             const float xc = __fadd_rn(box.x, __fdiv_rn(ws, 2.f)), yc = __fadd_rn(box.y, __fdiv_rn(hs, 2.f));
-            keep = (ws >= min_size) && (hs >= min_size) && (xc < P.im_w) && (yc < P.im_h);
+            keep = (ws >= min_size) && (hs >= min_size) && (xc < im_w) && (yc < im_h);
         }
         int tot;
         const int r = block_rank(keep, scratch, &tot);
@@ -875,6 +907,7 @@ struct DetParams {
     const float* bbox;        // [B*R, 4*NC]
     int B, R, NC;
     float scaling_factor, im_h, im_w;      // original image size = network size / scaling_factor
+    const float* im_info;                  // per-image scale and original size (image_info), null = the scalars above
     float wx, wy, ww, wh;                  // bbox_reg_weights (10,10,5,5)
     float score_thresh, nms_thresh;
     int max_dets, out_cap;                 // 100, and the padded capacity of the outputs (>= max_dets)
@@ -902,6 +935,7 @@ static __global__ void __launch_bounds__(256) det_class_kernel(const __grid_cons
     __shared__ int scratch[33];
     const int j = blockIdx.x + 1, b = blockIdx.y;
     const int R = P.roi_counts ? min(P.roi_counts[b], P.R) : P.R;
+    const ImageInfo img = image_info(P.im_info, b, 1, 0, 0, P.scaling_factor, P.im_h, P.im_w);
     unsigned char* flag = P.keep_flag + ((size_t)b * P.NC + j) * P.R;
     float4* dbox = P.dec_box + ((size_t)b * P.NC + j) * P.R;
     // candidates: score > thresh (strict, result_utils.py:127), ascending RoI order
@@ -943,11 +977,11 @@ static __global__ void __launch_bounds__(256) det_class_kernel(const __grid_cons
     for (int i = threadIdx.x; i < nc; i += blockDim.x) {
         const int ri = (int)(skey[i] & 0xffffffffu);
         const float* r = P.rois + ((size_t)b * P.R + ri) * 5;
-        const float4 box = make_float4(__fdiv_rn(r[1], P.scaling_factor), __fdiv_rn(r[2], P.scaling_factor),
-                                       __fdiv_rn(r[3], P.scaling_factor), __fdiv_rn(r[4], P.scaling_factor));
+        const float4 box = make_float4(__fdiv_rn(r[1], img.scale), __fdiv_rn(r[2], img.scale), __fdiv_rn(r[3], img.scale),
+                                       __fdiv_rn(r[4], img.scale));
         const float* d = P.bbox + ((size_t)b * P.R + ri) * 4 * P.NC + 4 * j;
         float4 o = decode_box(box, __fdiv_rn(d[0], P.wx), __fdiv_rn(d[1], P.wy), __fdiv_rn(d[2], P.ww), __fdiv_rn(d[3], P.wh));
-        o = clip_box(o, P.im_w - 1.f, P.im_h - 1.f);
+        o = clip_box(o, img.orig_w - 1.f, img.orig_h - 1.f);
         sbox[i] = o;
         dbox[ri] = o;
     }
@@ -1070,15 +1104,17 @@ static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_con
     if (threadIdx.x == 0) P.out_counts[b] = min(nout, P.out_cap);
 }
 
-// detections -> mask RoIs: boxes_final * scaling_factor, FPN level (eval_mask_FPN.ipynb cell 10; multilevel_rois.py:19-39)
+// detections -> mask RoIs: boxes_final * scaling_factor, FPN level (eval_mask_FPN.ipynb cell 10; multilevel_rois.py:19-39).
+// im_info (may be null): image b's own scaling factor (image_info)
 static __global__ void mask_rois_kernel(const float* __restrict__ boxes, const int* __restrict__ counts, int B, int cap, float scaling_factor,
-                                 int k_min, int k_max, float* __restrict__ rois5, int* __restrict__ levels) {
+                                 int k_min, int k_max, float* __restrict__ rois5, int* __restrict__ levels, const float* __restrict__ im_info) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B * cap) return;
     const int b = i / cap, d = i - b * cap;
     float* r = rois5 + (size_t)i * 5;
     r[0] = (float)b;
     if (d < counts[b]) {
+        scaling_factor = image_info(im_info, b, 1, 0, 0, scaling_factor).scale;
         const float* s = boxes + (size_t)i * 4;
         const float4 box = make_float4(__fmul_rn(s[0], scaling_factor), __fmul_rn(s[1], scaling_factor), __fmul_rn(s[2], scaling_factor),
                                        __fmul_rn(s[3], scaling_factor));

@@ -117,6 +117,9 @@ struct RoiLevels {
     int H[5], W[5];
     float scale[5];
     int num_levels;
+    // per-image sizes (image_info): the bounds of a RoI of image b are b's extent at the level's stride, not the canvas map.  Null = off.
+    const float* im_info = nullptr;
+    int stride[5] = {0, 0, 0, 0, 0};
 };
 
 // rois [R,5] (batch,x1,y1,x2,y2); level[R] (index into lv, or nullptr -> level 0); out [R,PH,PW,C].
@@ -138,13 +141,14 @@ static __global__ void __launch_bounds__(256) roi_align_nhwc_kernel(RoiLevels lv
         const int l = level ? level[n] : 0;
         const int H = lv.H[l], W = lv.W[l];
         const RoiGeom g = roi_geom(rois + (size_t)n * 5, 5, lv.scale[l], PH, PW, sampling_ratio);
+        const ImageInfo ext = image_info(lv.im_info, g.batch, lv.stride[l], H, W);     // sample bounds (H, W stay the row pitch)
         const int ny = PH * g.grid_h, nx = PW * g.grid_w;
         const bool tabled = (ny <= kMaxAxisSamples) && (nx <= kMaxAxisSamples);
         __syncthreads();
         if (tabled) {
             for (int i = threadIdx.x; i < ny + nx; i += blockDim.x) {
-                if (i < ny) ytab[i] = axis_tap(sample_coord(g.start_h, i / g.grid_h, g.bin_h, i % g.grid_h, g.grid_h), H);
-                else { const int k = i - ny; xtab[k] = axis_tap(sample_coord(g.start_w, k / g.grid_w, g.bin_w, k % g.grid_w, g.grid_w), W); }
+                if (i < ny) ytab[i] = axis_tap(sample_coord(g.start_h, i / g.grid_h, g.bin_h, i % g.grid_h, g.grid_h), ext.h);
+                else { const int k = i - ny; xtab[k] = axis_tap(sample_coord(g.start_w, k / g.grid_w, g.bin_w, k % g.grid_w, g.grid_w), ext.w); }
             }
         }
         __syncthreads();
@@ -195,9 +199,9 @@ static __global__ void __launch_bounds__(256) roi_align_nhwc_kernel(RoiLevels lv
             const int pw = bin % PW, ph = bin / PW;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int iy = 0; iy < g.grid_h; ++iy) {
-                const AxisTap ty = tabled ? ytab[ph * g.grid_h + iy] : axis_tap(sample_coord(g.start_h, ph, g.bin_h, iy, g.grid_h), H);
+                const AxisTap ty = tabled ? ytab[ph * g.grid_h + iy] : axis_tap(sample_coord(g.start_h, ph, g.bin_h, iy, g.grid_h), ext.h);
                 for (int ix = 0; ix < g.grid_w; ++ix) {
-                    const AxisTap tx = tabled ? xtab[pw * g.grid_w + ix] : axis_tap(sample_coord(g.start_w, pw, g.bin_w, ix, g.grid_w), W);
+                    const AxisTap tx = tabled ? xtab[pw * g.grid_w + ix] : axis_tap(sample_coord(g.start_w, pw, g.bin_w, ix, g.grid_w), ext.w);
                     if (ty.valid && tx.valid) {
                         const float w1 = __fmul_rn(ty.wl, tx.wl), w2 = __fmul_rn(ty.wl, tx.wh);
                         const float w3 = __fmul_rn(ty.wh, tx.wl), w4 = __fmul_rn(ty.wh, tx.wh);
@@ -264,9 +268,10 @@ static __global__ void __launch_bounds__(256) roi_align_fast_nhwc_kernel(RoiLeve
         const int l = level ? level[n] : 0;
         const int H = lv.H[l], W = lv.W[l];
         const RoiGeom g = roi_geom(rois + (size_t)n * 5, 5, lv.scale[l], PH, PW, 2);
+        const ImageInfo ext = image_info(lv.im_info, g.batch, lv.stride[l], H, W);     // sample bounds (H, W stay the row pitch)
         __syncthreads();
-        if (threadIdx.x < PH) ytab[threadIdx.x] = axis_bin2(g.start_h, threadIdx.x, g.bin_h, H);
-        else if (threadIdx.x >= 32 && threadIdx.x < 32 + PW) xtab[threadIdx.x - 32] = axis_bin2(g.start_w, threadIdx.x - 32, g.bin_w, W);
+        if (threadIdx.x < PH) ytab[threadIdx.x] = axis_bin2(g.start_h, threadIdx.x, g.bin_h, ext.h);
+        else if (threadIdx.x >= 32 && threadIdx.x < 32 + PW) xtab[threadIdx.x - 32] = axis_bin2(g.start_w, threadIdx.x - 32, g.bin_w, ext.w);
         __syncthreads();
         const float4* fb = reinterpret_cast<const float4*>(lv.feat[l] + (size_t)g.batch * H * W * C);
         float4* ob = reinterpret_cast<float4*>(out + (size_t)n * PH * PW * C);

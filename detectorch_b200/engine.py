@@ -68,6 +68,7 @@ def _bind_engine_api(L):
     L.dt_engine_param_count.restype, L.dt_engine_param_count.argtypes = ci, [vp]
     L.dt_engine_param_info.restype, L.dt_engine_param_info.argtypes = ci, [vp, ci, ctypes.c_char_p, ci, ctypes.POINTER(c64)]
     L.dt_engine_set_original_size.restype, L.dt_engine_set_original_size.argtypes = ci, [vp, cf, cf]
+    L.dt_engine_use_image_info.restype, L.dt_engine_use_image_info.argtypes = ci, [vp, ci]
     L.dt_engine_run.restype, L.dt_engine_run.argtypes = ci, [vp, vp, cf, ci, ci, vp]
     L.dt_engine_count_launches.restype, L.dt_engine_count_launches.argtypes = ci, [vp, ci, ci]
     L.dt_engine_profile.restype, L.dt_engine_profile.argtypes = ci, [vp, vp, cf, ci, ci, vp, vp, vp, vp, vp, ci]
@@ -255,6 +256,27 @@ class Engine:
 
     def set_original_size(self, h, w):
         self.L.dt_engine_set_original_size(self.h, float(h), float(w))
+
+    def set_image_info(self, net_hw, scaling_factors, orig_hw=None):
+        """Batch of differently-sized images on the engine's canvas: image b occupies the top-left net_hw[b] (multiples of 32, at most the
+        canvas) of its slot, with its own scaling factor and original size (default net / scaling_factor).  Each image's outputs then equal
+        a batch-1 run of that image at its own size.  The table is written on the current stream -- the one the next run() goes on -- so a
+        run still queued from before never sees it, and a captured graph replays with whatever table was written last.  The table stays
+        in use for every following run (forward-style stage runs included) until clear_image_info()."""
+        B = self.cfg.batch
+        net = torch.as_tensor(net_hw, dtype=torch.float64).reshape(-1, 2)
+        sf = torch.as_tensor(scaling_factors, dtype=torch.float64).reshape(-1)
+        orig = torch.zeros((B, 2), dtype=torch.float64) if orig_hw is None else torch.as_tensor(orig_hw, dtype=torch.float64).reshape(-1, 2)
+        if net.shape[0] != B or sf.numel() != B or orig.shape[0] != B:
+            raise ValueError("set_image_info: %d images in the engine batch" % B)
+        table = torch.cat([net, sf[:, None], orig], 1).float().pin_memory()
+        with torch.cuda.device(self.device):
+            self.buffer("im_info").copy_(table, non_blocking=True)      # the pinned block is not reused before the copy has run
+        _lib.check(self.L.dt_engine_use_image_info(self.h, 1), "dt_engine_use_image_info")
+
+    def clear_image_info(self):
+        """Back to whole-canvas images with the scalar scaling factor."""
+        _lib.check(self.L.dt_engine_use_image_info(self.h, 0), "dt_engine_use_image_info")
 
     def profile(self, image, scaling_factor=1.0, first=0, last=11):
         """One event-bracketed pass: list of (ms, algorithmic_flops, stage, block_n) per launch."""

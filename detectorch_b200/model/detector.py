@@ -368,25 +368,93 @@ class detector(torch.nn.Module):
         return eng.buffer("masks_full")[:n]
 
     # ------------------------------------------------------------------ fused batched path
-    def detect(self, images, scaling_factor=1.0, with_masks=None):
+    @staticmethod
+    def _image_table(B, Hc, Wc, scaling_factor, image_sizes, original_sizes):
+        """Host-side check of detect()'s per-image arguments -> (net_hw, scales, orig_hw) lists, or None when every image fills the canvas
+        and shares one scaling factor (the uniform path)."""
+        # one value (a float, or a one-element tensor as forward() accepts) is the uniform scaling factor
+        per_image_sf = (torch.is_tensor(scaling_factor) or isinstance(scaling_factor, (list, tuple, np.ndarray))) and np.size(
+            scaling_factor.detach().cpu().numpy() if torch.is_tensor(scaling_factor) else scaling_factor) != 1
+        if not per_image_sf and not isinstance(scaling_factor, (int, float)):
+            scaling_factor = float(np.asarray(scaling_factor.detach().cpu() if torch.is_tensor(scaling_factor) else scaling_factor).reshape(-1)[0])
+        if image_sizes is None and original_sizes is None and not per_image_sf:
+            return None
+        if per_image_sf:
+            sf = np.asarray(scaling_factor.detach().cpu() if torch.is_tensor(scaling_factor) else scaling_factor, dtype=np.float64).reshape(-1)
+            if sf.size != B:
+                raise ValueError("detect: %d scaling factors for %d images" % (sf.size, B))
+        else:
+            sf = np.full(B, float(scaling_factor))
+        if not np.all(np.isfinite(sf) & (sf > 0)):
+            raise ValueError("detect: scaling factors must be positive")
+        if image_sizes is None:
+            net = np.tile(np.array([[Hc, Wc]], dtype=np.float64), (B, 1))
+        else:
+            net = np.asarray(image_sizes.detach().cpu() if torch.is_tensor(image_sizes) else image_sizes, dtype=np.float64)
+            if net.ndim != 2 or net.shape != (B, 2):
+                raise ValueError("detect: image_sizes must be [%d, 2] (one (height, width) per image)" % B)
+            if not np.all((net > 0) & (net % 32 == 0)) or np.any(net[:, 0] > Hc) or np.any(net[:, 1] > Wc):
+                raise ValueError("detect: image sizes must be positive multiples of 32 within the %dx%d canvas" % (Hc, Wc))
+        if original_sizes is None:
+            orig = np.zeros((B, 2))                              # net / scaling_factor, like the uniform path
+        else:
+            orig = np.asarray(original_sizes.detach().cpu() if torch.is_tensor(original_sizes) else original_sizes, dtype=np.float64)
+            if orig.ndim != 2 or orig.shape != (B, 2):
+                raise ValueError("detect: original_sizes must be [%d, 2] (one (height, width) per image)" % B)
+            if not np.all(np.isfinite(orig) & (orig > 0)):
+                raise ValueError("detect: original sizes must be positive")
+        return net, sf, orig
+
+    def detect(self, images, scaling_factor=1.0, with_masks=None, image_sizes=None, original_sizes=None):
         """Fused path: images [B,3,H,W] -> dict of padded per-image detections (boxes [B,cap,4], scores, classes, counts,
         masks [B,cap,28,28] of the detected class).  No host synchronisation inside.
         `images` may live in (pinned) HOST memory: the upload then goes through two device staging buffers on a copy stream, so the
         H2D copy of call i+1 overlaps the compute of call i.  The returned tensors are views of engine buffers: read them (e.g. an
-        asynchronous copy to pinned memory on the current stream) before the next detect() on the same input shape."""
+        asynchronous copy to pinned memory on the current stream) before the next detect() on the same input shape.
+
+        Differently-sized images (FPN models): `images` is a canvas and image b occupies the top-left image_sizes[b] = (h, w) of its
+        slot -- its own im_list_to_blob(fpn_on=True) size, a multiple of 32 (utils.blob.images_to_batch builds such batches).
+        `scaling_factor` may then be one value per image, and original_sizes [B,2] gives each image's un-scaled size for the final clip
+        (default: size / scaling_factor).  Image b's results equal a batch-1 run of that image alone; the canvas outside the images is
+        ignored.  One captured graph serves every size mix on the same canvas."""
         if not self.use_rpn_head:
             raise RuntimeError("detect() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois)")
+        table = self._image_table(images.size(0), images.size(2), images.size(3), scaling_factor, image_sizes, original_sizes)
+        if table is not None and self.family != "fpn":
+            raise NotImplementedError("detect: per-image sizes and scaling factors are built for the FPN models only")
         eng = self.engine_for(images.size(0), images.size(2), images.size(3))
-        eng.last_scaling_factor = float(scaling_factor)
         eng.set_original_size(0, 0)          # clip to the network input / scaling_factor (a previous postprocess_output may have set an image size)
+        scaling_factor = float(scaling_factor) if table is None else 1.0      # with the table its per-image factors apply
+        eng.last_scaling_factor = scaling_factor
         with_masks = self.use_mask_head if with_masks is None else with_masks
         last = ST_MASK_OUT if with_masks else ST_DETECT
+        if table is not None:
+            eng.set_image_info(*table)       # on the current stream, after every run already queued there
+        try:
+            self._launch_detect(eng, images, scaling_factor, last, table is not None)
+        finally:
+            # The table is scoped to this launch: the engine is shared with forward() / postprocess_output / mask_head of the same input
+            # shape, which keep the batch-1 contract.  Launched kernels (and captured graphs) already hold what they read.
+            if table is not None:
+                eng.clear_image_info()
+        B, cap = images.size(0), eng.cfg.det_cap
+        # "range_flag" (int32 [1]) is non-zero if an activation left the fp16 range of the default kind::f16 convolutions: read it together
+        # with the results (no extra synchronisation here), or call engine_owning(out['boxes']).check_range()
+        out = {"boxes": eng.buffer("det_boxes"), "scores": eng.buffer("det_scores"), "classes": eng.buffer("det_classes"),
+               "counts": eng.buffer("det_counts"), "roi_idx": eng.buffer("det_roi_idx"), "range_flag": eng.buffer("range_flag")}
+        if with_masks:
+            m = eng.buffer("masks")
+            out["masks"] = m.view(B, cap, m.shape[-2], m.shape[-1])
+        return out
+
+    def _launch_detect(self, eng, images, scaling_factor, last, use_table):
         if not images.is_cuda:
             images = self._upload(eng, images)
             st = eng._stage_state
             # host input = fixed device staging buffers: the ~110 launches of the step are captured once per (buffer, scaling factor, stage
-            # range) in a CUDA graph (second call on; the first one runs eagerly and warms every kernel up) and replayed afterwards
-            key = (st["pending"], float(scaling_factor), last)
+            # range) in a CUDA graph (second call on; the first one runs eagerly and warms every kernel up) and replayed afterwards.  With
+            # per-image sizes the kernels read the table at run time: the key records only that it is in use, not its values.
+            key = (st["pending"], "image_info" if use_table else float(scaling_factor), last)
             g = st["graphs"].get(key)
             if g is None and st["seen"].get(key, 0) >= 1 and self.capture_graphs:
                 g = torch.cuda.CUDAGraph()
@@ -402,15 +470,6 @@ class detector(torch.nn.Module):
             st["pending"] = None
         else:
             eng.run(images.contiguous().float(), float(scaling_factor), ST_TRUNK, last)
-        B, cap = images.size(0), eng.cfg.det_cap
-        # "range_flag" (int32 [1]) is non-zero if an activation left the fp16 range of the default kind::f16 convolutions: read it together
-        # with the results (no extra synchronisation here), or call engine_owning(out['boxes']).check_range()
-        out = {"boxes": eng.buffer("det_boxes"), "scores": eng.buffer("det_scores"), "classes": eng.buffer("det_classes"),
-               "counts": eng.buffer("det_counts"), "roi_idx": eng.buffer("det_roi_idx"), "range_flag": eng.buffer("range_flag")}
-        if with_masks:
-            m = eng.buffer("masks")
-            out["masks"] = m.view(B, cap, m.shape[-2], m.shape[-1])
-        return out
 
     def _upload(self, eng, host_images):
         """Host -> device through two staging buffers and a dedicated copy stream (2-deep pipeline across successive detect() calls)."""

@@ -218,6 +218,15 @@ int dt_engine_param_count(dt_engine_t e);
 int dt_engine_param_info(dt_engine_t e, int i, char* name_out, int name_cap, int64_t* numel);
 /* original (un-scaled) image size used by the detection clip (result_utils.py:86); 0,0 = network size / scaling_factor */
 int dt_engine_set_original_size(dt_engine_t e, float orig_h, float orig_w);
+/* Batches of differently-sized images (FPN engine; returns 0 for C4).  The network input [batch,3,height,width] is then a canvas:
+ * image b occupies the top-left net_h x net_w of its slot (its own im_list_to_blob size, a multiple of 32 <= the canvas) and has its
+ * own scaling factor and original size.  The caller writes them into the engine buffer "im_info", float32 [batch, 5] =
+ * (net_h, net_w, scaling_factor, orig_h, orig_w), orig <= 0 meaning net / scaling_factor; what the canvas holds outside the images
+ * is ignored (NaN included).  Kernels read the table when they run, not when they are launched: a CUDA graph captured with the table
+ * on replays for any size mix; write it on the stream of the run, before the run.  Each image's outputs are bit-identical to a
+ * batch-1 run of that image at its own size; the scaling_factor argument of dt_engine_run is ignored while the table is on.
+ * enabled = 0 returns to whole-canvas images and the scalar scaling factor / dt_engine_set_original_size. */
+int dt_engine_use_image_info(dt_engine_t e, int enabled);
 /* stages: 0 trunk, 1 FPN, 2 RPN convs, 3 proposals, 4 collect, 5 RoIAlign(box), 6 box head, 7 detect (decode+NMS+limit),
  *         8 mask RoIs, 9 RoIAlign(mask), 10 mask convs, 11 mask output */
 int dt_engine_run(dt_engine_t e, const float* image_nchw, float scaling_factor, int first_stage, int last_stage, dt_stream_t stream);
