@@ -5,6 +5,9 @@
 // a static program of kernel launches over pre-built TMA descriptors, with zero host synchronisation
 // (the reference syncs >= 17 times per image, SURVEY.md 3.1).  Memory is supplied by the caller as two
 // flat device buffers (weights, workspace) so that the host language (PyTorch here) stays pure plumbing.
+// Both model families of the reference are built by the same code: FPN (R-50/101-FPN) and C4 (Fast / Faster / Mask R-CNN R-50/101-C4:
+// trunk to layer3, single-level RPN with 15 anchors, RoIAlign 14x14 with the adaptive sampling grid, the res5 head = layer4 + avgpool
+// per RoI, and the 'upshare' mask head that re-runs layer4 on the detections).  What differs between them is data (Family).
 #include <algorithm>
 #include <map>
 #include <string>
@@ -141,6 +144,22 @@ struct ParamSlot {
     bool loaded = false;
 };
 
+// element count of the tensor a parameter is loaded from
+long long param_numel(const ParamSlot& s) {
+    switch (s.kind) {
+        case PK_CONV_W: return (long long)s.d0 * s.d1 * s.d2 * s.d3;
+        case PK_FC6_W: return (long long)s.d0 * s.d1 * s.d2;
+        case PK_STEM_W:
+        case PK_ROWS_W: return (long long)s.d0 * s.d1;
+        case PK_DECONV_W: return 4ll * s.d0 * s.d1;
+        default: return s.d0;
+    }
+}
+
+// A conv's weight matrix, scale and shift (float offsets into the weight buffer) and its GEMM shape.  flop_cout / flop_cin are the
+// layer's own output channels and K per tap before the matrix is padded (what its algorithmic FLOPs count).
+struct ConvW { size_t w = 0, scale = 0, shift = 0; int cout = 0, cin = 0, k = 1, flop_cout = 0, flop_cin = 0; };
+
 struct Buf {
     size_t off = 0;      // byte offset in workspace
     size_t bytes = 0;
@@ -162,15 +181,52 @@ struct Op {
     int matrix = -1;
 };
 
+// one RoIAlign launch: n RoIs (on the level `levels` gives, or all on level 0 when it is null) -> out [n, res, res, ch]
+struct RoiPool { const char* rois; const char* levels; const char* out; int n, ch, res, sampling; bool fast; };
+
+// What the FPN and C4 families build differently.  Level l is the map at stride 2^l (C2..C5, P2..P6); LH / LW[l - 2] is its size.
+struct Family {
+    bool c4;
+    const char* feat;        // the maps the RPN and RoIAlign read: "P" (FPN P2..P6) or "C" (C4)
+    int lv_min, lv_max;      // RoI levels (collect, RoIAlign, mask RoIs): FPN 2..5, C4 4
+    int rpn_levels;          // RPN levels from lv_min: FPN 5 (P2..P6), C4 1
+    int rpn_ch, anchors;     // RPN conv width, anchors per position
+    int box_feat;            // input width of the class / box head: FPN fc7, C4 the pooled res5 output
+    int mask_in, mask_res;   // mask head: deconv input channels, mask resolution
+    RoiPool box_pool, mask_pool;
+};
+
+Family family_of(const dt_engine_config& c) {
+    Family f;
+    f.c4 = c.model_type == 1;
+    const int R = c.batch * c.post_nms_top_n, D = c.batch * c.det_cap;
+    if (f.c4) {
+        // 15 anchors on the one 1024-channel C4 map; RoIAlign always runs the exact kernel with the adaptive sampling grid (ratio 0)
+        f.feat = "C"; f.lv_min = f.lv_max = 4; f.rpn_levels = 1; f.rpn_ch = 1024; f.anchors = 15;
+        f.box_feat = 2048; f.mask_in = 2048; f.mask_res = 14;
+        f.box_pool = RoiPool{"rois", nullptr, "roi_feat", R, 1024, 14, 0, false};
+        f.mask_pool = RoiPool{"mask_rois", nullptr, "mask_feat", D, 1024, 14, 0, false};
+    } else {
+        f.feat = "P"; f.lv_min = 2; f.lv_max = 5; f.rpn_levels = 5; f.rpn_ch = 256; f.anchors = 3;
+        f.box_feat = 1024; f.mask_in = 256; f.mask_res = 28;
+        f.box_pool = RoiPool{"rois", "roi_levels", "roi_feat", R, 256, 7, 2, !c.exact_roialign};
+        f.mask_pool = RoiPool{"mask_rois", "mask_levels", "mask_feat", D, 256, 14, 2, !c.exact_roialign};
+    }
+    return f;
+}
+
 struct Engine;
 typedef cudaError_t (*StageFn)(Engine*, cudaStream_t);
 
 struct Engine {
     dt_engine_config cfg;
+    Family fam;
     // weights
     std::map<std::string, ParamSlot> params;
+    std::map<std::string, ConvW> convs;     // by layer: what the program's conv launches read
     size_t mat_floats = 0;      // hi-region floats (lo region has the same size)
     size_t vec_floats = 0;
+    size_t zeros = 0;           // vector-region offset of the zero shift (FPN: the second half of a K-split mask conv)
     float* wbase = nullptr;
     // workspace
     std::map<std::string, Buf> bufs;
@@ -188,7 +244,7 @@ struct Engine {
     int H1, W1, H2, W2;                 // stem out, pool out
     int Hp, Wp;                         // padded NHWC4 stem input
     bool stem_fused = true;
-    int LH[5], LW[5];                   // P2..P6
+    int LH[5], LW[5];                   // levels 2..6
     RpnParams rpn;
     CollectParams col;
     DetParams det;
@@ -226,14 +282,12 @@ struct Engine {
 };
 
 // ---- parameter table ---------------------------------------------------------------------------
-size_t add_mat(Engine* e, const std::string& name, ParamKind kind, int rows_total, int K, int d0, int d1, int d2, int d3, int row_off = 0) {
+size_t add_mat(Engine* e, const std::string& name, ParamKind kind, int rows_total, int K, int d0, int d1, int d2, int d3) {
     ParamSlot s;
-    s.kind = kind; s.d0 = d0; s.d1 = d1; s.d2 = d2; s.d3 = d3; s.row_off = row_off; s.Kout = K;
-    if (row_off == 0) {
-        s.off = e->mat_floats;
-        e->mat_floats += align_up((size_t)rows_total * K, 64);
-        e->matrices.push_back(std::make_pair(s.off, e->mat_floats - s.off));
-    }
+    s.kind = kind; s.d0 = d0; s.d1 = d1; s.d2 = d2; s.d3 = d3; s.row_off = 0; s.Kout = K;
+    s.off = e->mat_floats;
+    e->mat_floats += align_up((size_t)rows_total * K, 64);
+    e->matrices.push_back(std::make_pair(s.off, e->mat_floats - s.off));
     e->params[name] = s;
     return s.off;
 }
@@ -246,98 +300,93 @@ size_t add_vec(Engine* e, const std::string& name, ParamKind kind, int n_total, 
     return s.off;
 }
 
-struct ConvW { size_t w, scale, shift; int cout, cin, k; };
+constexpr size_t kOnes = 0;     // the all-ones scale vector of the bias-only convs (2048 floats) opens the vector region
 
-void build_param_table(Engine* e, std::map<std::string, ConvW>* cw) {
-    const int NC = e->cfg.num_classes;
-    // shared "ones" scale vector for bias-only convs (max Cout 2048)
-    size_t ones = e->vec_floats; e->vec_floats += 2048;
-    (*cw)["__ones"] = ConvW{0, ones, 0, 2048, 0, 0};
-    size_t zeros = e->vec_floats; e->vec_floats += 2048;     // zero shift vector for the second half of a K-split convolution
-    (*cw)["__zeros"] = ConvW{0, 0, zeros, 2048, 0, 0};
-    // stem
-    {
-        ConvW c; c.cout = 64; c.cin = 160; c.k = 1;
-        c.w = add_mat(e, "model.conv1.weight", PK_STEM_W, 64, 160 + 224, 64, 147, 160, 0);   // im2col layout [64][160], then window layout [64][224]
-        c.scale = add_vec(e, "model.bn1.weight", PK_BN_SCALE, 64, 64);
-        c.shift = add_vec(e, "model.bn1.bias", PK_VEC, 64, 64);
-        (*cw)["stem"] = c;
+// conv + frozen BatchNorm (folded into the scale / shift)
+void bn_conv(Engine* e, const std::string& name, const std::string& bn, int cout, int cin, int k) {
+    ConvW c; c.cout = c.flop_cout = cout; c.cin = c.flop_cin = cin; c.k = k;
+    c.w = add_mat(e, name + ".weight", PK_CONV_W, cout, cin * k * k, cout, cin, k, k);
+    c.scale = add_vec(e, bn + ".weight", PK_BN_SCALE, cout, cout);
+    c.shift = add_vec(e, bn + ".bias", PK_VEC, cout, cout);
+    e->convs[name] = c;
+}
+// conv with a bias
+void bias_conv(Engine* e, const std::string& name, int cout, int cin, int k) {
+    ConvW c; c.cout = c.flop_cout = cout; c.cin = c.flop_cin = cin; c.k = k;
+    c.w = add_mat(e, name + ".weight", PK_CONV_W, cout, cin * k * k, cout, cin, k, k);
+    c.scale = kOnes;
+    c.shift = add_vec(e, name + ".bias", PK_VEC, cout, cout);
+    e->convs[name] = c;
+}
+// fully connected layer `name` (n outputs) as a 1x1 conv whose matrix has n + n2 rows padded to a multiple of 4 (the padding rows
+// stay zero); `name2` fills rows [n, n + n2) (the fused heads: objectness + box deltas, class scores + box deltas)
+void fc_rows(Engine* e, const std::string& key, const std::string& name, int n, int cin, const std::string& name2 = "", int n2 = 0) {
+    const int rows = (int)align_up((size_t)(n + n2), 4);
+    ConvW c; c.cout = rows; c.flop_cout = n + n2; c.cin = c.flop_cin = cin;
+    c.w = add_mat(e, name + ".weight", PK_ROWS_W, rows, cin, n, cin, 0, 0);
+    c.scale = kOnes;
+    c.shift = add_vec(e, name + ".bias", PK_VEC, rows, n);
+    if (n2) {
+        ParamSlot s = e->params[name + ".weight"];
+        s.d0 = n2; s.row_off = n;
+        e->params[name2 + ".weight"] = s;
+        add_vec(e, name2 + ".bias", PK_VEC, 0, n2, n, c.shift);
+    }
+    e->convs[key] = c;
+}
+
+void build_param_table(Engine* e) {
+    const dt_engine_config& c = e->cfg;
+    const Family& f = e->fam;
+    const int NC = c.num_classes;
+    e->vec_floats += 2048;      // kOnes
+    if (!f.c4) { e->zeros = e->vec_floats; e->vec_floats += 2048; }
+    {   // stem: im2col layout [64][160] (K zero-padded 147 -> 160), then window layout [64][224]
+        ConvW s; s.cout = s.flop_cout = 64; s.cin = 160; s.flop_cin = 147;
+        s.w = add_mat(e, "model.conv1.weight", PK_STEM_W, 64, 160 + 224, 64, 147, 160, 0);
+        s.scale = add_vec(e, "model.bn1.weight", PK_BN_SCALE, 64, 64);
+        s.shift = add_vec(e, "model.bn1.bias", PK_VEC, 64, 64);
+        e->convs["stem"] = s;
     }
     int inpl = 64;
-    for (int li = 1; li <= 4; ++li) {
+    for (int li = 1; li <= 4; ++li) {       // all four layers: the C4 family runs layer4 as its RoI heads
         const int planes = 64 << (li - 1);
-        for (int b = 0; b < e->cfg.arch_blocks[li - 1]; ++b) {
+        for (int b = 0; b < c.arch_blocks[li - 1]; ++b) {
             const std::string p = "model.layer" + std::to_string(li) + "." + std::to_string(b) + ".";
-            auto conv = [&](const std::string& cn, const std::string& bn, int cout, int cin, int k) {
-                ConvW c; c.cout = cout; c.cin = cin; c.k = k;
-                c.w = add_mat(e, p + cn + ".weight", PK_CONV_W, cout, cin * k * k, cout, cin, k, k);
-                c.scale = add_vec(e, p + bn + ".weight", PK_BN_SCALE, cout, cout);
-                c.shift = add_vec(e, p + bn + ".bias", PK_VEC, cout, cout);
-                (*cw)[p + cn] = c;
-            };
-            conv("conv1", "bn1", planes, inpl, 1);
-            conv("conv2", "bn2", planes, planes, 3);
-            conv("conv3", "bn3", planes * 4, planes, 1);
-            if (b == 0) conv("downsample.0", "downsample.1", planes * 4, inpl, 1);
+            bn_conv(e, p + "conv1", p + "bn1", planes, inpl, 1);
+            bn_conv(e, p + "conv2", p + "bn2", planes, planes, 3);
+            bn_conv(e, p + "conv3", p + "bn3", planes * 4, planes, 1);
+            if (b == 0) bn_conv(e, p + "downsample.0", p + "downsample.1", planes * 4, inpl, 1);
             inpl = planes * 4;
         }
     }
-    auto bias_conv = [&](const std::string& name, int cout, int cin, int k) {
-        ConvW c; c.cout = cout; c.cin = cin; c.k = k;
-        c.w = add_mat(e, name + ".weight", PK_CONV_W, cout, cin * k * k, cout, cin, k, k);
-        c.scale = ones;
-        c.shift = add_vec(e, name + ".bias", PK_VEC, cout, cout);
-        (*cw)[name] = c;
-    };
-    const int cins[4] = {256, 512, 1024, 2048};
-    for (int i = 0; i < 4; ++i) {
-        bias_conv("conv_body.fpn_lateral." + std::to_string(i), 256, cins[i], 1);
-        bias_conv("conv_body.fpn_output." + std::to_string(i), 256, 256, 3);
+    if (!f.c4) {
+        const int cins[4] = {256, 512, 1024, 2048};
+        for (int i = 0; i < 4; ++i) {
+            bias_conv(e, "conv_body.fpn_lateral." + std::to_string(i), 256, cins[i], 1);
+            bias_conv(e, "conv_body.fpn_output." + std::to_string(i), 256, 256, 3);
+        }
     }
-    if (e->cfg.use_rpn) bias_conv("rpn.conv_rpn", 256, 256, 3);
-    if (e->cfg.use_rpn) {   // fused RPN 1x1: rows [0,3) objectness, [3,15) deltas, row 15 zero
-        ConvW c; c.cout = 16; c.cin = 256; c.k = 1;
-        c.w = add_mat(e, "rpn.rpn_cls_prob.weight", PK_ROWS_W, 16, 256, 3, 256, 0, 0);
-        e->params["rpn.rpn_cls_prob.weight"].row_off = 0;
-        ParamSlot s = e->params["rpn.rpn_cls_prob.weight"];
-        s.d0 = 12; s.row_off = 3;
-        e->params["rpn.rpn_bbox_pred.weight"] = s;
-        c.scale = ones;
-        c.shift = add_vec(e, "rpn.rpn_cls_prob.bias", PK_VEC, 16, 3);
-        add_vec(e, "rpn.rpn_bbox_pred.bias", PK_VEC, 0, 12, 3, c.shift);
-        (*cw)["rpn.head"] = c;
+    if (c.use_rpn) {
+        bias_conv(e, "rpn.conv_rpn", f.rpn_ch, f.rpn_ch, 3);
+        fc_rows(e, "rpn.head", "rpn.rpn_cls_prob", f.anchors, f.rpn_ch, "rpn.rpn_bbox_pred", 4 * f.anchors);
     }
-    {   // box head
-        ConvW c; c.cout = 1024; c.cin = 256 * 49; c.k = 1;
-        c.w = add_mat(e, "conv_head.fc6.weight", PK_FC6_W, 1024, 256 * 49, 1024, 256, 49, 0);
-        c.scale = ones; c.shift = add_vec(e, "conv_head.fc6.bias", PK_VEC, 1024, 1024);
-        (*cw)["fc6"] = c;
-        ConvW d; d.cout = 1024; d.cin = 1024; d.k = 1;
-        d.w = add_mat(e, "conv_head.fc7.weight", PK_ROWS_W, 1024, 1024, 1024, 1024, 0, 0);
-        d.scale = ones; d.shift = add_vec(e, "conv_head.fc7.bias", PK_VEC, 1024, 1024);
-        (*cw)["fc7"] = d;
-        const int HN = (int)align_up((size_t)5 * NC, 4);
-        ConvW h; h.cout = HN; h.cin = 1024; h.k = 1;
-        h.w = add_mat(e, "classif_head.weight", PK_ROWS_W, HN, 1024, NC, 1024, 0, 0);
-        ParamSlot s = e->params["classif_head.weight"];
-        s.d0 = 4 * NC; s.row_off = NC;
-        e->params["bbox_head.weight"] = s;
-        h.scale = ones;
-        h.shift = add_vec(e, "classif_head.bias", PK_VEC, HN, NC);
-        add_vec(e, "bbox_head.bias", PK_VEC, 0, 4 * NC, NC, h.shift);
-        (*cw)["head"] = h;
+    if (!f.c4) {
+        ConvW c6; c6.cout = c6.flop_cout = 1024; c6.cin = c6.flop_cin = 256 * 49;
+        c6.w = add_mat(e, "conv_head.fc6.weight", PK_FC6_W, 1024, 256 * 49, 1024, 256, 49, 0);
+        c6.scale = kOnes; c6.shift = add_vec(e, "conv_head.fc6.bias", PK_VEC, 1024, 1024);
+        e->convs["fc6"] = c6;
+        fc_rows(e, "fc7", "conv_head.fc7", 1024, 1024);
     }
-    if (e->cfg.use_mask) {
-        for (int i = 1; i <= 4; ++i) bias_conv("mask_head.conv_head.fcn" + std::to_string(i), 256, 256, 3);
-        ConvW d; d.cout = 256; d.cin = 256; d.k = 1;
-        d.w = add_mat(e, "mask_head.transposed_conv.weight", PK_DECONV_W, 4 * 256, 256, 256, 256, 0, 0);
-        d.scale = ones; d.shift = add_vec(e, "mask_head.transposed_conv.bias", PK_VEC, 256, 256);
-        (*cw)["deconv"] = d;
-        const int MN = (int)align_up((size_t)NC, 4);
-        ConvW m; m.cout = MN; m.cin = 256; m.k = 1;
-        m.w = add_mat(e, "mask_head.classif_logits.weight", PK_ROWS_W, MN, 256, NC, 256, 0, 0);
-        m.scale = ones; m.shift = add_vec(e, "mask_head.classif_logits.bias", PK_VEC, MN, NC);
-        (*cw)["mask_logits"] = m;
+    fc_rows(e, "head", "classif_head", NC, f.box_feat, "bbox_head", 4 * NC);
+    if (c.use_mask) {
+        if (!f.c4)
+            for (int i = 1; i <= 4; ++i) bias_conv(e, "mask_head.conv_head.fcn" + std::to_string(i), 256, 256, 3);
+        ConvW d; d.cout = d.flop_cout = 256; d.cin = d.flop_cin = f.mask_in;
+        d.w = add_mat(e, "mask_head.transposed_conv.weight", PK_DECONV_W, 4 * 256, f.mask_in, f.mask_in, 256, 0, 0);
+        d.scale = kOnes; d.shift = add_vec(e, "mask_head.transposed_conv.bias", PK_VEC, 256, 256);
+        e->convs["deconv"] = d;
+        fc_rows(e, "mask_logits", "mask_head.classif_logits", NC, 256);
     }
 }
 
@@ -356,42 +405,53 @@ void add_buf(Engine* e, const std::string& name, std::initializer_list<long long
 
 int conv_out(int x, int k, int s, int p) { return (x + 2 * p - k) / s + 1; }
 
+// the buffers of ResNet layer li (add_layer) over N maps whose output is h x w, named pre + "b<block>.t1" / ".t2" / ".ds" / ".out"
+void plan_layer(Engine* e, const std::string& pre, int li, long long N, int h, int w) {
+    const int planes = 64 << (li - 1);
+    for (int b = 0; b < e->cfg.arch_blocks[li - 1]; ++b) {
+        const std::string p = pre + "b" + std::to_string(b);
+        add_buf(e, p + ".t1", {N, h, w, planes});
+        add_buf(e, p + ".t2", {N, h, w, planes});
+        if (b == 0) add_buf(e, p + ".ds", {N, h, w, planes * 4});
+        add_buf(e, p + ".out", {N, h, w, planes * 4});
+    }
+}
+std::string layer_out(const Engine* e, const std::string& pre, int li) { return pre + "b" + std::to_string(e->cfg.arch_blocks[li - 1] - 1) + ".out"; }
+
 void plan_buffers(Engine* e) {
     const dt_engine_config& c = e->cfg;
+    const Family& f = e->fam;
     const int B = c.batch;
     e->H1 = conv_out(c.height, 7, 2, 3); e->W1 = conv_out(c.width, 7, 2, 3);
     e->H2 = conv_out(e->H1, 3, 2, 1); e->W2 = conv_out(e->W1, 3, 2, 1);
     e->Hp = std::max(c.height + 6, 2 * e->H1 + 5); e->Wp = std::max(c.width + 6, 2 * e->W1 + 6);
     add_buf(e, "stem_x4", {B, e->Hp, e->Wp, 4});
-    add_buf(e, "stem_col", {(long long)B * e->H1 * e->W1, 160});     // fallback path only (see build_program)
+    add_buf(e, "stem_col", {(long long)B * e->H1 * e->W1, 160});     // fallback path only (see add_stem)
     add_buf(e, "c1", {B, e->H1, e->W1, 64});
     add_buf(e, "pool", {B, e->H2, e->W2, 64});
     int h = e->H2, w = e->W2;
-    for (int li = 1; li <= 4; ++li) {
-        const int planes = 64 << (li - 1);
+    for (int li = 1; li <= (f.c4 ? 3 : 4); ++li) {
         if (li > 1) { h = conv_out(h, 1, 2, 0); w = conv_out(w, 1, 2, 0); }
         e->LH[li - 1] = h; e->LW[li - 1] = w;
-        for (int b = 0; b < c.arch_blocks[li - 1]; ++b) {
-            const std::string p = "l" + std::to_string(li) + "b" + std::to_string(b);
-            add_buf(e, p + ".t1", {B, h, w, planes});
-            add_buf(e, p + ".t2", {B, h, w, planes});
-            if (b == 0) add_buf(e, p + ".ds", {B, h, w, planes * 4});
-            add_buf(e, p + ".out", {B, h, w, planes * 4});
+        const std::string pre = "l" + std::to_string(li);
+        plan_layer(e, pre, li, B, h, w);
+        e->bufs["C" + std::to_string(li + 1)] = e->bufs[layer_out(e, pre, li)];
+    }
+    if (!f.c4) {
+        e->LH[4] = (e->LH[3] - 1) / 2 + 1; e->LW[4] = (e->LW[3] - 1) / 2 + 1;    // max_pool2d(k=1,s=2)
+        for (int i = 0; i < 4; ++i) {
+            add_buf(e, "inner" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 256});
+            add_buf(e, "P" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 256});
         }
+        add_buf(e, "P6", {B, e->LH[4], e->LW[4], 256});
     }
-    e->LH[4] = (e->LH[3] - 1) / 2 + 1; e->LW[4] = (e->LW[3] - 1) / 2 + 1;    // max_pool2d(k=1,s=2)
-    for (int i = 0; i < 4; ++i) {
-        add_buf(e, "inner" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 256});
-        add_buf(e, "P" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 256});
-    }
-    add_buf(e, "P6", {B, e->LH[4], e->LW[4], 256});
-    const int L = 5, pre = c.pre_nms_top_n, post = c.post_nms_top_n;
-    if (c.use_rpn) {       // Fast R-CNN with the FPN body (eval_fast_FPN.ipynb) has no RPN: the caller fills `rois` / `roi_levels` / `roi_counts`
+    const int L = f.rpn_levels, pre = c.pre_nms_top_n, post = c.post_nms_top_n;
+    if (c.use_rpn) {       // Fast R-CNN (eval_fast*.ipynb) has no RPN: the caller fills `rois` / `roi_levels` / `roi_counts`
         long long anchors_total = 0;
-        for (int i = 0; i < 5; ++i) {
-            add_buf(e, "rpn_t" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 256});
-            add_buf(e, "rpn_out" + std::to_string(i + 2), {B, e->LH[i], e->LW[i], 16});
-            anchors_total += (long long)e->LH[i] * e->LW[i] * 3;
+        for (int l = f.lv_min; l < f.lv_min + L; ++l) {
+            add_buf(e, "rpn_t" + std::to_string(l), {B, e->LH[l - 2], e->LW[l - 2], f.rpn_ch});
+            add_buf(e, "rpn_out" + std::to_string(l), {B, e->LH[l - 2], e->LW[l - 2], e->convs["rpn.head"].cout});
+            anchors_total += (long long)e->LH[l - 2] * e->LW[l - 2] * f.anchors;
         }
         add_buf(e, "rpn_k0", {B, anchors_total}, 1); add_buf(e, "rpn_k1", {B, anchors_total}, 1);
         add_buf(e, "rpn_v0", {B, anchors_total}, 1); add_buf(e, "rpn_v1", {B, anchors_total}, 1);
@@ -404,11 +464,17 @@ void plan_buffers(Engine* e) {
         add_buf(e, "col_v0", {B, L * post}, 1); add_buf(e, "col_v1", {B, L * post}, 1);
     }
     add_buf(e, "rois", {B, post, 5}); add_buf(e, "roi_levels", {B, post}, 1); add_buf(e, "roi_counts", {B}, 1);
-    add_buf(e, "roi_feat", {(long long)B * post, 7, 7, 256});
-    add_buf(e, "fc6", {(long long)B * post, 1024}); add_buf(e, "fc7", {(long long)B * post, 1024});
-    const int NC = c.num_classes, HN = (int)align_up((size_t)5 * NC, 4);
-    add_buf(e, "head", {(long long)B * post, HN});
-    add_buf(e, "cls_prob", {(long long)B * post, NC}); add_buf(e, "bbox_pred", {(long long)B * post, 4 * NC});
+    const long long R = (long long)B * post;
+    add_buf(e, "roi_feat", {R, f.box_pool.res, f.box_pool.res, f.box_pool.ch});
+    if (f.c4) {
+        plan_layer(e, "r5", 4, R, 7, 7);
+        add_buf(e, "pooled", {R, 2048});
+    } else {
+        add_buf(e, "fc6", {R, 1024}); add_buf(e, "fc7", {R, 1024});
+    }
+    const int NC = c.num_classes;
+    add_buf(e, "head", {R, e->convs["head"].cout});
+    add_buf(e, "cls_prob", {R, NC}); add_buf(e, "bbox_pred", {R, 4 * NC});
     // detection
     const int cap = c.det_cap;
     add_buf(e, "det_flag", {B, NC, post}, 2, 1);
@@ -418,16 +484,20 @@ void plan_buffers(Engine* e) {
     add_buf(e, "det_boxes", {B, cap, 4}); add_buf(e, "det_scores", {B, cap}); add_buf(e, "det_classes", {B, cap}, 1);
     add_buf(e, "det_roi_idx", {B, cap}, 1); add_buf(e, "det_counts", {B}, 1);
     add_buf(e, "range_flag", {1}, 1);     // raised by a kind::f16 conv when an activation does not fit fp16
-    add_buf(e, "im_info", {B, 5});        // per-image (net_h, net_w, scaling_factor, orig_h, orig_w), read when dt_engine_use_image_info is on
+    // per-image (net_h, net_w, scaling_factor, orig_h, orig_w), read when dt_engine_use_image_info is on (FPN only)
+    if (!f.c4) add_buf(e, "im_info", {B, 5});
     if (c.use_mask) {
         const long long D = (long long)B * cap;
+        const int M = f.mask_res;
         add_buf(e, "mask_rois", {D, 5}); add_buf(e, "mask_levels", {D}, 1);
-        add_buf(e, "mask_feat", {D, 14, 14, 256});
-        for (int i = 1; i <= 4; ++i) add_buf(e, "mask_c" + std::to_string(i), {D, 14, 14, 256});
-        add_buf(e, "mask_up", {D, 28, 28, 256});
-        add_buf(e, "mask_logits", {D, 28, 28, (long long)align_up((size_t)NC, 4)});
-        add_buf(e, "masks", {D, 28, 28});
-        add_buf(e, "masks_full", {D, NC, 28, 28});
+        add_buf(e, "mask_feat", {D, 14, 14, f.mask_pool.ch});
+        if (f.c4) plan_layer(e, "m5", 4, D, 7, 7);
+        else
+            for (int i = 1; i <= 4; ++i) add_buf(e, "mask_c" + std::to_string(i), {D, 14, 14, 256});
+        add_buf(e, "mask_up", {D, M, M, 256});
+        add_buf(e, "mask_logits", {D, M, M, e->convs["mask_logits"].cout});
+        add_buf(e, "masks", {D, M, M});
+        add_buf(e, "masks_full", {D, NC, M, M});
     }
 }
 
@@ -435,28 +505,39 @@ void plan_buffers(Engine* e) {
 enum Stage { ST_TRUNK = 0, ST_FPN = 1, ST_RPN = 2, ST_PROPOSALS = 3, ST_COLLECT = 4, ST_ROI_BOX = 5, ST_BOX_HEAD = 6, ST_DETECT = 7,
              ST_MASK_ROIS = 8, ST_MASK_ROI_FEAT = 9, ST_MASK_HEAD = 10, ST_MASK_OUT = 11, ST_COUNT = 12 };
 
+// the optional parts of a conv launch (ProgBuilder::conv); a call site sets the fields it uses
+struct ConvOpt {
+    int res_mode = RES_NONE;
+    const float* res = nullptr;                             // RES_TILE: added before the ReLU (the output's geometry)
+    const float* up = nullptr; int up_h = 0, up_w = 0;      // RES_UPSAMPLE2X: the coarser map, upsampled 2x and added
+    int sigmoid_ch = 0;                                     // output channels [0, sigmoid_ch) get a sigmoid (RPN objectness)
+    size_t w_off = 0;                                       // float offset of the weight sub-matrix (a deconv quadrant)
+    int out_h = 0, out_w = 0, out_step = 0, out_y0 = 0, out_x0 = 0;   // output remap (transposed conv, see ConvSpec)
+    bool precise = false;                                   // 64-wide tiles with 3 rotating main-term accumulators
+    int tap0 = 0, ntaps = 0;                                // K-split: only filter taps [tap0, tap0 + ntaps)
+    bool zero_shift = false;                                // add no shift (the other half of the K-split adds it)
+    bool planes_in = false, planes_out = false;             // fp16 hi/lo plane hand-over (kind::f16 only)
+};
+
 struct ProgBuilder {
     Engine* e;
-    std::map<std::string, ConvW>* cw;
     bool ok = true;
     int img_stride = 0;     // > 0: the following convs write image-shaped maps at this stride (masked per image when the table is on)
 
     void conv(int stage, const std::string& wname, const float* x, int N, int H, int W, int xstride, float* y, int ystride, int kpad,
-              int stride, bool relu, int res_mode = RES_NONE, const float* res = nullptr, const float* up = nullptr, int up_h = 0,
-              int up_w = 0, int sigmoid_ch = 0, size_t w_extra_off = 0, int out_h = 0, int out_w = 0, int out_step = 0, int oy = 0,
-              int ox = 0, int force_bn = 0, int tap0 = 0, int ntaps = 0, bool zero_shift = false, int planes_in = 0, int planes_out = 0) {
-        const ConvW& c = (*cw)[wname];
+              int stride, bool relu, const ConvOpt& o = ConvOpt()) {
+        const ConvW& c = e->convs[wname];
         ConvSpec s;
         memset(&s, 0, sizeof(s));
         s.x = x; s.N = N; s.H = H; s.W = W; s.Cin = c.cin; s.x_pix_stride = xstride;
         Op op;
         s.Cout = c.cout; s.kh = c.k; s.kw = c.k; s.pad = kpad; s.stride = stride;
-        s.shift = zero_shift ? e->wvec((*cw)["__zeros"].shift) : e->wvec(c.shift);
-        s.tap0 = tap0; s.ntaps = ntaps;
+        s.shift = e->wvec(o.zero_shift ? e->zeros : c.shift);
+        s.tap0 = o.tap0; s.ntaps = o.ntaps;
         if (e->cfg.conv_kind == 0) {
             // kind::f16 three-term product: fp16 halves of w * multiplier(matrix); the multiplier is undone through a per-op scale vector
             const size_t n16 = align_up((size_t)c.cout, 64);
-            op.matrix = e->matrix_of(c.w + w_extra_off);
+            op.matrix = e->matrix_of(c.w + o.w_off);
             if (op.matrix < 0 || e->scale16_used + n16 > Engine::kScale16Floats) {
                 ok = false;
                 fprintf(stderr, "[detectorch_b200] engine: scale16 arena / matrix lookup failed for %s\n", wname.c_str());
@@ -465,32 +546,25 @@ struct ProgBuilder {
             op.scale_src = e->wvec(c.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = c.cout;
             e->scale16_used += n16;
             s.kind = KIND_F16X3;
-            s.w_hi = e->whi16(c.w + w_extra_off); s.w_lo = e->wlo16(c.w + w_extra_off);
+            s.w_hi = e->whi16(c.w + o.w_off); s.w_lo = e->wlo16(c.w + o.w_off);
             s.scale = op.scale16;
             s.range_flag = e->buf<int>("range_flag");
         } else {
             s.kind = KIND_TF32X3;
-            s.w_hi = e->wmat(c.w + w_extra_off); s.w_lo = e->wlo(c.w + w_extra_off);
+            s.w_hi = e->wmat(c.w + o.w_off); s.w_lo = e->wlo(c.w + o.w_off);
             s.scale = e->wvec(c.scale);
         }
         s.y = y; s.y_pix_stride = ystride;
+        const int Ho = conv_out(H, c.k, stride, kpad), Wo = conv_out(W, c.k, stride, kpad);
         // fp16 hi/lo plane hand-over (kind::f16 only): the fp32 buffer of N*H*W*C floats holds the two fp16 planes back to back
-        if (planes_in && e->cfg.conv_kind == 0) s.x_lo = reinterpret_cast<const __half*>(x) + (size_t)N * H * W * c.cin;
-        if (planes_out && e->cfg.conv_kind == 0) {
-            const int Ho_ = (H + 2 * kpad - c.k) / stride + 1, Wo_ = (W + 2 * kpad - c.k) / stride + 1;
-            s.y_lo = reinterpret_cast<__half*>(y) + (size_t)N * Ho_ * Wo_ * c.cout;
-        }
-        s.out_h = out_h; s.out_w = out_w; s.out_step = out_step; s.out_y0 = oy; s.out_x0 = ox;
-        s.residual = res; s.res_pix_stride = c.cout; s.up_src = up; s.up_h = up_h; s.up_w = up_w;
-        s.res_mode = res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = sigmoid_ch; s.passes = e->cfg.passes; s.force_block_n = force_bn; s.precise = (force_bn == 128) ? 1 : 0;
+        if (o.planes_in && e->cfg.conv_kind == 0) s.x_lo = reinterpret_cast<const __half*>(x) + (size_t)N * H * W * c.cin;
+        if (o.planes_out && e->cfg.conv_kind == 0) s.y_lo = reinterpret_cast<__half*>(y) + (size_t)N * Ho * Wo * c.cout;
+        s.out_h = o.out_h; s.out_w = o.out_w; s.out_step = o.out_step; s.out_y0 = o.out_y0; s.out_x0 = o.out_x0;
+        s.residual = o.res; s.res_pix_stride = c.cout; s.up_src = o.up; s.up_h = o.up_h; s.up_w = o.up_w;
+        s.res_mode = o.res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = o.sigmoid_ch; s.passes = e->cfg.passes; s.precise = o.precise ? 1 : 0;
         s.im_stride = img_stride;
         op.stage = stage; op.kind = 0; op.fn = -1;
-        {
-            const int Ho = (H + 2 * kpad - c.k) / stride + 1, Wo = (W + 2 * kpad - c.k) / stride + 1;
-            const double cin_alg = (wname == "stem") ? 147.0 : (double)c.cin;   // the stem K is zero-padded 147 -> 160
-            const double cout_alg = (wname == "rpn.head") ? 15.0 : (wname == "head") ? 5.0 * e->cfg.num_classes : (wname == "mask_logits") ? (double)e->cfg.num_classes : (double)c.cout;
-            op.flops = 2.0 * (double)N * Ho * Wo * cout_alg * cin_alg * (ntaps > 0 ? ntaps : c.k * c.k);
-        }
+        op.flops = 2.0 * (double)N * Ho * Wo * c.flop_cout * c.flop_cin * (o.ntaps > 0 ? o.ntaps : c.k * c.k);
         if (!conv_build(s, &op.conv)) { ok = false; fprintf(stderr, "[detectorch_b200] engine: conv_build failed for %s\n", wname.c_str()); }
         e->ops.push_back(op);
     }
@@ -541,21 +615,22 @@ cudaError_t fn_p6(Engine* e, cudaStream_t s) {
 // (rpn_select_*_kernel, one CTA per 4096 anchors), then one CTA per (level, image) sorts the ~1000 selected candidates, decodes, clips,
 // filters and runs the NMS.  DT_RPN_SPLIT=0 keeps the whole level in that one CTA (the round-1 kernel; P2's 182 400 anchors were its long pole).
 // which of the two splits a proposal launch uses (also what dt_engine_count_launches reports before the first run)
-void rpn_modes(Engine* e, int levels) {
+void rpn_modes(Engine* e) {
     static int split = -1, nms_split = -1;
     if (split < 0) { const char* v = getenv("DT_RPN_SPLIT"); split = (v && v[0] == '0') ? 0 : 1; }
     if (nms_split < 0) { const char* v = getenv("DT_RPN_NMS_SPLIT"); nms_split = (v && v[0] == '0') ? 0 : 1; }
     RpnParams& P = e->rpn;
     int max_n = 0;
-    for (int l = 0; l < levels; ++l) max_n = std::max(max_n, P.lv[l].n);
+    for (int l = 0; l < P.num_levels; ++l) max_n = std::max(max_n, P.lv[l].n);
     P.split = (split && max_n <= kRpnChunk * kRpnMaxChunks) ? 1 : 0;
     P.nms_split = (nms_split && P.pre_nms <= 8192 && P.nms_thresh > 0.f) ? 1 : 0;
 }
-cudaError_t launch_proposals(Engine* e, cudaStream_t s, int levels) {
+cudaError_t fn_proposals(Engine* e, cudaStream_t s) {
     RpnParams& P = e->rpn;
+    const int levels = P.num_levels;
     P.scaling_factor = e->scaling_factor;
     P.im_info = e->im_info();
-    rpn_modes(e, levels);
+    rpn_modes(e);
     int max_n = 0;
     for (int l = 0; l < levels; ++l) max_n = std::max(max_n, P.lv[l].n);
     if (P.split) {
@@ -575,21 +650,26 @@ cudaError_t launch_proposals(Engine* e, cudaStream_t s, int levels) {
     }
     return cudaGetLastError();
 }
-cudaError_t fn_proposals(Engine* e, cudaStream_t s) { return launch_proposals(e, s, 5); }
 cudaError_t fn_collect(Engine* e, cudaStream_t s) {
     collect_kernel<<<e->cfg.batch, 1024, 0, s>>>(e->col);
     return cudaGetLastError();
 }
-cudaError_t fn_roi_box(Engine* e, cudaStream_t s) {
-    const int R = e->cfg.batch * e->cfg.post_nms_top_n;
+// per-image counts: padded rows carry zero boxes (collect_kernel) -> harmless, fully defined output
+cudaError_t roi_align(Engine* e, const RoiPool& a, cudaStream_t s) {
     e->roi_lv.im_info = e->im_info();
-    // per-image counts: padded rows carry zero boxes (collect_kernel) -> harmless, fully defined output
-    if (e->cfg.exact_roialign)
-        roi_align_nhwc_kernel<<<R < num_sms() * 64 ? R : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), nullptr, R, 256, 7, 7,
-                                                                          2, e->buf("roi_feat"));
+    const int* levels = a.levels ? e->buf<int>(a.levels) : nullptr;
+    const int grid = std::min(a.n, num_sms() * 64);
+    if (a.fast)
+        roi_align_fast_nhwc_kernel<<<grid, 256, 0, s>>>(e->roi_lv, e->buf(a.rois), levels, a.n, a.ch, a.res, a.res, e->buf(a.out));
     else
-        roi_align_fast_nhwc_kernel<<<R < num_sms() * 64 ? R : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("rois"), e->buf<int>("roi_levels"), R, 256, 7, 7,
-                                                                               e->buf("roi_feat"));
+        roi_align_nhwc_kernel<<<grid, 256, 0, s>>>(e->roi_lv, e->buf(a.rois), levels, nullptr, a.n, a.ch, a.res, a.res, a.sampling, e->buf(a.out));
+    return cudaGetLastError();
+}
+cudaError_t fn_roi_box(Engine* e, cudaStream_t s) { return roi_align(e, e->fam.box_pool, s); }
+cudaError_t fn_mask_roi_feat(Engine* e, cudaStream_t s) { return roi_align(e, e->fam.mask_pool, s); }
+cudaError_t fn_avgpool(Engine* e, cudaStream_t s) {
+    const int R = e->cfg.batch * e->cfg.post_nms_top_n;
+    avgpool_nhwc_kernel<<<grid_for((long long)R * 512), 256, 0, s>>>(e->buf(layer_out(e, "r5", 4)), R, 49, 2048, e->buf("pooled"));
     return cudaGetLastError();
 }
 cudaError_t fn_softmax(Engine* e, cudaStream_t s) {
@@ -611,132 +691,118 @@ cudaError_t fn_detect(Engine* e, cudaStream_t s) {
 }
 cudaError_t fn_mask_rois(Engine* e, cudaStream_t s) {
     const int n = e->cfg.batch * e->cfg.det_cap;
-    mask_rois_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->buf("det_boxes"), e->buf<int>("det_counts"), e->cfg.batch, e->cfg.det_cap, e->scaling_factor, 2, 5,
-                                                    e->buf("mask_rois"), e->buf<int>("mask_levels"), e->im_info());
-    return cudaGetLastError();
-}
-cudaError_t fn_mask_roi_feat(Engine* e, cudaStream_t s) {
-    const int D = e->cfg.batch * e->cfg.det_cap;
-    e->roi_lv.im_info = e->im_info();
-    if (e->cfg.exact_roialign)
-        roi_align_nhwc_kernel<<<D < num_sms() * 64 ? D : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), nullptr, D, 256, 14,
-                                                                          14, 2, e->buf("mask_feat"));
-    else
-        roi_align_fast_nhwc_kernel<<<D < num_sms() * 64 ? D : num_sms() * 64, 256, 0, s>>>(e->roi_lv, e->buf("mask_rois"), e->buf<int>("mask_levels"), D, 256, 14, 14,
-                                                                               e->buf("mask_feat"));
+    mask_rois_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->buf("det_boxes"), e->buf<int>("det_counts"), e->cfg.batch, e->cfg.det_cap, e->scaling_factor,
+                                                    e->fam.lv_min, e->fam.lv_max, e->buf("mask_rois"), e->buf<int>("mask_levels"), e->im_info());
     return cudaGetLastError();
 }
 cudaError_t fn_mask_out(Engine* e, cudaStream_t s) {
-    const int D = e->cfg.batch * e->cfg.det_cap, NC = e->cfg.num_classes;
-    const long long n = (long long)D * 28 * 28;
-    mask_select_kernel<<<grid_for(n), 256, 0, s>>>(e->buf("mask_logits"), e->buf<int>("det_classes"), D, 28, (int)align_up((size_t)NC, 4), NC,
-                                                  e->cfg.output_prob, e->buf("masks"), e->cfg.emit_full_masks ? e->buf("masks_full") : nullptr);
+    const int D = e->cfg.batch * e->cfg.det_cap, NC = e->cfg.num_classes, M = e->fam.mask_res;
+    mask_select_kernel<<<grid_for((long long)D * M * M), 256, 0, s>>>(e->buf("mask_logits"), e->buf<int>("det_classes"), D, M, (int)align_up((size_t)NC, 4), NC,
+                                                                    e->cfg.output_prob, e->buf("masks"), e->cfg.emit_full_masks ? e->buf("masks_full") : nullptr);
     return cudaGetLastError();
 }
 
-// generate_anchors.py:54-122 on the host (float64, np.round == rint half-to-even)
-void gen_anchors(double stride, double size, float* out /*3x4*/) {
+// generate_anchors.py:54-122 on the host (float64, np.round == rint half-to-even): ratio-major, size-minor rows
+void gen_anchors(double stride, const double* sizes, int nsizes, float* out) {
     const double ratios[3] = {0.5, 1.0, 2.0};
-    const double base = stride, cx = 0.5 * (base - 1), area = base * base;
+    const double cx = 0.5 * (stride - 1), area = stride * stride;
+    int row = 0;
     for (int r = 0; r < 3; ++r) {
         const double wr = nearbyint(sqrt(area / ratios[r]));
         const double hr = nearbyint(wr * ratios[r]);
-        const double sc = size / stride;
-        const double ws = wr * sc, hs = hr * sc;
-        out[r * 4 + 0] = (float)(cx - 0.5 * (ws - 1)); out[r * 4 + 1] = (float)(cx - 0.5 * (hs - 1));
-        out[r * 4 + 2] = (float)(cx + 0.5 * (ws - 1)); out[r * 4 + 3] = (float)(cx + 0.5 * (hs - 1));
+        for (int s = 0; s < nsizes; ++s, ++row) {
+            const double sc = sizes[s] / stride, ws = wr * sc, hs = hr * sc;
+            out[row * 4 + 0] = (float)(cx - 0.5 * (ws - 1)); out[row * 4 + 1] = (float)(cx - 0.5 * (hs - 1));
+            out[row * 4 + 2] = (float)(cx + 0.5 * (ws - 1)); out[row * 4 + 3] = (float)(cx + 0.5 * (hs - 1));
+        }
     }
 }
 
-bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
+// the stem (detector.py:170-172): the fused-window conv over the packed image, or im2col + GEMM when stem_im2col asks for it or the
+// driver rejects the overlapping-stride map.  f16: the fused stem runs the kind::f16 product (else 3xTF32 from the fp32 weights).
+void add_stem(ProgBuilder& pb, bool f16, int handover) {
+    Engine* e = pb.e;
     const dt_engine_config& c = e->cfg;
     const int B = c.batch;
-    ProgBuilder pb{e, cw};
-    // ---- trunk (detector.py:170-183)
-    {
-        // fused-window stem (no im2col buffer); falls back to im2col + GEMM if the driver rejects the overlapping-stride map
-        const ConvW& sw = (*cw)["stem"];
-        Op op;
-        op.stage = ST_TRUNK; op.kind = 0; op.fn = -1;
-        op.flops = 2.0 * (double)B * e->H1 * e->W1 * 64.0 * 147.0;
-        bool stem_planes = false;
-        if (c.stem_im2col) {
-            e->stem_fused = false;
-        } else if (c.conv_kind == 0) {
-            op.matrix = e->matrix_of(sw.w);
-            op.scale_src = e->wvec(sw.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = 64;
-            e->scale16_used += 64;
-            // plane_handover >= 3: the packed image arrives as two fp16 planes (the stem's converter warps -- 7 k-blocks of fp32 -> fp16
-            // splits per 64-wide tile -- were what bounded it)
-            stem_planes = c.plane_handover >= 3 && (e->Wp % 2) == 0;
-            e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w + 64 * 160), e->wlo16(sw.w + 64 * 160),
-                                            op.scale16, e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"),
-                                            stem_planes);
-            if (!e->stem_fused) { op.scale16 = nullptr; op.scale_src = nullptr; }
-        } else {
-            e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w + 64 * 160), e->wlo(sw.w + 64 * 160),
-                                            e->wvec(sw.scale), e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv);
-        }
-        if (e->stem_fused) {
-            pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
-            op.conv.p.im_stride = 2;        // c1 is image-shaped (the im2col stem's GEMM-shaped output is not: the pool bounds its reads)
-            e->ops.push_back(op);
-        } else {
-            if (!c.stem_im2col) fprintf(stderr, "[detectorch_b200] engine: fused stem descriptor rejected, using the im2col stem\n");
-            pb.fn(ST_TRUNK, fn_stem_im2col);
-            pb.conv(ST_TRUNK, "stem", e->buf("stem_col"), 1, 1, B * e->H1 * e->W1, 160, e->buf("c1"), 64, 0, 1, true);
-        }
+    const ConvW& sw = e->convs["stem"];
+    Op op;
+    op.stage = ST_TRUNK; op.kind = 0; op.fn = -1;
+    op.flops = 2.0 * (double)B * e->H1 * e->W1 * sw.flop_cout * sw.flop_cin;
+    bool stem_planes = false;
+    if (c.stem_im2col) {
+        e->stem_fused = false;
+    } else if (f16) {
+        op.matrix = e->matrix_of(sw.w);
+        op.scale_src = e->wvec(sw.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = 64;
+        e->scale16_used += 64;
+        // plane_handover >= 3: the packed image arrives as two fp16 planes (the stem's converter warps -- 7 k-blocks of fp32 -> fp16
+        // splits per 64-wide tile -- were what bounded it)
+        stem_planes = handover >= 3 && (e->Wp % 2) == 0;
+        e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w + 64 * 160), e->wlo16(sw.w + 64 * 160),
+                                        op.scale16, e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"),
+                                        stem_planes);
+        if (!e->stem_fused) { op.scale16 = nullptr; op.scale_src = nullptr; }
+    } else {
+        e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w + 64 * 160), e->wlo(sw.w + 64 * 160),
+                                        e->wvec(sw.scale), e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv);
     }
-    // plane_handover >= 4 (opt-in): the pooled map leaves as fp16 planes too (its two consumers -- conv1 and the downsample conv of the first
-    // bottleneck -- then load their operand tiles directly).  Measured twice, before and after the epilogue rewrite: the consumers gain 7 us
-    // each, the pool kernel loses 16 us -- no net gain, so the default hand-over level stays 3.
-    const int pool_planes = (c.conv_kind == 0 && c.plane_handover >= 4) ? 1 : 0;
-    pb.fn(ST_TRUNK, pool_planes ? fn_maxpool_planes : fn_maxpool);
-    const float* x = e->buf("pool");
-    int h = e->H2, w = e->W2, cin = 64;
-    for (int li = 1; li <= 4; ++li) {
-        const int planes = 64 << (li - 1);
-        pb.img_stride = 4 << (li - 1);
-        for (int b = 0; b < c.arch_blocks[li - 1]; ++b) {
-            const std::string p = "l" + std::to_string(li) + "b" + std::to_string(b);
-            const std::string wp = "model.layer" + std::to_string(li) + "." + std::to_string(b) + ".";
-            const int stride = (b == 0 && li > 1) ? 2 : 1;
-            const int ho = e->LH[li - 1], wo = e->LW[li - 1];
-            // conv1 -> conv2 hand-over as fp16 hi/lo planes: the 3x3 conv would otherwise re-convert every input element once per filter tap
-            // (the converter warps' fp32->fp16 packs are what bounds the 64/128-wide layers)
-            const int pl = c.plane_handover ? 1 : 0;
-            const int xin_planes = (li == 1 && b == 0) ? pool_planes : 0;
-            pb.conv(ST_TRUNK, wp + "conv1", x, B, h, w, cin, e->buf(p + ".t1"), planes, 0, stride, true, RES_NONE, nullptr, nullptr, 0, 0, 0, 0, 0, 0, 0, 0, 0,
-                    0, 0, 0, false, xin_planes, pl);
-            // conv2 -> conv3 the same way (plane_handover >= 2): conv3 is a 1x1 conv, so this saves one conversion per element, the converter
-            // warps' shared-memory round trip (16 KB read + 16 KB written per k-block) and their issue slots in the epilogue-bound conv3
-            const int pl2 = c.plane_handover >= 2 ? 1 : 0;
-            pb.conv(ST_TRUNK, wp + "conv2", e->buf(p + ".t1"), B, ho, wo, planes, e->buf(p + ".t2"), planes, 1, 1, true, RES_NONE, nullptr, nullptr, 0, 0, 0,
-                    0, 0, 0, 0, 0, 0, 0, 0, 0, false, pl, pl2);
-            const float* idt = x;
-            if (b == 0) {
-                pb.conv(ST_TRUNK, wp + "downsample.0", x, B, h, w, cin, e->buf(p + ".ds"), planes * 4, 0, stride, false, RES_NONE, nullptr, nullptr, 0, 0, 0,
-                        0, 0, 0, 0, 0, 0, 0, 0, 0, false, xin_planes, 0);
-                idt = e->buf(p + ".ds");
-            }
-            pb.conv(ST_TRUNK, wp + "conv3", e->buf(p + ".t2"), B, ho, wo, planes, e->buf(p + ".out"), planes * 4, 0, 1, true, RES_TILE, idt, nullptr, 0, 0, 0,
-                    0, 0, 0, 0, 0, 0, 0, 0, 0, false, pl2, 0);
-            x = e->buf(p + ".out");
-            h = ho; w = wo; cin = planes * 4;
-        }
-        e->bufs["C" + std::to_string(li + 1)] = e->bufs["l" + std::to_string(li) + "b" + std::to_string(c.arch_blocks[li - 1] - 1) + ".out"];
+    if (e->stem_fused) {
+        pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
+        op.conv.p.im_stride = 2;        // c1 is image-shaped (the im2col stem's GEMM-shaped output is not: the pool bounds its reads)
+        e->ops.push_back(op);
+    } else {
+        if (!c.stem_im2col) fprintf(stderr, "[detectorch_b200] engine: fused stem descriptor rejected, using the im2col stem\n");
+        pb.fn(ST_TRUNK, fn_stem_im2col);
+        pb.conv(ST_TRUNK, "stem", e->buf("stem_col"), 1, 1, B * e->H1 * e->W1, 160, e->buf("c1"), 64, 0, 1, true);
     }
-    // ---- FPN (detector.py:35-52)
+}
+
+// ResNet layer li (detector.py:183; the C4 res5 head: detector.py:136,191,217) over N maps of h x w, into the buffers
+// plan_layer(pre) made: bottlenecks 1x1 -> 3x3 -> 1x1 + identity (downsample in the first block, which has stride 2 unless li == 1).
+// handover: the plane_handover level inside each block (0 = none); x_planes: x arrives as fp16 planes.  Returns the output map and
+// leaves its size in h, w.
+const float* add_layer(ProgBuilder& pb, int stage, const std::string& pre, int li, const float* x, int N, int& h, int& w, int handover,
+                       bool x_planes) {
+    Engine* e = pb.e;
+    const int planes = 64 << (li - 1);
+    for (int b = 0; b < e->cfg.arch_blocks[li - 1]; ++b) {
+        const std::string p = pre + "b" + std::to_string(b);
+        const std::string wp = "model.layer" + std::to_string(li) + "." + std::to_string(b) + ".";
+        const int stride = (b == 0 && li > 1) ? 2 : 1, cin = e->convs[wp + "conv1"].cin;
+        const int ho = conv_out(h, 1, stride, 0), wo = conv_out(w, 1, stride, 0);
+        // conv1 -> conv2 hand-over as fp16 hi/lo planes: the 3x3 conv would otherwise re-convert every input element once per filter tap
+        // (the converter warps' fp32->fp16 packs are what bounds the 64/128-wide layers)
+        ConvOpt o1; o1.planes_in = b == 0 && x_planes; o1.planes_out = handover >= 1;
+        pb.conv(stage, wp + "conv1", x, N, h, w, cin, e->buf(p + ".t1"), planes, 0, stride, true, o1);
+        // conv2 -> conv3 the same way (plane_handover >= 2): conv3 is a 1x1 conv, so this saves one conversion per element, the converter
+        // warps' shared-memory round trip (16 KB read + 16 KB written per k-block) and their issue slots in the epilogue-bound conv3
+        ConvOpt o2; o2.planes_in = handover >= 1; o2.planes_out = handover >= 2;
+        pb.conv(stage, wp + "conv2", e->buf(p + ".t1"), N, ho, wo, planes, e->buf(p + ".t2"), planes, 1, 1, true, o2);
+        const float* idt = x;
+        if (b == 0) {
+            ConvOpt od; od.planes_in = x_planes;
+            pb.conv(stage, wp + "downsample.0", x, N, h, w, cin, e->buf(p + ".ds"), planes * 4, 0, stride, false, od);
+            idt = e->buf(p + ".ds");
+        }
+        ConvOpt o3; o3.res_mode = RES_TILE; o3.res = idt; o3.planes_in = handover >= 2;
+        pb.conv(stage, wp + "conv3", e->buf(p + ".t2"), N, ho, wo, planes, e->buf(p + ".out"), planes * 4, 0, 1, true, o3);
+        x = e->buf(p + ".out");
+        h = ho; w = wo;
+    }
+    return x;
+}
+
+// FPN (detector.py:35-52): 1x1 laterals top-down, each adding the coarser one upsampled 2x, then the 3x3 outputs and P6
+void add_fpn(ProgBuilder& pb) {
+    Engine* e = pb.e;
+    const int B = e->cfg.batch;
     const int cins[4] = {256, 512, 1024, 2048};
     for (int i = 3; i >= 0; --i) {
-        const std::string ln = "conv_body.fpn_lateral." + std::to_string(i);
         pb.img_stride = 4 << i;
-        const float* src = e->buf("C" + std::to_string(i + 2));
-        if (i == 3)
-            pb.conv(ST_FPN, ln, src, B, e->LH[i], e->LW[i], cins[i], e->buf("inner5"), 256, 0, 1, false);
-        else
-            pb.conv(ST_FPN, ln, src, B, e->LH[i], e->LW[i], cins[i], e->buf("inner" + std::to_string(i + 2)), 256, 0, 1, false, RES_UPSAMPLE2X,
-                    nullptr, e->buf("inner" + std::to_string(i + 3)), e->LH[i + 1], e->LW[i + 1]);
+        ConvOpt o;
+        if (i < 3) { o.res_mode = RES_UPSAMPLE2X; o.up = e->buf("inner" + std::to_string(i + 3)); o.up_h = e->LH[i + 1]; o.up_w = e->LW[i + 1]; }
+        pb.conv(ST_FPN, "conv_body.fpn_lateral." + std::to_string(i), e->buf("C" + std::to_string(i + 2)), B, e->LH[i], e->LW[i], cins[i],
+                e->buf("inner" + std::to_string(i + 2)), 256, 0, 1, false, o);
     }
     for (int i = 0; i < 4; ++i) {
         pb.img_stride = 4 << i;
@@ -744,128 +810,179 @@ bool build_program(Engine* e, std::map<std::string, ConvW>* cw) {
                 e->buf("P" + std::to_string(i + 2)), 256, 1, 1, false);
     }
     pb.fn(ST_FPN, fn_p6);
-    // ---- RPN head on P2..P6 (detector.py:251)
-    for (int i = 0; i < 5 && c.use_rpn; ++i) {
-        const std::string L = std::to_string(i + 2);
-        pb.img_stride = 4 << i;
-        pb.conv(ST_RPN, "rpn.conv_rpn", e->buf("P" + L), B, e->LH[i], e->LW[i], 256, e->buf("rpn_t" + L), 256, 1, 1, true);
-        pb.conv(ST_RPN, "rpn.head", e->buf("rpn_t" + L), B, e->LH[i], e->LW[i], 256, e->buf("rpn_out" + L), 16, 0, 1, false, RES_NONE, nullptr,
-                nullptr, 0, 0, 3);
+}
+
+// RPN head on every RPN level (detector.py:251), the proposals (generate_proposals.py) and collect (collect_and_distribute...py;
+// for one level it only formats the RoIs as [batch,x1,y1,x2,y2] rows, the scores being already descending)
+void add_rpn(ProgBuilder& pb) {
+    Engine* e = pb.e;
+    const dt_engine_config& c = e->cfg;
+    const Family& f = e->fam;
+    const int B = c.batch, A = f.anchors, rows = e->convs["rpn.head"].cout;
+    for (int l = f.lv_min; l < f.lv_min + f.rpn_levels; ++l) {
+        const std::string L = std::to_string(l);
+        pb.img_stride = 1 << l;
+        pb.conv(ST_RPN, "rpn.conv_rpn", e->buf(f.feat + L), B, e->LH[l - 2], e->LW[l - 2], f.rpn_ch, e->buf("rpn_t" + L), f.rpn_ch, 1, 1, true);
+        ConvOpt o; o.sigmoid_ch = A;
+        pb.conv(ST_RPN, "rpn.head", e->buf("rpn_t" + L), B, e->LH[l - 2], e->LW[l - 2], f.rpn_ch, e->buf("rpn_out" + L), rows, 0, 1, false, o);
     }
-    pb.img_stride = 0;      // everything below is RoI-shaped
-    // ---- proposals (generate_proposals.py) + collect (collect_and_distribute...py)
-    if (c.use_rpn) {
-        RpnParams& P = e->rpn;
-        memset(&P, 0, sizeof(P));
-        P.num_levels = 5; P.B = B;
-        P.pre_nms = c.pre_nms_top_n; P.post_nms = c.post_nms_top_n;
-        P.nms_thresh = c.rpn_nms_thresh; P.min_size = c.rpn_min_size; P.scaling_factor = 1.f;
-        P.im_h = (float)c.height; P.im_w = (float)c.width;
-        long long off = 0;
-        for (int i = 0; i < 5; ++i) {
-            RpnLevel& lv = P.lv[i];
-            lv.rpn_out = e->buf("rpn_out" + std::to_string(i + 2));
-            lv.H = e->LH[i]; lv.W = e->LW[i]; lv.A = 3; lv.ch_stride = 16;
-            lv.stride = (float)(4 << i);
-            gen_anchors((double)(4 << i), (double)(32 << i), lv.anchors);
-            lv.n = lv.H * lv.W * 3;
-            lv.ws_off = off;
-            off += lv.n;
-        }
-        P.ws_per_image = off;
-        P.k0 = e->buf<uint32_t>("rpn_k0"); P.k1 = e->buf<uint32_t>("rpn_k1");
-        P.v0 = e->buf<int>("rpn_v0"); P.v1 = e->buf<int>("rpn_v1");
-        P.cand = e->buf<float4>("rpn_cand"); P.cand_score = e->buf("rpn_cand_score");
-        P.out_props = e->buf("props"); P.out_scores = e->buf("prop_scores"); P.out_counts = e->buf<int>("prop_counts");
-        P.dbg_order = e->buf<int>("rpn_order");
-        P.sel_hist = e->buf<uint32_t>("rpn_sel_hist"); P.sel_chunk_counts = e->buf<int>("rpn_sel_cc"); P.sel_info = e->buf<int>("rpn_sel_info");
-        P.cand_counts = e->buf<int>("rpn_cand_counts"); P.nms_mask = e->buf<unsigned long long>("rpn_nms_mask"); P.nms_chunks = (c.pre_nms_top_n + 63) / 64;
-        pb.fn(ST_PROPOSALS, fn_proposals);
-        CollectParams& C = e->col;
-        memset(&C, 0, sizeof(C));
-        C.props = P.out_props; C.scores = P.out_scores; C.counts = P.out_counts;
-        C.B = B; C.L = 5; C.post_nms = c.post_nms_top_n; C.top_n = c.post_nms_top_n; C.k_min = 2; C.k_max = 5;
-        C.k0 = e->buf<uint32_t>("col_k0"); C.k1 = e->buf<uint32_t>("col_k1"); C.v0 = e->buf<int>("col_v0"); C.v1 = e->buf<int>("col_v1");
-        C.rois = e->buf("rois"); C.levels = e->buf<int>("roi_levels"); C.roi_counts = e->buf<int>("roi_counts");
-        pb.fn(ST_COLLECT, fn_collect);
+    RpnParams& P = e->rpn;
+    memset(&P, 0, sizeof(P));
+    P.num_levels = f.rpn_levels; P.B = B;
+    P.pre_nms = c.pre_nms_top_n; P.post_nms = c.post_nms_top_n;
+    P.nms_thresh = c.rpn_nms_thresh; P.min_size = c.rpn_min_size; P.scaling_factor = 1.f;
+    P.im_h = (float)c.height; P.im_w = (float)c.width;
+    long long off = 0;
+    for (int i = 0; i < f.rpn_levels; ++i) {
+        const int l = f.lv_min + i;
+        RpnLevel& lv = P.lv[i];
+        lv.rpn_out = e->buf("rpn_out" + std::to_string(l));
+        lv.H = e->LH[l - 2]; lv.W = e->LW[l - 2]; lv.A = A; lv.ch_stride = rows;
+        lv.stride = (float)(1 << l);
+        double sizes[5];        // A / 3 anchor sizes, doubling from 32 << i
+        for (int s = 0; s < A / 3; ++s) sizes[s] = (double)(32 << (i + s));
+        gen_anchors((double)(1 << l), sizes, A / 3, lv.anchors);
+        lv.n = lv.H * lv.W * A;
+        lv.ws_off = off;
+        off += lv.n;
     }
-    // ---- RoIAlign 7x7 over P2..P5 in collected order (detector.py:259-270)
-    e->roi_lv.num_levels = 4;
-    for (int i = 0; i < 4; ++i) {
-        e->roi_lv.feat[i] = e->buf("P" + std::to_string(i + 2));
-        e->roi_lv.H[i] = e->LH[i]; e->roi_lv.W[i] = e->LW[i];
-        e->roi_lv.scale[i] = 1.f / (float)(4 << i);
-        e->roi_lv.stride[i] = 4 << i;
-    }
-    pb.fn(ST_ROI_BOX, fn_roi_box);
-    // ---- box head (detector.py:61-64,277-284)
-    const int R = B * c.post_nms_top_n, NC = c.num_classes, HN = (int)align_up((size_t)5 * NC, 4);
-    pb.conv(ST_BOX_HEAD, "fc6", e->buf("roi_feat"), 1, 1, R, 49 * 256, e->buf("fc6"), 1024, 0, 1, true);
-    pb.conv(ST_BOX_HEAD, "fc7", e->buf("fc6"), 1, 1, R, 1024, e->buf("fc7"), 1024, 0, 1, true);
-    pb.conv(ST_BOX_HEAD, "head", e->buf("fc7"), 1, 1, R, 1024, e->buf("head"), HN, 0, 1, false);
-    pb.fn(ST_BOX_HEAD, fn_softmax);
-    // ---- detection post-processing (result_utils.py:76-168)
-    {
-        DetParams& D = e->det;
-        memset(&D, 0, sizeof(D));
-        D.rois = e->buf("rois"); D.roi_counts = e->buf<int>("roi_counts"); D.cls = e->buf("cls_prob"); D.bbox = e->buf("bbox_pred");
-        D.B = B; D.R = c.post_nms_top_n; D.NC = NC;
-        D.wx = 10.f; D.wy = 10.f; D.ww = 5.f; D.wh = 5.f;
-        D.score_thresh = c.score_thresh; D.nms_thresh = c.det_nms_thresh; D.max_dets = c.max_dets; D.out_cap = c.det_cap;
-        D.keep_flag = e->buf<unsigned char>("det_flag"); D.dec_box = e->buf<float4>("det_dec"); D.cls_counts = e->buf<int>("det_cls_counts");
-        D.k0 = e->buf<uint32_t>("det_k0"); D.k1 = e->buf<uint32_t>("det_k1"); D.v0 = e->buf<int>("det_v0"); D.v1 = e->buf<int>("det_v1");
-        D.out_boxes = e->buf("det_boxes"); D.out_scores = e->buf("det_scores"); D.out_classes = e->buf<int>("det_classes");
-        D.out_roi_idx = e->buf<int>("det_roi_idx"); D.out_counts = e->buf<int>("det_counts");
-        pb.fn(ST_DETECT, fn_detect);
-    }
-    // ---- mask head (detector.py:99-112)
-    if (c.use_mask) {
-        const int D = B * c.det_cap, MN = (int)align_up((size_t)NC, 4);
+    P.ws_per_image = off;
+    P.k0 = e->buf<uint32_t>("rpn_k0"); P.k1 = e->buf<uint32_t>("rpn_k1");
+    P.v0 = e->buf<int>("rpn_v0"); P.v1 = e->buf<int>("rpn_v1");
+    P.cand = e->buf<float4>("rpn_cand"); P.cand_score = e->buf("rpn_cand_score");
+    P.out_props = e->buf("props"); P.out_scores = e->buf("prop_scores"); P.out_counts = e->buf<int>("prop_counts");
+    P.dbg_order = e->buf<int>("rpn_order");
+    P.sel_hist = e->buf<uint32_t>("rpn_sel_hist"); P.sel_chunk_counts = e->buf<int>("rpn_sel_cc"); P.sel_info = e->buf<int>("rpn_sel_info");
+    P.cand_counts = e->buf<int>("rpn_cand_counts"); P.nms_mask = e->buf<unsigned long long>("rpn_nms_mask"); P.nms_chunks = (c.pre_nms_top_n + 63) / 64;
+    pb.fn(ST_PROPOSALS, fn_proposals);
+    CollectParams& C = e->col;
+    memset(&C, 0, sizeof(C));
+    C.props = P.out_props; C.scores = P.out_scores; C.counts = P.out_counts;
+    C.B = B; C.L = f.rpn_levels; C.post_nms = c.post_nms_top_n; C.top_n = c.post_nms_top_n; C.k_min = f.lv_min; C.k_max = f.lv_max;
+    C.k0 = e->buf<uint32_t>("col_k0"); C.k1 = e->buf<uint32_t>("col_k1"); C.v0 = e->buf<int>("col_v0"); C.v1 = e->buf<int>("col_v1");
+    C.rois = e->buf("rois"); C.levels = e->buf<int>("roi_levels"); C.roi_counts = e->buf<int>("roi_counts");
+    pb.fn(ST_COLLECT, fn_collect);
+}
+
+// detection post-processing (result_utils.py:76-168)
+void setup_detect(Engine* e) {
+    const dt_engine_config& c = e->cfg;
+    DetParams& D = e->det;
+    memset(&D, 0, sizeof(D));
+    D.rois = e->buf("rois"); D.roi_counts = e->buf<int>("roi_counts"); D.cls = e->buf("cls_prob"); D.bbox = e->buf("bbox_pred");
+    D.B = c.batch; D.R = c.post_nms_top_n; D.NC = c.num_classes;
+    D.wx = 10.f; D.wy = 10.f; D.ww = 5.f; D.wh = 5.f;
+    D.score_thresh = c.score_thresh; D.nms_thresh = c.det_nms_thresh; D.max_dets = c.max_dets; D.out_cap = c.det_cap;
+    D.keep_flag = e->buf<unsigned char>("det_flag"); D.dec_box = e->buf<float4>("det_dec"); D.cls_counts = e->buf<int>("det_cls_counts");
+    D.k0 = e->buf<uint32_t>("det_k0"); D.k1 = e->buf<uint32_t>("det_k1"); D.v0 = e->buf<int>("det_v0"); D.v1 = e->buf<int>("det_v1");
+    D.out_boxes = e->buf("det_boxes"); D.out_scores = e->buf("det_scores"); D.out_classes = e->buf<int>("det_classes");
+    D.out_roi_idx = e->buf<int>("det_roi_idx"); D.out_counts = e->buf<int>("det_counts");
+}
+
+// mask head (detector.py:99-112): RoIs from the detections, their 14x14 features, the FPN 4-conv tower or the C4 'upshare' head
+// (layer4 again, on the detections: detector.py:217-218), then the 2x deconv and the per-class logits
+void add_mask_head(ProgBuilder& pb) {
+    Engine* e = pb.e;
+    const dt_engine_config& c = e->cfg;
+    const Family& f = e->fam;
+    const int D = c.batch * c.det_cap, M = f.mask_res;
+    pb.fn(ST_MASK_ROIS, fn_mask_rois);
+    pb.fn(ST_MASK_ROI_FEAT, fn_mask_roi_feat);
+    const float* mx = e->buf("mask_feat");
+    bool precise = false;
+    if (f.c4) {
+        int h = 14, w = 14;
+        mx = add_layer(pb, ST_MASK_HEAD, "m5", 4, mx, D, h, w, 0, false);
+    } else {
         // The mask logits carry the tightest parity bar (1e-4 absolute) and sit behind four K = 2304 convolutions, where the tensor
         // core's truncating fp32 accumulate is the error floor.  precise_mask shortens the chains by SPLITTING K: each 3x3 convolution
         // runs as two launches over filter taps [0,5) and [5,9); the second adds the first's fp32 result in its epilogue (RES_TILE on the
         // output buffer itself, round-to-nearest) before the ReLU.  precise_mask = 2 instead runs 64-wide tiles with 3 rotating
         // main-term accumulators.
-        const int mbn = c.precise_mask == 2 ? 128 : 0;
-        pb.fn(ST_MASK_ROIS, fn_mask_rois);
-        pb.fn(ST_MASK_ROI_FEAT, fn_mask_roi_feat);
-        const float* mx = e->buf("mask_feat");
+        precise = c.precise_mask == 2;
         for (int i = 1; i <= 4; ++i) {
             const std::string wn = "mask_head.conv_head.fcn" + std::to_string(i);
             float* my = e->buf("mask_c" + std::to_string(i));
             if (c.precise_mask == 1) {
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, RES_NONE, nullptr, nullptr, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 5);
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, RES_TILE, my, nullptr, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 5, 4, true);
+                ConvOpt lo; lo.ntaps = 5;
+                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, lo);
+                ConvOpt hi; hi.res_mode = RES_TILE; hi.res = my; hi.tap0 = 5; hi.ntaps = 4; hi.zero_shift = true;
+                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, hi);
             } else {
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, RES_NONE, nullptr, nullptr, 0, 0, 0, 0, 0, 0, 0, 0, 0, mbn);
+                ConvOpt o; o.precise = precise;
+                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, o);
             }
             mx = my;
         }
-        for (int ij = 0; ij < 4; ++ij)     // ConvTranspose2d(2, stride 2) == 4 GEMMs scattered on the 2x grid
-            pb.conv(ST_MASK_HEAD, "deconv", mx, D, 14, 14, 256, e->buf("mask_up"), 256, 0, 1, true, RES_NONE, nullptr, nullptr, 0, 0, 0,
-                    (size_t)ij * 256 * 256, 28, 28, 2, ij / 2, ij % 2, mbn);
-        pb.conv(ST_MASK_HEAD, "mask_logits", e->buf("mask_up"), D, 28, 28, 256, e->buf("mask_logits"), MN, 0, 1, false);
-        pb.fn(ST_MASK_OUT, fn_mask_out);
     }
-    return pb.ok;
+    for (int ij = 0; ij < 4; ++ij) {     // ConvTranspose2d(2, stride 2) == 4 GEMMs scattered on the 2x grid
+        ConvOpt o;
+        o.w_off = (size_t)ij * 256 * f.mask_in;
+        o.out_h = o.out_w = M; o.out_step = 2; o.out_y0 = ij / 2; o.out_x0 = ij % 2;
+        o.precise = precise;
+        pb.conv(ST_MASK_HEAD, "deconv", mx, D, M / 2, M / 2, f.mask_in, e->buf("mask_up"), 256, 0, 1, true, o);
+    }
+    pb.conv(ST_MASK_HEAD, "mask_logits", e->buf("mask_up"), D, M, M, 256, e->buf("mask_logits"), e->convs["mask_logits"].cout, 0, 1, false);
+    pb.fn(ST_MASK_OUT, fn_mask_out);
 }
 
-#include "engine_c4.inc"
+bool build_program(Engine* e) {
+    const dt_engine_config& c = e->cfg;
+    const Family& f = e->fam;
+    const int B = c.batch;
+    ProgBuilder pb{e};
+    // ---- trunk (detector.py:170-183): to layer4 for FPN, to layer3 for C4 (which runs layer4 per RoI).  The C4 family always builds
+    // the fused stem from the fp32 weights and hands no fp16 planes over.
+    const int handover = f.c4 ? 0 : c.plane_handover;
+    add_stem(pb, !f.c4 && c.conv_kind == 0, handover);
+    // plane_handover >= 4 (opt-in): the pooled map leaves as fp16 planes too (its two consumers -- conv1 and the downsample conv of the first
+    // bottleneck -- then load their operand tiles directly).  Measured twice, before and after the epilogue rewrite: the consumers gain 7 us
+    // each, the pool kernel loses 16 us -- no net gain, so the default hand-over level stays 3.
+    const bool pool_planes = c.conv_kind == 0 && handover >= 4;
+    pb.fn(ST_TRUNK, pool_planes ? fn_maxpool_planes : fn_maxpool);
+    const float* x = e->buf("pool");
+    int h = e->H2, w = e->W2;
+    for (int li = 1; li <= (f.c4 ? 3 : 4); ++li) {
+        pb.img_stride = 4 << (li - 1);
+        x = add_layer(pb, ST_TRUNK, "l" + std::to_string(li), li, x, B, h, w, handover, li == 1 && pool_planes);
+    }
+    if (!f.c4) add_fpn(pb);
+    if (c.use_rpn) add_rpn(pb);
+    pb.img_stride = 0;      // everything below is RoI-shaped
+    // ---- RoIAlign in collected order (detector.py:259-270)
+    e->roi_lv.num_levels = f.lv_max - f.lv_min + 1;
+    for (int l = f.lv_min; l <= f.lv_max; ++l) {
+        const int i = l - f.lv_min;
+        e->roi_lv.feat[i] = e->buf(f.feat + std::to_string(l));
+        e->roi_lv.H[i] = e->LH[l - 2]; e->roi_lv.W[i] = e->LW[l - 2];
+        e->roi_lv.scale[i] = 1.f / (float)(1 << l);
+        e->roi_lv.stride[i] = 1 << l;
+    }
+    pb.fn(ST_ROI_BOX, fn_roi_box);
+    // ---- box head (detector.py:61-64,277-284; C4: the res5 head, detector.py:136,191,273)
+    const int R = B * c.post_nms_top_n;
+    if (f.c4) {
+        int rh = 14, rw = 14;
+        add_layer(pb, ST_BOX_HEAD, "r5", 4, e->buf("roi_feat"), R, rh, rw, 0, false);
+        pb.fn(ST_BOX_HEAD, fn_avgpool);
+    } else {
+        pb.conv(ST_BOX_HEAD, "fc6", e->buf("roi_feat"), 1, 1, R, 49 * 256, e->buf("fc6"), 1024, 0, 1, true);
+        pb.conv(ST_BOX_HEAD, "fc7", e->buf("fc6"), 1, 1, R, 1024, e->buf("fc7"), 1024, 0, 1, true);
+    }
+    pb.conv(ST_BOX_HEAD, "head", e->buf(f.c4 ? "pooled" : "fc7"), 1, 1, R, f.box_feat, e->buf("head"), e->convs["head"].cout, 0, 1, false);
+    pb.fn(ST_BOX_HEAD, fn_softmax);
+    setup_detect(e);
+    pb.fn(ST_DETECT, fn_detect);
+    if (c.use_mask) add_mask_head(pb);
+    return pb.ok;
+}
 
 int load_param(Engine* e, const std::string& name, const float* src, long long numel, cudaStream_t st) {
     auto it = e->params.find(name);
     if (it == e->params.end()) return 2;   // not a hot-path parameter (running stats, fc, duplicates): ignored
     ParamSlot& s = it->second;
     if (!e->wbase) { fprintf(stderr, "[detectorch_b200] engine: bind weights before loading parameters\n"); return 0; }
-    long long expect = 0;
-    switch (s.kind) {
-        case PK_CONV_W: expect = (long long)s.d0 * s.d1 * s.d2 * s.d3; break;
-        case PK_STEM_W: expect = (long long)s.d0 * s.d1; break;
-        case PK_FC6_W: expect = (long long)s.d0 * s.d1 * s.d2; break;
-        case PK_ROWS_W: expect = (long long)s.d0 * s.d1; break;
-        case PK_DECONV_W: expect = 4ll * s.d0 * s.d1; break;
-        default: expect = s.d0;
-    }
+    const long long expect = param_numel(s);
     if (expect != numel) {
         fprintf(stderr, "[detectorch_b200] engine: parameter %s has %lld elements, expected %lld\n", name.c_str(), numel, expect);
         return 0;
@@ -905,9 +1022,9 @@ dt_engine_t dt_engine_create(const dt_engine_config* cfg) {
     Engine* e = new Engine();
     e->cfg = *cfg;
     if (e->cfg.passes != 1) e->cfg.passes = 3;
-    std::map<std::string, ConvW> cw;
-    if (e->cfg.model_type == 1) { build_param_table_c4(e, &cw); plan_buffers_c4(e); }
-    else { build_param_table(e, &cw); plan_buffers(e); }
+    e->fam = family_of(e->cfg);
+    build_param_table(e);
+    plan_buffers(e);
     return e;
 }
 
@@ -931,20 +1048,13 @@ static int bind_impl(Engine* e, void* weights, void* workspace, cudaStream_t st,
     if (fresh) {
         DT_CHECK_CUDA(cudaMemsetAsync(weights, 0, (2 * e->mat_floats + e->vec_floats) * sizeof(float), st));
         // the shared all-ones scale vector sits at the start of the vector region
-        fill_kernel<<<8, 256, 0, st>>>(e->wvec(0), 2048, 1.f);
-        if (e->cfg.model_type != 1) fill_kernel<<<8, 256, 0, st>>>(e->wvec(2048), 2048, 0.f);
+        fill_kernel<<<8, 256, 0, st>>>(e->wvec(kOnes), 2048, 1.f);
         DT_CHECK_CUDA(cudaGetLastError());
     }
     e->ops.clear();
     e->scale16_used = 0;
     e->fns.clear();
-    std::map<std::string, ConvW> cw;
-    {   // rebuild the (deterministic) table to recover the ConvW offsets
-        Engine tmp;
-        tmp.cfg = e->cfg;
-        if (e->cfg.model_type == 1) build_param_table_c4(&tmp, &cw); else build_param_table(&tmp, &cw);
-    }
-    if (!(e->cfg.model_type == 1 ? build_program_c4(e, &cw) : build_program(e, &cw))) return 0;
+    if (!build_program(e)) return 0;
     apply_image_info(e);
     e->bound = true;
     return 1;
@@ -1020,17 +1130,7 @@ int dt_engine_param_info(dt_engine_t h, int i, char* name_out, int name_cap, int
     auto it = e->params.begin();
     std::advance(it, i);
     snprintf(name_out, name_cap, "%s", it->first.c_str());
-    const ParamSlot& s = it->second;
-    long long n = 0;
-    switch (s.kind) {
-        case PK_CONV_W: n = (long long)s.d0 * s.d1 * s.d2 * s.d3; break;
-        case PK_STEM_W: n = (long long)s.d0 * s.d1; break;
-        case PK_FC6_W: n = (long long)s.d0 * s.d1 * s.d2; break;
-        case PK_ROWS_W: n = (long long)s.d0 * s.d1; break;
-        case PK_DECONV_W: n = 4ll * s.d0 * s.d1; break;
-        default: n = s.d0;
-    }
-    *numel = n;
+    *numel = param_numel(it->second);
     return 1;
 }
 
@@ -1110,7 +1210,7 @@ int dt_engine_profile(dt_engine_t h, const float* image_nchw, float scaling_fact
 int dt_engine_count_launches(dt_engine_t h, int first_stage, int last_stage) {
     Engine* e = reinterpret_cast<Engine*>(h);
     int n = 0;
-    if (e->cfg.use_rpn) rpn_modes(e, e->rpn.num_levels);
+    if (e->cfg.use_rpn) rpn_modes(e);
     for (const Op& op : e->ops)
         if (op.stage >= first_stage && op.stage <= last_stage)
             n += (op.kind == 1 && e->fns[op.fn] == fn_detect) ? 2 : ((op.kind == 1 && op.stage == ST_PROPOSALS) ? ((e->rpn.split ? 5 : 1) + (e->rpn.nms_split ? 2 : 0)) : 1);
