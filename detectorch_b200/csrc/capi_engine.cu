@@ -40,15 +40,6 @@ __global__ void pack_conv_w_kernel(const float* __restrict__ src, int Cout, int 
         dst[i] = src[(((size_t)o * Cin + c) * kh + y) * kw + x];
     }
 }
-// rows [Cout][Kin] -> [Cout][Kout] zero padded (stem 147 -> 160, plain copies)
-__global__ void pack_rows_kernel(const float* __restrict__ src, int rows, int Kin, int Kout, float* __restrict__ dst) {
-    const long long total = (long long)rows * Kout;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int k = (int)(i % Kout);
-        const int r = (int)(i / Kout);
-        dst[i] = k < Kin ? src[(size_t)r * Kin + k] : 0.f;
-    }
-}
 // stem [64][3][7][7] -> [64][7 (ky)][32 (kx*4 + c; kx < 7, c < 3; rest 0)]  (fused-window stem, conv_build_stem)
 __global__ void pack_stem_window_kernel(const float* __restrict__ src, float* __restrict__ dst) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -243,7 +234,6 @@ struct Engine {
     // static geometry
     int H1, W1, H2, W2;                 // stem out, pool out
     int Hp, Wp;                         // padded NHWC4 stem input
-    bool stem_fused = true;
     int LH[5], LW[5];                   // levels 2..6
     RpnParams rpn;
     CollectParams col;
@@ -341,9 +331,9 @@ void build_param_table(Engine* e) {
     const int NC = c.num_classes;
     e->vec_floats += 2048;      // kOnes
     if (!f.c4) { e->zeros = e->vec_floats; e->vec_floats += 2048; }
-    {   // stem: im2col layout [64][160] (K zero-padded 147 -> 160), then window layout [64][224]
-        ConvW s; s.cout = s.flop_cout = 64; s.cin = 160; s.flop_cin = 147;
-        s.w = add_mat(e, "model.conv1.weight", PK_STEM_W, 64, 160 + 224, 64, 147, 160, 0);
+    {   // stem: the window layout [64][224] of conv_build_stem (pack_stem_window_kernel)
+        ConvW s; s.cout = s.flop_cout = 64; s.cin = s.flop_cin = 147;
+        s.w = add_mat(e, "model.conv1.weight", PK_STEM_W, 64, 224, 64, 147, 0, 0);
         s.scale = add_vec(e, "model.bn1.weight", PK_BN_SCALE, 64, 64);
         s.shift = add_vec(e, "model.bn1.bias", PK_VEC, 64, 64);
         e->convs["stem"] = s;
@@ -426,7 +416,6 @@ void plan_buffers(Engine* e) {
     e->H2 = conv_out(e->H1, 3, 2, 1); e->W2 = conv_out(e->W1, 3, 2, 1);
     e->Hp = std::max(c.height + 6, 2 * e->H1 + 5); e->Wp = std::max(c.width + 6, 2 * e->W1 + 6);
     add_buf(e, "stem_x4", {B, e->Hp, e->Wp, 4});
-    add_buf(e, "stem_col", {(long long)B * e->H1 * e->W1, 160});     // fallback path only (see add_stem)
     add_buf(e, "c1", {B, e->H1, e->W1, 64});
     add_buf(e, "pool", {B, e->H2, e->W2, 64});
     int h = e->H2, w = e->W2;
@@ -447,17 +436,18 @@ void plan_buffers(Engine* e) {
     }
     const int L = f.rpn_levels, pre = c.pre_nms_top_n, post = c.post_nms_top_n;
     if (c.use_rpn) {       // Fast R-CNN (eval_fast*.ipynb) has no RPN: the caller fills `rois` / `roi_levels` / `roi_counts`
-        long long anchors_total = 0;
+        long long anchors_total = 0, anchors_max = 0;
         for (int l = f.lv_min; l < f.lv_min + L; ++l) {
             add_buf(e, "rpn_t" + std::to_string(l), {B, e->LH[l - 2], e->LW[l - 2], f.rpn_ch});
             add_buf(e, "rpn_out" + std::to_string(l), {B, e->LH[l - 2], e->LW[l - 2], e->convs["rpn.head"].cout});
             anchors_total += (long long)e->LH[l - 2] * e->LW[l - 2] * f.anchors;
+            anchors_max = std::max(anchors_max, (long long)e->LH[l - 2] * e->LW[l - 2] * f.anchors);
         }
         add_buf(e, "rpn_k0", {B, anchors_total}, 1); add_buf(e, "rpn_k1", {B, anchors_total}, 1);
         add_buf(e, "rpn_v0", {B, anchors_total}, 1); add_buf(e, "rpn_v1", {B, anchors_total}, 1);
         add_buf(e, "rpn_cand", {B, L, pre, 4}); add_buf(e, "rpn_cand_score", {B, L, pre});
         add_buf(e, "rpn_order", {B, L, pre}, 1);
-        add_buf(e, "rpn_sel_hist", {B, L, 2, 2048}, 1); add_buf(e, "rpn_sel_cc", {B, L, kRpnMaxChunks}, 1); add_buf(e, "rpn_sel_info", {B, L, 4}, 1);
+        add_buf(e, "rpn_sel_hist", {B, L, 2, 2048}, 1); add_buf(e, "rpn_sel_cc", {B, L, (anchors_max + kRpnChunk - 1) / kRpnChunk}, 1); add_buf(e, "rpn_sel_info", {B, L, 4}, 1);
         add_buf(e, "rpn_cand_counts", {B, L}, 1); add_buf(e, "rpn_nms_mask", {B, L, pre, (pre + 63) / 64, 2}, 1);
         add_buf(e, "props", {B, L, post, 4}); add_buf(e, "prop_scores", {B, L, post}); add_buf(e, "prop_counts", {B, L}, 1);
         add_buf(e, "col_k0", {B, L * post}, 1); add_buf(e, "col_k1", {B, L * post}, 1);
@@ -577,11 +567,6 @@ struct ProgBuilder {
     }
 };
 
-cudaError_t fn_stem_im2col(Engine* e, cudaStream_t s) {
-    const long long n = (long long)e->cfg.batch * e->H1 * e->W1 * 40;
-    stem_im2col_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->H1, e->W1, e->buf("stem_col"), e->im_info());
-    return cudaGetLastError();
-}
 cudaError_t fn_stem_pack(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->Hp * e->Wp;
     stem_pack_nhwc4_kernel<<<grid_for(n), 256, 0, s>>>(e->image, e->cfg.batch, e->cfg.height, e->cfg.width, e->Hp, e->Wp, e->buf("stem_x4"), e->im_info());
@@ -612,40 +597,24 @@ cudaError_t fn_p6(Engine* e, cudaStream_t s) {
     return cudaGetLastError();
 }
 // Proposal generation: the keys / two-level radix select / ordered compaction of every (level, image) run at full-GPU width
-// (rpn_select_*_kernel, one CTA per 4096 anchors), then one CTA per (level, image) sorts the ~1000 selected candidates, decodes, clips,
-// filters and runs the NMS.  DT_RPN_SPLIT=0 keeps the whole level in that one CTA (the round-1 kernel; P2's 182 400 anchors were its long pole).
-// which of the two splits a proposal launch uses (also what dt_engine_count_launches reports before the first run)
-void rpn_modes(Engine* e) {
-    static int split = -1, nms_split = -1;
-    if (split < 0) { const char* v = getenv("DT_RPN_SPLIT"); split = (v && v[0] == '0') ? 0 : 1; }
-    if (nms_split < 0) { const char* v = getenv("DT_RPN_NMS_SPLIT"); nms_split = (v && v[0] == '0') ? 0 : 1; }
-    RpnParams& P = e->rpn;
-    int max_n = 0;
-    for (int l = 0; l < P.num_levels; ++l) max_n = std::max(max_n, P.lv[l].n);
-    P.split = (split && max_n <= kRpnChunk * kRpnMaxChunks) ? 1 : 0;
-    P.nms_split = (nms_split && P.pre_nms <= 8192 && P.nms_thresh > 0.f) ? 1 : 0;
-}
+// (rpn_select_*_kernel, one CTA per 4096 anchors), then one CTA per (level, image) sorts the ~1000 selected candidates, decodes, clips
+// and filters them; the NMS runs as the suppression bit-matrix on every SM (nms_mask_kernel) and a survivor walk per (level, image).
 cudaError_t fn_proposals(Engine* e, cudaStream_t s) {
     RpnParams& P = e->rpn;
     const int levels = P.num_levels;
     P.scaling_factor = e->scaling_factor;
     P.im_info = e->im_info();
-    rpn_modes(e);
-    int max_n = 0;
-    for (int l = 0; l < levels; ++l) max_n = std::max(max_n, P.lv[l].n);
-    if (P.split) {
-        cudaError_t err = cudaMemsetAsync(P.sel_hist, 0, (size_t)e->cfg.batch * levels * 4096 * sizeof(uint32_t), s);
-        if (err != cudaSuccess) return err;
-        const dim3 grid((max_n + kRpnChunk - 1) / kRpnChunk, levels, e->cfg.batch);
-        rpn_select_keys_kernel<<<grid, 1024, 0, s>>>(P);
-        rpn_select_hist2_kernel<<<grid, 1024, 0, s>>>(P);
-        rpn_select_count_kernel<<<grid, 1024, 0, s>>>(P);
-        rpn_select_scatter_kernel<<<grid, 1024, 0, s>>>(P);
-    }
+    cudaError_t err = cudaMemsetAsync(P.sel_hist, 0, (size_t)e->cfg.batch * levels * 4096 * sizeof(uint32_t), s);
+    if (err != cudaSuccess) return err;
+    const dim3 grid(P.sel_chunks, levels, e->cfg.batch);
+    rpn_select_keys_kernel<<<grid, 1024, 0, s>>>(P);
+    rpn_select_hist2_kernel<<<grid, 1024, 0, s>>>(P);
+    rpn_select_count_kernel<<<grid, 1024, 0, s>>>(P);
+    rpn_select_scatter_kernel<<<grid, 1024, 0, s>>>(P);
     rpn_proposals_kernel<<<dim3(levels, e->cfg.batch), 1024, 0, s>>>(P);
-    if (P.nms_split) {
-        // DT_RPN_NMS_SPLIT=0 keeps the NMS inside rpn_proposals_kernel (one CTA per (level, image) sweeping every candidate over the survivors)
-        rpn_nms_mask_kernel<<<dim3(P.nms_chunks, P.nms_chunks, levels * e->cfg.batch), 64, 0, s>>>(P);
+    if (P.nms_thresh > 0.f) {
+        nms_mask_kernel<<<dim3(P.nms_chunks, P.nms_chunks, levels * e->cfg.batch), 64, 0, s>>>(P.cand, P.cand_counts, P.pre_nms, P.nms_chunks,
+                                                                                            P.nms_thresh, P.nms_mask);
         rpn_nms_scan_kernel<<<dim3(levels, e->cfg.batch), 1024, 0, s>>>(P);
     }
     return cudaGetLastError();
@@ -718,8 +687,8 @@ void gen_anchors(double stride, const double* sizes, int nsizes, float* out) {
     }
 }
 
-// the stem (detector.py:170-172): the fused-window conv over the packed image, or im2col + GEMM when stem_im2col asks for it or the
-// driver rejects the overlapping-stride map.  f16: the fused stem runs the kind::f16 product (else 3xTF32 from the fp32 weights).
+// the stem (detector.py:170-172): the fused-window conv over the packed image.  f16: it runs the kind::f16 product (else 3xTF32 from
+// the fp32 weights).
 void add_stem(ProgBuilder& pb, bool f16, int handover) {
     Engine* e = pb.e;
     const dt_engine_config& c = e->cfg;
@@ -728,33 +697,24 @@ void add_stem(ProgBuilder& pb, bool f16, int handover) {
     Op op;
     op.stage = ST_TRUNK; op.kind = 0; op.fn = -1;
     op.flops = 2.0 * (double)B * e->H1 * e->W1 * sw.flop_cout * sw.flop_cin;
-    bool stem_planes = false;
-    if (c.stem_im2col) {
-        e->stem_fused = false;
-    } else if (f16) {
+    bool stem_planes = false, ok;
+    if (f16) {
         op.matrix = e->matrix_of(sw.w);
         op.scale_src = e->wvec(sw.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = 64;
         e->scale16_used += 64;
         // plane_handover >= 3: the packed image arrives as two fp16 planes (the stem's converter warps -- 7 k-blocks of fp32 -> fp16
         // splits per 64-wide tile -- were what bounded it)
         stem_planes = handover >= 3 && (e->Wp % 2) == 0;
-        e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w + 64 * 160), e->wlo16(sw.w + 64 * 160),
-                                        op.scale16, e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"),
-                                        stem_planes);
-        if (!e->stem_fused) { op.scale16 = nullptr; op.scale_src = nullptr; }
+        ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w), e->wlo16(sw.w), op.scale16, e->wvec(sw.shift),
+                             e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"), stem_planes);
     } else {
-        e->stem_fused = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w + 64 * 160), e->wlo(sw.w + 64 * 160),
-                                        e->wvec(sw.scale), e->wvec(sw.shift), e->buf("c1"), c.passes, &op.conv);
+        ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w), e->wlo(sw.w), e->wvec(sw.scale), e->wvec(sw.shift),
+                             e->buf("c1"), c.passes, &op.conv);
     }
-    if (e->stem_fused) {
-        pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
-        op.conv.p.im_stride = 2;        // c1 is image-shaped (the im2col stem's GEMM-shaped output is not: the pool bounds its reads)
-        e->ops.push_back(op);
-    } else {
-        if (!c.stem_im2col) fprintf(stderr, "[detectorch_b200] engine: fused stem descriptor rejected, using the im2col stem\n");
-        pb.fn(ST_TRUNK, fn_stem_im2col);
-        pb.conv(ST_TRUNK, "stem", e->buf("stem_col"), 1, 1, B * e->H1 * e->W1, 160, e->buf("c1"), 64, 0, 1, true);
-    }
+    if (!ok) { pb.ok = false; fprintf(stderr, "[detectorch_b200] engine: conv_build_stem failed\n"); return; }
+    pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
+    op.conv.p.im_stride = 2;        // c1 is an image-shaped map at stride 2 (masked per image when the table is on)
+    e->ops.push_back(op);
 }
 
 // ResNet layer li (detector.py:183; the C4 res5 head: detector.py:136,191,217) over N maps of h x w, into the buffers
@@ -853,6 +813,7 @@ void add_rpn(ProgBuilder& pb) {
     P.out_props = e->buf("props"); P.out_scores = e->buf("prop_scores"); P.out_counts = e->buf<int>("prop_counts");
     P.dbg_order = e->buf<int>("rpn_order");
     P.sel_hist = e->buf<uint32_t>("rpn_sel_hist"); P.sel_chunk_counts = e->buf<int>("rpn_sel_cc"); P.sel_info = e->buf<int>("rpn_sel_info");
+    P.sel_chunks = e->bufs["rpn_sel_cc"].dims[2];
     P.cand_counts = e->buf<int>("rpn_cand_counts"); P.nms_mask = e->buf<unsigned long long>("rpn_nms_mask"); P.nms_chunks = (c.pre_nms_top_n + 63) / 64;
     pb.fn(ST_PROPOSALS, fn_proposals);
     CollectParams& C = e->col;
@@ -989,12 +950,9 @@ int load_param(Engine* e, const std::string& name, const float* src, long long n
     }
     switch (s.kind) {
         case PK_CONV_W: pack_conv_w_kernel<<<grid_for(numel), 256, 0, st>>>(src, s.d0, s.d1, s.d2, s.d3, e->wmat(s.off)); break;
-        case PK_STEM_W:
-            pack_rows_kernel<<<grid_for((long long)s.d0 * s.d2), 256, 0, st>>>(src, s.d0, s.d1, s.d2, e->wmat(s.off));
-            pack_stem_window_kernel<<<(64 * 224 + 255) / 256, 256, 0, st>>>(src, e->wmat(s.off) + 64 * 160);
-            break;
+        case PK_STEM_W: pack_stem_window_kernel<<<(64 * 224 + 255) / 256, 256, 0, st>>>(src, e->wmat(s.off)); break;
         case PK_FC6_W: pack_fc6_kernel<<<grid_for(numel), 256, 0, st>>>(src, s.d0, s.d1, s.d2, e->wmat(s.off)); break;
-        case PK_ROWS_W: pack_rows_kernel<<<grid_for(numel), 256, 0, st>>>(src, s.d0, s.d1, s.d1, e->wmat(s.off) + (size_t)s.row_off * s.Kout); break;
+        case PK_ROWS_W: copy_kernel<<<grid_for(numel), 256, 0, st>>>(src, numel, e->wmat(s.off) + (size_t)s.row_off * s.Kout); break;
         case PK_DECONV_W: pack_deconv_kernel<<<grid_for(numel), 256, 0, st>>>(src, s.d0, s.d1, e->wmat(s.off)); break;
         case PK_BN_SCALE: bn_scale_kernel<<<(s.d0 + 255) / 256, 256, 0, st>>>(src, s.d0, e->wvec(s.off)); break;
         case PK_VEC: copy_kernel<<<grid_for(numel), 256, 0, st>>>(src, numel, e->wvec(s.off) + s.row_off); break;
@@ -1210,10 +1168,9 @@ int dt_engine_profile(dt_engine_t h, const float* image_nchw, float scaling_fact
 int dt_engine_count_launches(dt_engine_t h, int first_stage, int last_stage) {
     Engine* e = reinterpret_cast<Engine*>(h);
     int n = 0;
-    if (e->cfg.use_rpn) rpn_modes(e);
     for (const Op& op : e->ops)
         if (op.stage >= first_stage && op.stage <= last_stage)
-            n += (op.kind == 1 && e->fns[op.fn] == fn_detect) ? 2 : ((op.kind == 1 && op.stage == ST_PROPOSALS) ? ((e->rpn.split ? 5 : 1) + (e->rpn.nms_split ? 2 : 0)) : 1);
+            n += (op.kind == 1 && e->fns[op.fn] == fn_detect) ? 2 : ((op.kind == 1 && op.stage == ST_PROPOSALS) ? (e->rpn.nms_thresh > 0.f ? 7 : 5) : 1);
     return n;
 }
 

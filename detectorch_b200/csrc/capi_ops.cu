@@ -269,6 +269,7 @@ struct NmsWs {
     float4* sorted;
     unsigned long long* removed;
     int* flags;
+    int* count;          // the set size, for nms_mask_kernel (large sets)
 };
 __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 inline NmsWs carve_nms_ws(void* ws, int64_t n) {
@@ -281,165 +282,80 @@ inline NmsWs carve_nms_ws(void* ws, int64_t n) {
     w.v1 = (int*)p; p += n4;
     w.flags = (int*)p; p += n4;
     w.sorted = (float4*)p; p += align_up((size_t)n * 16, 256);
+    w.count = (int*)p; p += 256;
     w.removed = (unsigned long long*)p;
     return w;
+}
+
+// boxes sorted by descending score (ties: ascending index) into w.sorted, their original indices in w.v0; w.flags cleared
+__device__ void nms_sort_boxes(const float* __restrict__ dets, int n, const NmsWs& w, uint32_t* hist) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        w.k0[i] = float_desc_key(dets[(size_t)i * 5 + 4]);
+        w.v0[i] = i;
+        w.flags[i] = 0;
+    }
+    __syncthreads();
+    block_radix_sort_asc_u32(w.k0, w.v0, w.k1, w.v1, n, hist);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float* d = dets + (size_t)w.v0[i] * 5;
+        w.sorted[i] = make_float4(d[0], d[1], d[2], d[3]);
+    }
+}
+
+// flags (original index space) -> ascending kept indices
+__device__ void nms_compact(const int* flags, int n, long long* __restrict__ keep_out, int* __restrict__ num_keep) {
+    __shared__ int scratch[33];
+    int running = 0;
+    for (int base = 0; base < n; base += blockDim.x) {
+        const int i = base + threadIdx.x;
+        const bool f = i < n && flags[i];
+        int tot;
+        const int r = block_rank(f, scratch, &tot);
+        if (f) keep_out[running + r] = i;
+        running += tot;
+    }
+    if (threadIdx.x == 0) *num_keep = running;
 }
 
 __global__ void __launch_bounds__(1024) nms_single_kernel(const float* __restrict__ dets, int n, float thresh, NmsWs w,
                                                          long long* __restrict__ keep_out, int* __restrict__ num_keep) {
     __shared__ uint32_t hist[32 * 256];
     __shared__ NmsSmem nsm;
-    __shared__ int scan_warp[32];
-    __shared__ int running;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        w.k0[i] = float_desc_key(dets[(size_t)i * 5 + 4]);
-        w.v0[i] = i;
-        w.flags[i] = 0;
-    }
+    nms_sort_boxes(dets, n, w, hist);
     __syncthreads();
-    block_radix_sort_asc_u32(w.k0, w.v0, w.k1, w.v1, n, hist);
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float* d = dets + (size_t)w.v0[i] * 5;
-        w.sorted[i] = make_float4(d[0], d[1], d[2], d[3]);
-    }
-    __syncthreads();
-    block_nms_sorted(w.sorted, n, thresh, 0, w.removed, &nsm);
+    block_nms_sorted(w.sorted, n, thresh, w.removed, &nsm);
     for (int i = threadIdx.x; i < n; i += blockDim.x)
         if (!((w.removed[i >> 6] >> (i & 63)) & 1ull)) w.flags[w.v0[i]] = 1;
-    if (threadIdx.x == 0) running = 0;
     __syncthreads();
-    // ordered compaction of the flags -> ascending original indices
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < n; base += blockDim.x) {
-        const int i = base + threadIdx.x;
-        const int f = (i < n) ? w.flags[i] : 0;
-        const unsigned b = __ballot_sync(0xffffffffu, f);
-        if (lane == 0) scan_warp[warp] = __popc(b);
-        __syncthreads();
-        if (warp == 0) {
-            int v = scan_warp[lane], inc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-            scan_warp[lane] = inc - v;
-            if (lane == 31) nsm.kcount = inc;   // block total (reuse a scratch int)
-        }
-        __syncthreads();
-        if (f) keep_out[running + scan_warp[warp] + __popc(b & ((1u << lane) - 1u))] = i;
-        __syncthreads();
-        if (threadIdx.x == 0) running += nsm.kcount;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *num_keep = running;
+    nms_compact(w.flags, n, keep_out, num_keep);
 }
 
 
-// ---- large sets (n > kNmsSingleCtaMax): sort (1 CTA) -> 64x64 IoU bit-matrix (all SMs) -> chunked scan (1 CTA) -> compaction
+// ---- large sets (n > kNmsSingleCtaMax): sort (1 CTA) -> 64x64 IoU bit-matrix (nms_mask_kernel, all SMs) -> survivor walk (1 CTA) -> compaction
 static constexpr int kNmsSingleCtaMax = 4096;
 
 __global__ void __launch_bounds__(1024) nms_big_sort_kernel(const float* __restrict__ dets, int n, NmsWs w) {
     __shared__ uint32_t hist[32 * 256];
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        w.k0[i] = float_desc_key(dets[(size_t)i * 5 + 4]);
-        w.v0[i] = i;
-        w.flags[i] = 0;
-    }
-    __syncthreads();
-    block_radix_sort_asc_u32(w.k0, w.v0, w.k1, w.v1, n, hist);
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float* d = dets + (size_t)w.v0[i] * 5;
-        w.sorted[i] = make_float4(d[0], d[1], d[2], d[3]);
-    }
-}
-
-// grid (nchunks, nchunks), 64 threads: block (bj, bi) with bj >= bi fills mask[i][bj] for the 64 boxes i of chunk bi:
-// bit b set  <=>  sorted box i suppresses sorted box bj*64 + b (only later boxes: index > i)
-__global__ void __launch_bounds__(64) nms_big_mask_kernel(const float4* __restrict__ boxes, int n, int nchunks, float thresh,
-                                                        unsigned long long* __restrict__ mask) {
-    const int bj = blockIdx.x, bi = blockIdx.y;
-    if (bj < bi) return;
-    __shared__ float4 jb[64];
-    __shared__ float ja[64];
-    const int j0 = bj * 64, i = bi * 64 + threadIdx.x;
-    const int jn = min(64, n - j0);
-    if ((int)threadIdx.x < jn) { const float4 b = boxes[j0 + threadIdx.x]; jb[threadIdx.x] = b; ja[threadIdx.x] = box_area_p1(b); }
-    __syncthreads();
-    if (i >= n) return;
-    const float4 me = boxes[i];
-    const float ma = box_area_p1(me);
-    unsigned long long bits = 0ull;
-    for (int b = 0; b < jn; ++b)
-        if (j0 + b > i && iou_suppresses(me, ma, jb[b], ja[b], thresh)) bits |= 1ull << b;
-    mask[(size_t)i * nchunks + bj] = bits;
+    nms_sort_boxes(dets, n, w, hist);
+    if (threadIdx.x == 0) *w.count = n;
 }
 
 __global__ void __launch_bounds__(1024) nms_big_scan_kernel(const unsigned long long* __restrict__ mask, int n, int nchunks, NmsWs w) {
     extern __shared__ unsigned long long removed[];     // nchunks words
-    __shared__ unsigned long long diag[64];
-    __shared__ int kept_list[64];
-    __shared__ int kcount;
-    for (int i = threadIdx.x; i < nchunks; i += blockDim.x) removed[i] = 0ull;
-    __syncthreads();
-    for (int c = 0; c < nchunks; ++c) {
-        const int cn = min(64, n - c * 64);
-        if ((int)threadIdx.x < cn) diag[threadIdx.x] = mask[(size_t)(c * 64 + threadIdx.x) * nchunks + c];
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            const unsigned long long valid = (cn == 64) ? ~0ull : ((1ull << cn) - 1ull);
-            unsigned long long alive = ~removed[c] & valid;
-            int kc = 0;
-            while (alive) {
-                const int b = __ffsll((long long)alive) - 1;
-                kept_list[kc++] = c * 64 + b;
-                w.flags[w.v0[c * 64 + b]] = 1;        // survivor, in original index space
-                alive &= ~diag[b];
-                alive &= ~(1ull << b);
-            }
-            kcount = kc;
-        }
-        __syncthreads();
-        const int kc = kcount;
-        for (int wd = c + 1 + threadIdx.x; wd < nchunks; wd += blockDim.x) {
-            unsigned long long acc = 0ull;
-            for (int k = 0; k < kc; ++k) acc |= mask[(size_t)kept_list[k] * nchunks + wd];
-            removed[wd] |= acc;
-        }
-        __syncthreads();
-    }
+    __shared__ NmsWalkSmem wsm;
+    block_nms_walk(mask, n, nchunks, 0, removed, &wsm);
+    for (int i = threadIdx.x; i < n; i += blockDim.x)
+        if (!((removed[i >> 6] >> (i & 63)) & 1ull)) w.flags[w.v0[i]] = 1;        // survivor, in original index space
 }
 
-// flags (original index space) -> ascending kept indices
 __global__ void __launch_bounds__(1024) nms_compact_kernel(const int* __restrict__ flags, int n, long long* __restrict__ keep_out, int* __restrict__ num_keep) {
-    __shared__ int scan_warp[33];
-    __shared__ int running;
-    if (threadIdx.x == 0) running = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < n; base += blockDim.x) {
-        const int i = base + threadIdx.x;
-        const int f = (i < n) ? flags[i] : 0;
-        const unsigned b = __ballot_sync(0xffffffffu, f);
-        if (lane == 0) scan_warp[warp] = __popc(b);
-        __syncthreads();
-        if (warp == 0) {
-            int v = scan_warp[lane], inc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-            scan_warp[lane] = inc - v;
-            if (lane == 31) scan_warp[32] = inc;
-        }
-        __syncthreads();
-        if (f) keep_out[running + scan_warp[warp] + __popc(b & ((1u << lane) - 1u))] = i;
-        __syncthreads();
-        if (threadIdx.x == 0) running += scan_warp[32];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *num_keep = running;
+    nms_compact(flags, n, keep_out, num_keep);
 }
 }  // namespace
 
 extern "C" int64_t dt_nms_workspace_bytes(int64_t n) {
     if (n < 1) n = 1;
-    int64_t base = (int64_t)(5 * align_up((size_t)n * 4, 256) + align_up((size_t)n * 16, 256) + align_up(((size_t)n + 63) / 64 * 8, 256));
+    int64_t base = (int64_t)(5 * align_up((size_t)n * 4, 256) + align_up((size_t)n * 16, 256) + 256 + align_up(((size_t)n + 63) / 64 * 8, 256));
     if (n > kNmsSingleCtaMax) base += (int64_t)align_up((size_t)n * (((size_t)n + 63) / 64) * 8, 256);      // the 64-bit suppression matrix
     return base;
 }
@@ -463,7 +379,7 @@ extern "C" int dt_nms(const float* dets, int n, float thresh, int64_t* keep_out,
     }
     unsigned long long* mask = reinterpret_cast<unsigned long long*>(reinterpret_cast<uint8_t*>(w.removed) + align_up((size_t)nchunks * 8, 256));
     nms_big_sort_kernel<<<1, 1024, 0, st>>>(dets, n, w);
-    nms_big_mask_kernel<<<dim3(nchunks, nchunks), 64, 0, st>>>(w.sorted, n, nchunks, thresh, mask);
+    nms_mask_kernel<<<dim3(nchunks, nchunks, 1), 64, 0, st>>>(w.sorted, w.count, n, nchunks, thresh, mask);
     static bool attr_set = false;
     if (!attr_set) {
         DT_CHECK_CUDA(cudaFuncSetAttribute(nms_big_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));

@@ -1,6 +1,6 @@
 // detectorch_b200 -- the non-GEMM device stages of the detector, all on-device and sync-free:
-//   stem im2col, maxpool, P6 subsample                      (torchvision trunk glue, detector.py:183,250)
-//   rpn_proposals_kernel   top-k + decode + clip + filter + NMS(0.7)   generate_proposals.py:31-122
+//   stem image packing, maxpool, P6 subsample               (torchvision trunk glue, detector.py:183,250)
+//   rpn_select_*_kernel, rpn_proposals_kernel, rpn_nms_scan_kernel  top-k + decode + clip + filter + NMS(0.7)   generate_proposals.py:31-122
 //   collect_kernel         merge levels, top-N, FPN level map           collect_and_distribute...py:84-128,
 //                                                                       multilevel_rois.py:41-53
 //   softmax_split_kernel   class softmax + split cls/bbox               detector.py:277-284
@@ -15,35 +15,6 @@
 namespace dt {
 
 static constexpr float kBBoxXformClip = 4.135166556742356f;   // log(1000/16), boxes.py:73
-
-// ---------------------------------------------------------------------------------- stem im2col
-// image NCHW [B,3,H,W] -> col [B*Ho*Wo, 160], k = c*49 + ky*7 + kx (torch weight order), k >= 147 zero.
-// 7x7 stride 2 pad 3 (torchvision resnet conv1).  im_info (may be null): pixels outside image b read as zero (image_info).
-static __global__ void stem_im2col_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int Wo, float* __restrict__ col,
-                                          const float* __restrict__ im_info) {
-    const long long total = (long long)B * Ho * Wo * 40;   // float4 granules
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int k4 = (int)(i % 40);
-        long long m = i / 40;
-        const int wo = (int)(m % Wo); m /= Wo;
-        const int ho = (int)(m % Ho);
-        const int b = (int)(m / Ho);
-        const ImageInfo g = image_info(im_info, b, 1, H, W);
-        float v[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int k = k4 * 4 + j;
-            float x = 0.f;
-            if (k < 147) {
-                const int c = k / 49, r = k - c * 49, ky = r / 7, kx = r - ky * 7;
-                const int y = ho * 2 - 3 + ky, xx = wo * 2 - 3 + kx;
-                if (y >= 0 && y < g.h && xx >= 0 && xx < g.w) x = __ldg(img + (((size_t)b * 3 + c) * H + y) * W + xx);
-            }
-            v[j] = x;
-        }
-        reinterpret_cast<float4*>(col)[i] = make_float4(v[0], v[1], v[2], v[3]);
-    }
-}
 
 // image NCHW [B,3,H,W] -> zero-bordered NHWC4 [B,Hp,Wp,4] (3-pixel border = the conv1 padding; channel 3 = 0).  im_info (may be null):
 // everything outside image b is written as zero, whatever the canvas holds there (NaN included)
@@ -202,48 +173,6 @@ __device__ __forceinline__ float4 clip_box(float4 b, float wmax, float hmax) {  
     return b;
 }
 
-// exclusive prefix of a per-thread count over the block (all threads must call); *total receives the block total.  scratch: 33 ints
-__device__ __forceinline__ int block_rank_count(int cnt, int* scratch, int* total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    int incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-    __syncthreads();
-    if (lane == 31) scratch[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        const int x = lane < nw ? scratch[lane] : 0;
-        int w = x;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += u; }
-        scratch[lane] = w - x;
-        if (lane == 31) scratch[32] = w;
-    }
-    __syncthreads();
-    *total = scratch[32];
-    return scratch[warp] + incl - cnt;
-}
-
-// block-wide ordered compaction helper: returns the exclusive rank of `flag` among threads of this block
-// sweep (all threads must call); *total receives the block total.  scratch: 33 ints of shared memory.
-__device__ __forceinline__ int block_rank(bool flag, int* scratch, int* total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    const unsigned b = __ballot_sync(0xffffffffu, flag);
-    __syncthreads();
-    if (lane == 0) scratch[warp] = __popc(b);
-    __syncthreads();
-    if (warp == 0) {
-        int v = lane < nw ? scratch[lane] : 0, inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-        scratch[lane] = inc - v;
-        if (lane == 31) scratch[32] = inc;
-    }
-    __syncthreads();
-    *total = scratch[32];
-    return scratch[warp] + __popc(b & ((1u << lane) - 1u));
-}
-
 // ---------------------------------------------------------------------------------- RPN proposals
 struct RpnLevel {
     const float* rpn_out;    // NHWC [B,H,W,ch_stride]: ch [0,A) = objectness prob, [A+4a, A+4a+4) = deltas of anchor a
@@ -272,17 +201,15 @@ struct RpnParams {
     int* dbg_order;          // [B, L, pre_nms] flat anchor index of the sorted top-k
     // multi-CTA selection (rpn_select_*_kernel): per (image, level) two 2048-bin digit histograms, per-chunk selected counts, (b1, b2, total)
     uint32_t* sel_hist;      // [B, L, 2, 2048], zeroed before every run
-    int* sel_chunk_counts;   // [B, L, kRpnMaxChunks]
+    int sel_chunks;          // ceil(largest level / kRpnChunk): the x extent of the selection grid
+    int* sel_chunk_counts;   // [B, L, sel_chunks]
     int* sel_info;           // [B, L, 4]: b1, b2, total (-1: not narrowed -> full sort), unused
-    int split;               // 1: selection done by the multi-CTA kernels, rpn_proposals_kernel only finishes
-    // NMS at full-GPU width (rpn_nms_mask_kernel + rpn_nms_scan_kernel): rpn_proposals_kernel then stops after decode / filter
-    int nms_split;
+    // NMS at full-GPU width (nms_mask_kernel + rpn_nms_scan_kernel) when nms_thresh > 0: rpn_proposals_kernel then stops after decode / filter
     int nms_chunks;          // ceil(pre_nms / 64)
     int* cand_counts;        // [B, L] candidates that passed the filter
     unsigned long long* nms_mask;   // [B, L, pre_nms, nms_chunks]: bit b of word (i, w) set <=> candidate i suppresses candidate w*64 + b (> i)
 };
 static constexpr int kRpnChunk = 4096;        // anchors per CTA of the selection kernels (1024 threads x 4)
-static constexpr int kRpnMaxChunks = 64;      // >= ceil(largest level / kRpnChunk): 182 400 / 4096 = 45 at 800x1216; levels above this use the one-CTA path
 
 __host__ __device__ __forceinline__ bool rpn_level_selects(int n, int K) { return n > 4 * K && n > 8192; }
 
@@ -432,10 +359,10 @@ static __global__ void __launch_bounds__(1024) rpn_select_count_kernel(const __g
     }
     int tot;
     block_rank_count(cnt, scratch, &tot);
-    if (threadIdx.x == 0) P.sel_chunk_counts[((size_t)b * P.num_levels + l) * kRpnMaxChunks + blockIdx.x] = tot;
+    if (threadIdx.x == 0) P.sel_chunk_counts[((size_t)b * P.num_levels + l) * P.sel_chunks + blockIdx.x] = tot;
 }
 
-// ---- selection pass 4: ordered compaction (ascending anchor index, like the one-CTA path) into (k1, v1)
+// ---- selection pass 4: ordered compaction (ascending anchor index) into (k1, v1)
 static __global__ void __launch_bounds__(1024) rpn_select_scatter_kernel(const __grid_constant__ RpnParams P) {
     __shared__ int scratch[33];
     __shared__ int offset;
@@ -450,7 +377,7 @@ static __global__ void __launch_bounds__(1024) rpn_select_scatter_kernel(const _
     if (info[2] < 0) return;
     const uint32_t b1 = (uint32_t)info[0], b2 = (uint32_t)info[1];
     if (threadIdx.x == 0) {
-        const int* cc = P.sel_chunk_counts + ((size_t)b * P.num_levels + l) * kRpnMaxChunks;
+        const int* cc = P.sel_chunk_counts + ((size_t)b * P.num_levels + l) * P.sel_chunks;
         int o = 0;
         for (int c = 0; c < (int)blockIdx.x; ++c) o += cc[c];
         offset = o;
@@ -480,9 +407,7 @@ static __global__ void __launch_bounds__(1024) rpn_select_scatter_kernel(const _
 
 // grid (L, B), 1024 threads
 static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid_constant__ RpnParams P) {
-    __shared__ __align__(16) uint32_t hist[32 * 256];
-    __shared__ NmsSmem nsm;
-    __shared__ unsigned long long removed[128];   // up to 8192 candidates
+    __shared__ uint32_t hist[32 * 256];
     __shared__ int scratch[33];
     const int l = blockIdx.x, b = blockIdx.y;
     const RpnLevel& lv = P.lv[l];
@@ -493,147 +418,16 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
     int* v0 = P.v0 + (size_t)b * P.ws_per_image + lv.ws_off;
     int* v1 = P.v1 + (size_t)b * P.ws_per_image + lv.ws_off;
     const float* base = lv.rpn_out + (size_t)b * lv.H * lv.W * lv.ch_stride;
-    // 1. keys in (H,W,A) order (generate_proposals.py:64,72)
-    // 2. top-K by descending score (:77-86).  A full sort of ~180k keys by one CTA costs >1 ms, so first narrow the set
-    //    with a two-level 11+11-bit radix select on the key (exact: every key below the boundary sub-bin plus the whole
-    //    boundary sub-bin is kept, in index order), then stable-sort only those candidates.
-    //    The passes over the level are latency-bound (one CTA): every thread keeps 4 independent loads in flight.
+    // 1. keys in (H,W,A) order (generate_proposals.py:64,72): rpn_select_keys_kernel left them in (k0, v0)
+    // 2. top-K by descending score (:77-86).  A full sort of ~180k keys by one CTA costs >1 ms, so rpn_select_*_kernel first narrowed
+    //    the set with a two-level 11+11-bit radix select on the key (exact: every key below the boundary sub-bin plus the whole boundary
+    //    sub-bin is kept): (k1, v1) hold those `total` pairs in ascending index order, and only they are stable-sorted here.  A level
+    //    that does not select, or whose boundary sub-bin left more than 8192 keys (total < 0), is sorted whole.
     const int K = (P.pre_nms <= 0 || P.pre_nms >= n) ? n : P.pre_nms;
-    const int* vs = v0;                 // sorted anchor indices end up here
-    bool narrowed = false;
-    // P.split: the keys, the two-level radix select and the ordered compaction were done at full-GPU width by rpn_select_*_kernel
-    // (one CTA per 4096 anchors instead of one CTA per level: the 182 400-anchor P2 level was the long pole of this kernel); (k1, v1)
-    // hold the `total` selected (key, index) pairs in ascending index order, (k0, v0) all keys.  What remains is per (level, image).
-    if (P.split && n <= kRpnChunk * kRpnMaxChunks) {
-        if (rpn_level_selects(n, K)) {
-            const int total = P.sel_info[((size_t)b * P.num_levels + l) * 4 + 2];
-            if (total >= 0) {
-                block_radix_sort_asc_u32(k1, v1, k0, v0, total, hist);
-                vs = v1;
-                narrowed = true;
-            }
-        }
-    } else {
-        const bool select = n > 4 * K && n > 8192;
-        uint32_t* h1 = hist;                // 2048 bins
-        uint32_t* h2 = hist + 2048;         // 2048 bins
-        __shared__ uint32_t sel[4];         // b1, c1, b2, count
-        if (select) {
-            for (int i = threadIdx.x; i < 4096; i += blockDim.x) hist[i] = 0;
-            __syncthreads();
-        }
-        for (int base_i = 0; base_i < n; base_i += 4 * blockDim.x) {
-            uint32_t k[4];
-            bool valid[4];
-    #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int i = base_i + j * blockDim.x + threadIdx.x;
-                valid[j] = i < n;
-                k[j] = 0u;
-                if (valid[j]) {
-                    const int a = i % lv.A, cell = i / lv.A;
-                    k[j] = float_desc_key(base[rpn_canvas_cell(cell, il.w, lv.W) * lv.ch_stride + a]);
-                }
-            }
-    #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int i = base_i + j * blockDim.x + threadIdx.x;
-                if (valid[j]) { k0[i] = k[j]; v0[i] = i; }
-                if (select) {
-                    // objectness scores cluster in a few exponent bins: aggregate equal digits inside the warp before touching shared memory
-                    const unsigned act = __ballot_sync(0xffffffffu, valid[j]);
-                    if (valid[j]) {
-                        const uint32_t d = k[j] >> 21;
-                        const unsigned m = __match_any_sync(act, d);
-                        if ((m & ((1u << (threadIdx.x & 31)) - 1u)) == 0) atomicAdd(&h1[d], (uint32_t)__popc(m));
-                    }
-                }
-            }
-        }
-        __syncthreads();
-        // first bin b with c + h[b] >= K (c = keys in the bins before it), by warp 0: 64 bins per lane, warp prefix, serial scan of one lane's bins
-        auto find_bin = [&](const uint32_t* h, uint32_t c0, uint32_t* out_bin, uint32_t* out_c) {
-            if (threadIdx.x < 32) {
-                const int lane = threadIdx.x;
-                uint32_t sum = 0;
-                for (int t = 0; t < 64; ++t) sum += h[lane * 64 + t];
-                uint32_t incl = sum;
-    #pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-                const uint32_t excl = c0 + incl - sum;
-                const bool hit = excl + sum >= (uint32_t)K;            // the crossing lies in or before this lane's bins
-                const unsigned hits = __ballot_sync(0xffffffffu, hit);
-                if (hits == 0) { if (lane == 0) { *out_bin = 2048; *out_c = c0 + __shfl_sync(0xffffffffu, incl, 31); } }
-                else if (lane == __ffs(hits) - 1) {
-                    uint32_t c = excl, bb = (uint32_t)lane * 64;
-                    for (; bb < (uint32_t)lane * 64 + 64; ++bb) { if (c + h[bb] >= (uint32_t)K) break; c += h[bb]; }
-                    *out_bin = bb; *out_c = c;
-                }
-            }
-        };
-        if (select) {
-            find_bin(h1, 0u, &sel[0], &sel[1]);
-            __syncthreads();
-            const uint32_t b1 = sel[0], c1 = sel[1];
-            for (int base_i = 0; base_i < n; base_i += 4 * blockDim.x) {
-                uint32_t k[4];
-    #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int i = base_i + j * blockDim.x + threadIdx.x;
-                    k[j] = i < n ? k0[i] : 0xffffffffu;
-                }
-    #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int i = base_i + j * blockDim.x + threadIdx.x;
-                    const bool valid = (i < n) && ((k[j] >> 21) == b1);
-                    const unsigned act = __ballot_sync(0xffffffffu, valid);
-                    if (valid) {
-                        const uint32_t d = (k[j] >> 10) & 2047u;
-                        const unsigned m = __match_any_sync(act, d);
-                        if ((m & ((1u << (threadIdx.x & 31)) - 1u)) == 0) atomicAdd(&h2[d], (uint32_t)__popc(m));
-                    }
-                }
-            }
-            __syncthreads();
-            find_bin(h2, c1, &sel[2], &sel[3]);
-            __syncthreads();
-            if (threadIdx.x == 0 && sel[2] < 2048u) sel[3] += h2[sel[2]];
-            __syncthreads();
-            const uint32_t b2 = sel[2], total = sel[3];
-            if (total <= 8192u) {
-                // ordered compaction: a thread owns 4 consecutive indices, one block scan per 4096 keys
-                int m = 0;
-                for (int base_i = 0; base_i < n; base_i += 4 * blockDim.x) {
-                    const int i0 = base_i + 4 * threadIdx.x;
-                    uint32_t k[4];
-                    bool f[4];
-                    int cnt = 0;
-    #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int i = i0 + j;
-                        k[j] = i < n ? k0[i] : 0xffffffffu;
-                    }
-    #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint32_t d1 = k[j] >> 21;
-                        f[j] = (i0 + j < n) && ((d1 < b1) || (d1 == b1 && ((k[j] >> 10) & 2047u) <= b2));
-                        cnt += f[j] ? 1 : 0;
-                    }
-                    int tot;
-                    int r = m + block_rank_count(cnt, scratch, &tot);
-    #pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        if (f[j]) { k1[r] = k[j]; v1[r] = i0 + j; ++r; }
-                    m += tot;
-                }
-                __syncthreads();
-                block_radix_sort_asc_u32(k1, v1, k0, v0, m, hist);
-                vs = v1;
-                narrowed = true;
-            }
-        }
-    }
-    if (!narrowed) block_radix_sort_asc_u32(k0, v0, k1, v1, n, hist);
+    const int total = rpn_level_selects(n, K) ? P.sel_info[((size_t)b * P.num_levels + l) * 4 + 2] : -1;
+    const bool narrowed = total >= 0;
+    block_radix_sort_asc_u32(narrowed ? k1 : k0, narrowed ? v1 : v0, narrowed ? k0 : k1, narrowed ? v0 : v1, narrowed ? total : n, hist);
+    const int* vs = narrowed ? v1 : v0;     // the sorted anchor indices
     // 3. decode + clip + filter on the top K (:96-112), order preserved
     float4* cand = P.cand + ((size_t)b * P.num_levels + l) * P.pre_nms;
     float* cscore = P.cand_score + ((size_t)b * P.num_levels + l) * P.pre_nms;
@@ -670,127 +464,32 @@ static __global__ void __launch_bounds__(1024) rpn_proposals_kernel(const __grid
         nc += tot;
     }
     __syncthreads();
-    if (P.nms_split && P.nms_thresh > 0.f) {
-        // the greedy NMS of the <= pre_nms candidates continues in rpn_nms_mask_kernel (all pair tests, every SM) and
-        // rpn_nms_scan_kernel (the sequential survivor walk): in this CTA the per-box sweep over the survivors was 45 % of the kernel
+    if (P.nms_thresh > 0.f) {
+        // 4. NMS (:114-120) of the candidates (already in descending-score order) continues in nms_mask_kernel (all pair tests, every SM)
+        // and rpn_nms_scan_kernel (the sequential survivor walk)
         if (threadIdx.x == 0) P.cand_counts[b * P.num_levels + l] = nc;
         return;
     }
-    // 4. NMS (:114-120); candidates are already in descending-score order
     float* op = P.out_props + ((size_t)b * P.num_levels + l) * P.post_nms * 4;
     float* os = P.out_scores + ((size_t)b * P.num_levels + l) * P.post_nms;
-    int nout = 0;
-    if (P.nms_thresh > 0.f) {
-        // the sort is over: its 32 KB histogram area holds up to 2048 candidate boxes, so the NMS reads them from shared memory
-        // instead of paying an L2 round trip per chunk (the FPN levels have at most 1000 candidates; the C4 level's 6000 stay global)
-        const float4* nms_boxes = cand;
-        if (nc <= 2048) {
-            float4* sb = reinterpret_cast<float4*>(hist);
-            for (int i = threadIdx.x; i < nc; i += blockDim.x) sb[i] = cand[i];
-            __syncthreads();
-            nms_boxes = sb;
-        }
-        block_nms_sorted(nms_boxes, nc, P.nms_thresh, P.post_nms, removed, &nsm);
-        for (int base_i = 0; base_i < nc; base_i += blockDim.x) {
-            const int i = base_i + threadIdx.x;
-            const bool keep = (i < nc) && !((removed[i >> 6] >> (i & 63)) & 1ull);
-            int tot;
-            const int r = block_rank(keep, scratch, &tot);
-            const int pos = nout + r;
-            if (keep && (P.post_nms <= 0 || pos < P.post_nms)) {
-                const float4 bx = cand[i];
-                op[pos * 4 + 0] = bx.x; op[pos * 4 + 1] = bx.y; op[pos * 4 + 2] = bx.z; op[pos * 4 + 3] = bx.w;
-                os[pos] = cscore[i];
-            }
-            nout += tot;
-        }
-        if (P.post_nms > 0 && nout > P.post_nms) nout = P.post_nms;
-    } else {
-        nout = min(nc, P.post_nms);
-        for (int i = threadIdx.x; i < nout; i += blockDim.x) {
-            const float4 bx = cand[i];
-            op[i * 4 + 0] = bx.x; op[i * 4 + 1] = bx.y; op[i * 4 + 2] = bx.z; op[i * 4 + 3] = bx.w;
-            os[i] = cscore[i];
-        }
+    const int nout = min(nc, P.post_nms);
+    for (int i = threadIdx.x; i < nout; i += blockDim.x) {
+        const float4 bx = cand[i];
+        op[i * 4 + 0] = bx.x; op[i * 4 + 1] = bx.y; op[i * 4 + 2] = bx.z; op[i * 4 + 3] = bx.w;
+        os[i] = cscore[i];
     }
     if (threadIdx.x == 0) P.out_counts[b * P.num_levels + l] = nout;
 }
 
-// ---- RPN NMS, part 1: the suppression bit-matrix of every (level, image), at full-GPU width.
-// grid (chunks, chunks, L*B), 64 threads: block (bj, bi) with bj >= bi fills word (i, bj) for the 64 candidates i of chunk bi:
-// bit b set <=> candidate i suppresses candidate bj*64 + b (only later candidates; cython_nms.pyx:76-85 semantics, iou_suppresses)
-static __global__ void __launch_bounds__(64) rpn_nms_mask_kernel(const __grid_constant__ RpnParams P) {
-    const int bj = blockIdx.x, bi = blockIdx.y, lb = blockIdx.z;      // lb = b * L + l
-    if (bj < bi) return;
-    const int n = P.cand_counts[lb];
-    if (bi * 64 >= n || bj * 64 >= n) return;
-    __shared__ float4 jb[64];
-    __shared__ float ja[64];
-    const float4* boxes = P.cand + (size_t)lb * P.pre_nms;
-    const int j0 = bj * 64, i = bi * 64 + threadIdx.x;
-    const int jn = min(64, n - j0);
-    if ((int)threadIdx.x < jn) { const float4 bx = boxes[j0 + threadIdx.x]; jb[threadIdx.x] = bx; ja[threadIdx.x] = box_area_p1(bx); }
-    __syncthreads();
-    if (i >= n) return;
-    const float4 me = boxes[i];
-    const float ma = box_area_p1(me);
-    unsigned long long bits = 0ull;
-    for (int t = 0; t < jn; ++t)
-        if (j0 + t > i && iou_suppresses(me, ma, jb[t], ja[t], P.nms_thresh)) bits |= 1ull << t;
-    P.nms_mask[((size_t)lb * P.pre_nms + i) * P.nms_chunks + bj] = bits;
-}
-
-// ---- RPN NMS, part 2: the sequential survivor walk over the bit-matrix + the first post_nms survivors out (generate_proposals.py:114-120).
-// grid (L, B), 1024 threads.
+// ---- RPN NMS, part 2 (part 1 is nms_mask_kernel over the (level, image) sets): the survivor walk over the bit-matrix + the first
+// post_nms survivors out (generate_proposals.py:114-120).  grid (L, B), 1024 threads.
 static __global__ void __launch_bounds__(1024) rpn_nms_scan_kernel(const __grid_constant__ RpnParams P) {
     __shared__ unsigned long long removed[128];   // up to 8192 candidates
-    __shared__ unsigned long long diag[64];
-    __shared__ int kept_list[64];
-    __shared__ int kcount, total_kept;
+    __shared__ NmsWalkSmem wsm;
     __shared__ int scratch[33];
     const int l = blockIdx.x, b = blockIdx.y, lb = b * P.num_levels + l;
     const int n = P.cand_counts[lb];
-    const int nchunks = (n + 63) >> 6, NCH = P.nms_chunks;
-    const unsigned long long* mask = P.nms_mask + (size_t)lb * P.pre_nms * NCH;
-    for (int i = threadIdx.x; i < 128; i += blockDim.x) removed[i] = 0ull;
-    if (threadIdx.x == 0) total_kept = 0;
-    __syncthreads();
-    for (int c = 0; c < nchunks; ++c) {
-        const int cn = min(64, n - c * 64);
-        if ((int)threadIdx.x < cn) diag[threadIdx.x] = mask[(size_t)(c * 64 + threadIdx.x) * NCH + c];
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            const unsigned long long valid = (cn == 64) ? ~0ull : ((1ull << cn) - 1ull);
-            unsigned long long alive = ~removed[c] & valid, kept = 0ull;
-            int kc = 0, tot = total_kept;
-            while (alive) {
-                const int t = __ffsll((long long)alive) - 1;
-                if (P.post_nms > 0 && tot >= P.post_nms) break;
-                kept |= 1ull << t;
-                kept_list[kc++] = c * 64 + t;
-                ++tot;
-                alive &= ~diag[t];
-                alive &= ~(1ull << t);
-            }
-            removed[c] = ~kept;
-            kcount = kc;
-            total_kept = tot;
-        }
-        __syncthreads();
-        if (P.post_nms > 0 && total_kept >= P.post_nms) {
-            for (int i = c + 1 + threadIdx.x; i < nchunks; i += blockDim.x) removed[i] = ~0ull;
-            __syncthreads();
-            break;
-        }
-        // the survivors of this chunk suppress later candidates: OR their matrix rows into `removed`, one (survivor, word) pair per thread
-        const int kc = kcount, words = nchunks - c - 1;
-        for (int p = threadIdx.x; p < kc * words; p += blockDim.x) {
-            const int k = p / words, wd = c + 1 + (p - k * words);
-            const unsigned long long v = mask[(size_t)kept_list[k] * NCH + wd];
-            if (v) atomicOr(&removed[wd], v);
-        }
-        __syncthreads();
-    }
+    block_nms_walk(P.nms_mask + (size_t)lb * P.pre_nms * P.nms_chunks, n, P.nms_chunks, P.post_nms, removed, &wsm);
     // ordered compaction of the survivors
     const float4* cand = P.cand + (size_t)lb * P.pre_nms;
     const float* cscore = P.cand_score + (size_t)lb * P.pre_nms;
@@ -986,7 +685,7 @@ static __global__ void __launch_bounds__(256) det_class_kernel(const __grid_cons
         dbox[ri] = o;
     }
     __syncthreads();
-    const int kept = block_nms_sorted(sbox, nc, P.nms_thresh, 0, removed, &nsm);
+    const int kept = block_nms_sorted(sbox, nc, P.nms_thresh, removed, &nsm);
     for (int i = threadIdx.x; i < nc; i += blockDim.x)
         if (!((removed[i >> 6] >> (i & 63)) & 1ull)) flag[(int)(skey[i] & 0xffffffffu)] = 1;
     if (threadIdx.x == 0) P.cls_counts[b * P.NC + j] = kept;

@@ -43,7 +43,7 @@ class EngineConfig(ctypes.Structure):
                 ("rpn_min_size", ctypes.c_float), ("num_classes", ctypes.c_int), ("score_thresh", ctypes.c_float),
                 ("det_nms_thresh", ctypes.c_float), ("max_dets", ctypes.c_int), ("det_cap", ctypes.c_int),
                 ("use_mask", ctypes.c_int), ("output_prob", ctypes.c_int), ("emit_full_masks", ctypes.c_int),
-                ("passes", ctypes.c_int), ("precise_mask", ctypes.c_int), ("stem_im2col", ctypes.c_int), ("exact_roialign", ctypes.c_int), ("model_type", ctypes.c_int), ("use_rpn", ctypes.c_int),
+                ("passes", ctypes.c_int), ("precise_mask", ctypes.c_int), ("exact_roialign", ctypes.c_int), ("model_type", ctypes.c_int), ("use_rpn", ctypes.c_int),
                 ("conv_kind", ctypes.c_int), ("plane_handover", ctypes.c_int)]
 
 
@@ -122,7 +122,7 @@ def fold_bn_running_stats(sd, eps=1e-5):
 class Engine:
     def __init__(self, arch="resnet50", batch=1, height=800, width=1216, pre_nms_top_n=1000, post_nms_top_n=1000,
                  rpn_nms_thresh=0.7, rpn_min_size=0.0, num_classes=81, score_thresh=0.05, det_nms_thresh=0.5, max_dets=100,
-                 det_cap=100, use_mask=True, output_prob=True, emit_full_masks=False, passes=3, precise_mask=True, stem_im2col=False, exact_roialign=False, model="fpn", use_rpn=True, conv_kind=None, device="cuda:0",
+                 det_cap=100, use_mask=True, output_prob=True, emit_full_masks=False, passes=3, precise_mask=True, exact_roialign=False, model="fpn", use_rpn=True, conv_kind=None, device="cuda:0",
                  share_weights_with=None):
         if not torch.cuda.is_available():
             raise RuntimeError("detectorch_b200.Engine needs a CUDA device (no CPU fallback)")
@@ -138,7 +138,6 @@ class Engine:
         cfg.max_dets, cfg.det_cap = max_dets, det_cap
         cfg.use_mask, cfg.output_prob, cfg.emit_full_masks, cfg.passes = int(use_mask), int(output_prob), int(emit_full_masks), passes
         cfg.precise_mask = int(precise_mask)          # 1/True = K-split mask convs, 2 = 64-wide tiles with 3 rotating accumulators, 0 = plain
-        cfg.stem_im2col = int(stem_im2col)
         cfg.exact_roialign = int(exact_roialign)
         cfg.model_type = 1 if model == "c4" else 0
         cfg.use_rpn = int(use_rpn)
@@ -176,7 +175,7 @@ class Engine:
         """What shapes the packed weight buffer (matrices, fp16 halves, and the per-conv-launch scale vectors, which are laid out in launch
         order): the model and the numerics mode -- not the image size, RoI / detection capacities or thresholds."""
         c = self.cfg
-        return tuple(c.arch_blocks) + (c.num_classes, c.use_mask, c.model_type, c.use_rpn, c.conv_kind, c.precise_mask, c.passes, c.stem_im2col)
+        return tuple(c.arch_blocks) + (c.num_classes, c.use_mask, c.model_type, c.use_rpn, c.conv_kind, c.precise_mask, c.passes)
 
     def owns(self, ptr):
         return self._ws_lo <= ptr < self._ws_hi

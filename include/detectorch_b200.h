@@ -180,7 +180,6 @@ typedef struct dt_engine_config {
     int passes;                  /* 3 = 3xTF32 (fp32-accurate, default), 1 = single-pass TF32 */
     int precise_mask;            /* mask-head 3x3 convs (K = 2304): 1 = K-split in two launches with an fp32 RN add between them (halves the
                                     truncating-accumulate error; default), 2 = 128-wide tiles with 3 rotating accumulators, 0 = plain */
-    int stem_im2col;             /* 1 = force the im2col + GEMM stem instead of the fused TMA-window stem (debug) */
     int exact_roialign;          /* 1 = RoIAlign in the reference's exact fp32 operation order (bit-identical to its CPU loop);
                                     0 = separable / FMA fast path (fp32 re-association only, ~1e-7 relative) */
     int model_type;              /* 0 = R-50/101-FPN + RPN (+ '1up4convs' mask head); 1 = R-50/101-C4 (res5 head, 'upshare' mask head) */

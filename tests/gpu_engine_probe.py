@@ -216,8 +216,6 @@ if __name__ == "__main__":
         print("C4 conv launches: %.1f GFLOP algorithmic in %.3f ms = %.1f TFLOP/s" % (fl / 1e9, tm, fl / tm / 1e9), flush=True)
     elif mode == "ops":
         ops()
-    elif mode == "ops_im2col":
-        ops(stem_im2col=True)
     elif mode == "timing":
         timing(int(sys.argv[2]) if len(sys.argv) > 2 else 8, passes=int(sys.argv[3]) if len(sys.argv) > 3 else 3)
     print("==== done", flush=True)
