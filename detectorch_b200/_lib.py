@@ -30,6 +30,10 @@ SIGNATURES = {
     "dt_segm_strings_bytes": (c_int64, [c_int, c_int]),
     "dt_segm_rle": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                             c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_segm_batch_workspace_bytes": (c_int64, [c_int, c_int, c_int]),
+    "dt_segm_batch_strings_bytes": (c_int64, [c_int, c_int, c_int]),
+    "dt_segm_rle_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_segm_paste": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                               c_void_p, c_void_p]),
     "dt_roi_align_backward_det_workspace_bytes": (c_int64, [c_int64, c_int64]),

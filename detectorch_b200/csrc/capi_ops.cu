@@ -472,11 +472,44 @@ size_t segm_smem_bytes(int M, int im_h, int im_w) {
     const int S = M + 2;
     return (size_t)((S * S + 3) & ~3) * 4 + (size_t)im_h * sizeof(SegmRowCoef) + (size_t)(im_w + 2) * 4 + 40 * 4;
 }
+
+// paste + RLE of `batch` images x `cap` slots, then the scan of the string lengths and the gather into `strings`.  The caller has
+// checked the pointers and the sizes except the shared-memory limit.  workspace: segm_ws_bytes(batch * cap, runs_cap)
+int segm_rle_launch(const char* who, const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,
+                    const int* expanded_boxes, const int* num_dets_dev, const int* im_sizes, int batch, int cap, int max_h, int max_w,
+                    float thresh_binarize, uint32_t* counts, int* num_counts, int runs_cap, uint8_t* strings, int64_t* str_offsets,
+                    int* overflow, void* workspace, cudaStream_t st) {
+    const size_t D = (size_t)batch * cap;
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
+    uint8_t* staging = ws + D * runs_cap * 4;
+    int* str_len = reinterpret_cast<int*>(staging + ((D * runs_cap * kSegmCharsPerRun + 15) / 16 * 16));
+    const size_t smem = segm_smem_bytes(mask_size, max_h, max_w);
+    if (smem > 200 * 1024) { fprintf(stderr, "%s: image too large for the row/column tables (%zu B)\n", who, smem); return 0; }
+    static size_t smem_set = 48 * 1024;
+    if (smem > smem_set) {
+        DT_CHECK_CUDA(cudaFuncSetAttribute(segm_rle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        smem_set = 200 * 1024;
+    }
+    DT_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
+    segm_rle_kernel<<<dim3(cap, batch), 256, smem, st>>>(masks, classes, classes ? num_mask_classes : 1, mask_size, ref_boxes, expanded_boxes,
+                                                         num_dets_dev, im_sizes, max_h, max_w, thresh_binarize, positions, counts, num_counts,
+                                                         runs_cap, staging, str_len, runs_cap * kSegmCharsPerRun, overflow);
+    DT_CHECK_CUDA(cudaGetLastError());
+    long long* offsets = reinterpret_cast<long long*>(str_offsets);
+    segm_offsets_kernel<<<1, 1024, 0, st>>>(str_len, (int)D, offsets);
+    DT_CHECK_CUDA(cudaGetLastError());
+    segm_compact_kernel<<<(unsigned)((D + 7) / 8), 256, 0, st>>>(staging, str_len, (int)D, runs_cap * kSegmCharsPerRun, offsets, strings);
+    DT_CHECK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int64_t segm_ws_bytes(int64_t slots, int runs_cap) {
+    return slots * runs_cap * 4 + slots * runs_cap * kSegmCharsPerRun + slots * 4 + 256;
+}
 }  // namespace
 
-extern "C" int64_t dt_segm_workspace_bytes(int max_dets, int runs_cap) {
-    return (int64_t)max_dets * runs_cap * 4 + (int64_t)max_dets * runs_cap * kSegmCharsPerRun + (int64_t)max_dets * 4 + 256;
-}
+extern "C" int64_t dt_segm_workspace_bytes(int max_dets, int runs_cap) { return segm_ws_bytes(max_dets, runs_cap); }
 
 extern "C" int64_t dt_segm_strings_bytes(int max_dets, int runs_cap) { return (int64_t)max_dets * runs_cap * kSegmCharsPerRun; }
 
@@ -493,27 +526,41 @@ extern "C" int dt_segm_rle(const float* masks, const int* classes, int num_mask_
         fprintf(stderr, "dt_segm_rle: unsupported size (mask %d, image %dx%d, runs_cap %d)\n", mask_size, im_h, im_w, runs_cap);
         return 0;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
-    uint8_t* staging = ws + (size_t)max_dets * runs_cap * 4;
-    int* str_len = reinterpret_cast<int*>(staging + (((size_t)max_dets * runs_cap * kSegmCharsPerRun + 15) / 16 * 16));
-    const size_t smem = segm_smem_bytes(mask_size, im_h, im_w);
-    if (smem > 200 * 1024) { fprintf(stderr, "dt_segm_rle: image too large for the row/column tables (%zu B)\n", smem); return 0; }
-    static size_t smem_set = 48 * 1024;
-    if (smem > smem_set) {
-        DT_CHECK_CUDA(cudaFuncSetAttribute(segm_rle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        smem_set = 200 * 1024;
+    return segm_rle_launch("dt_segm_rle", masks, classes, num_mask_classes, mask_size, ref_boxes, expanded_boxes, num_dets_dev, nullptr, 1,
+                           max_dets, im_h, im_w, thresh_binarize, counts, num_counts, runs_cap, strings, str_offsets, overflow, workspace,
+                           (cudaStream_t)stream);
+}
+
+// run lengths and their counts are scratch here: they follow the dt_segm_rle workspace of batch * cap slots
+extern "C" int64_t dt_segm_batch_workspace_bytes(int batch, int cap, int runs_cap) {
+    const int64_t slots = (int64_t)batch * cap;
+    return segm_ws_bytes(slots, runs_cap) + slots * runs_cap * 4 + slots * 4;
+}
+
+extern "C" int64_t dt_segm_batch_strings_bytes(int batch, int cap, int runs_cap) { return (int64_t)batch * cap * runs_cap * kSegmCharsPerRun; }
+
+extern "C" int dt_segm_rle_batch(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes,
+                                 const int* num_dets_dev, const int* im_sizes, int batch, int cap, int max_im_h, int max_im_w,
+                                 float thresh_binarize, int runs_cap, uint8_t* strings, int64_t* str_offsets, int* overflow, void* workspace,
+                                 dt_stream_t stream) {
+    if (batch <= 0 || cap <= 0) return 1;
+    if (!masks || !boxes || !num_dets_dev || !im_sizes || !strings || !str_offsets || !overflow || !workspace) {
+        fprintf(stderr, "dt_segm_rle_batch: null argument\n");
+        return 0;
     }
-    DT_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
-    segm_rle_kernel<<<max_dets, 256, smem, st>>>(masks, classes, classes ? num_mask_classes : 1, mask_size, ref_boxes, expanded_boxes,
-                                                 num_dets_dev, im_h, im_w, thresh_binarize, positions, counts, num_counts, runs_cap,
-                                                 staging, str_len, runs_cap * kSegmCharsPerRun, overflow);
-    DT_CHECK_CUDA(cudaGetLastError());
-    segm_compact_kernel<<<max_dets, 256, 0, st>>>(staging, str_len, max_dets, runs_cap * kSegmCharsPerRun, strings,
-                                                  reinterpret_cast<long long*>(str_offsets));
-    DT_CHECK_CUDA(cudaGetLastError());
-    return 1;
+    if (mask_size < 1 || mask_size > 126 || (classes && num_mask_classes < 1) || max_im_h < 1 || max_im_w < 1 ||
+        (int64_t)max_im_h * max_im_w >= (1ll << 32) || runs_cap < 2 || batch > 65535 || (int64_t)batch * cap >= (1ll << 31)) {
+        fprintf(stderr, "dt_segm_rle_batch: unsupported size (mask %d, %d classes, image %dx%d, runs_cap %d, %d x %d slots)\n", mask_size,
+                num_mask_classes, max_im_h, max_im_w, runs_cap, batch, cap);
+        return 0;
+    }
+    const int64_t slots = (int64_t)batch * cap;
+    uint8_t* scratch = reinterpret_cast<uint8_t*>(workspace) + segm_ws_bytes(slots, runs_cap);
+    uint32_t* counts = reinterpret_cast<uint32_t*>(scratch);
+    int* num_counts = reinterpret_cast<int*>(scratch + slots * runs_cap * 4);
+    return segm_rle_launch("dt_segm_rle_batch", masks, classes, num_mask_classes, mask_size, boxes, nullptr, num_dets_dev, im_sizes, batch,
+                           cap, max_im_h, max_im_w, thresh_binarize, counts, num_counts, runs_cap, strings, str_offsets, overflow, workspace,
+                           (cudaStream_t)stream);
 }
 
 extern "C" int dt_segm_paste(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,

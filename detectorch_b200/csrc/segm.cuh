@@ -3,11 +3,13 @@
 // reference box by (M+2)/M (lib/utils/boxes.py:245-261, fp32), truncate to int32, cv2.resize(INTER_LINEAR, float32) to the
 // box size, threshold, paste into an im_h x im_w uint8 image, pycocotools RLE-encode (maskApi.c rleEncode + rleToString).
 //
-// One CTA per detection.  Nothing of size im_h x im_w is materialised for the RLE: a thread owns image columns, walks the
-// rows of the pasted region evaluating OpenCV's two-pass bilinear resize on the fly (float coefficient tables exactly as
-// cv::resize builds them: double scale, float fx/fy, x clamped with weight (1,0), y by clipping the row index), and records
-// the positions of the column-major flattening where the bit changes.  A block scan turns per-column transition counts into
-// offsets, the differences of consecutive positions are the run lengths, and a second scan packs the LEB128-like string.
+// One CTA per (image, detection slot); each image has its own canvas size and live detection count.  Nothing of size im_h x im_w
+// is materialised for the RLE: a thread owns image columns, walks the rows of the pasted region evaluating OpenCV's two-pass
+// bilinear resize on the fly (float coefficient tables exactly as cv::resize builds them: double scale, float fx/fy, x clamped
+// with weight (1,0), y by clipping the row index), and records the positions of the column-major flattening where the bit
+// changes.  A block scan turns per-column transition counts into offsets, the differences of consecutive positions are the run
+// lengths, and a second scan packs the LEB128-like string.  One more block scans the string lengths of all slots, and the strings
+// are gathered into one packed buffer at those offsets.
 #pragma once
 #include "common.cuh"
 
@@ -102,20 +104,21 @@ __device__ __forceinline__ int block_exclusive_scan(int* a, int n, int* scratch)
     return scratch[32];
 }
 
-// exclusive prefix of one value per thread over the block; *total = sum.  scratch: 33 ints
-__device__ __forceinline__ int block_scan_value(int v, int* scratch, int* total) {
+// exclusive prefix of one value per thread over the block; *total = sum.  scratch: 33 values
+template <typename T>
+__device__ __forceinline__ T block_scan_value(T v, T* scratch, T* total) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int incl = v;
+    T incl = v;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+    for (int o = 1; o < 32; o <<= 1) { const T u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
     __syncthreads();
     if (lane == 31) scratch[warp] = incl;
     __syncthreads();
     if (warp == 0) {
-        const int x = lane < (int)(blockDim.x >> 5) ? scratch[lane] : 0;
-        int w = x;
+        const T x = lane < (int)(blockDim.x >> 5) ? scratch[lane] : T(0);
+        T w = x;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += u; }
+        for (int o = 1; o < 32; o <<= 1) { const T u = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += u; }
         scratch[lane] = w - x;
         if (lane == 31) scratch[32] = w;
     }
@@ -126,30 +129,36 @@ __device__ __forceinline__ int block_scan_value(int v, int* scratch, int* total)
 
 struct SegmRowCoef { int s; float w0, w1; int pad; };
 
-// masks: [D, K, M, M] (class-specific: K classes, cls[d] selects) or [D, M, M] (K == 1 / cls == NULL)
-// outputs per detection d: counts[d*runs_cap ..] (uint32 run lengths), num_counts[d], strings (cap str_cap per det), str_len[d]
-// paste (optional): uint8 [D, im_h, im_w]
+// Grid (cap, B): block (d, b) is detection slot d of image b, i.e. slot s = b * cap + d of the flat per-slot arrays.
+// masks: [B*cap, K, M, M] (class-specific: K classes, cls[s] selects) or [B*cap, M, M] (K == 1 / cls == NULL)
+// im_sizes: int32 [B, 2] (im_h, im_w) of each image's canvas, or NULL (every image is max_h x max_w).  The shared row / column tables
+// are sized for max_h x max_w; an image whose size is not within [1, max] produces empty results.
+// num_dets_dev: int32 [B] live slots per image (NULL: all); slots at or past the count produce empty results
+// outputs per slot s: counts[s*runs_cap ..] (uint32 run lengths), num_counts[s], strings (cap str_cap per slot), str_len[s]
 static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
                                                               const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
-                                                              const int* __restrict__ num_dets_dev, int im_h, int im_w, float thresh,
+                                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
+                                                              int max_h, int max_w, float thresh,
                                                               uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
                                                               int* __restrict__ num_counts, int runs_cap,
                                                               uint8_t* __restrict__ strings, int* __restrict__ str_len, int str_cap,
                                                               int* __restrict__ overflow) {
     extern __shared__ __align__(16) uint8_t segm_smem[];
-    const int d = blockIdx.x;
+    const int b = blockIdx.y, det = blockIdx.x;
+    const size_t d = (size_t)b * gridDim.x + det;
     const int S = M + 2;
     float* pm = reinterpret_cast<float*>(segm_smem);                                     // [S][S] zero-padded mask
-    SegmRowCoef* rows = reinterpret_cast<SegmRowCoef*>(pm + ((S * S + 3) & ~3));          // [im_h]
-    int* colcnt = reinterpret_cast<int*>(rows + im_h);                                   // [im_w + 2]
-    int* scratch = colcnt + im_w + 2;                                                    // [40]
-    if (num_dets_dev && d >= *num_dets_dev) {
+    SegmRowCoef* rows = reinterpret_cast<SegmRowCoef*>(pm + ((S * S + 3) & ~3));          // [max_h]
+    int* colcnt = reinterpret_cast<int*>(rows + max_h);                                  // [max_w + 2]
+    int* scratch = colcnt + max_w + 2;                                                   // [40]
+    const int im_h = im_sizes ? im_sizes[2 * b] : max_h, im_w = im_sizes ? im_sizes[2 * b + 1] : max_w;
+    if ((num_dets_dev && det >= num_dets_dev[b]) || im_h < 1 || im_w < 1 || im_h > max_h || im_w > max_w) {
         if (threadIdx.x == 0) { num_counts[d] = 0; str_len[d] = 0; }
         return;
     }
-    const SegmGeom g = segm_geom(ref_boxes ? ref_boxes + (size_t)d * 4 : nullptr, exp_boxes ? exp_boxes + (size_t)d * 4 : nullptr,
+    const SegmGeom g = segm_geom(ref_boxes ? ref_boxes + d * 4 : nullptr, exp_boxes ? exp_boxes + d * 4 : nullptr,
                                  (float)(((double)M + 2.0) / (double)M), im_h, im_w);
-    const float* msrc = masks + ((size_t)d * K + (cls ? cls[d] : 0)) * M * M;
+    const float* msrc = masks + (d * K + (cls ? cls[d] : 0)) * M * M;
     for (int i = threadIdx.x; i < S * S; i += blockDim.x) {
         const int r = i / S, c = i - r * S;
         pm[i] = (r >= 1 && r <= M && c >= 1 && c <= M) ? msrc[(r - 1) * M + (c - 1)] : 0.f;
@@ -173,8 +182,8 @@ static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __res
     const bool empty = g.x1 <= g.x0;
     const int xe = empty ? -1 : (g.x1 < im_w ? g.x1 : g.x1 - 1);        // last column that can hold a transition (pseudo column x1)
     const int ncols = empty ? 0 : xe - g.x0 + 1;
-    uint32_t* my_counts = counts + (size_t)d * runs_cap;
-    uint32_t* my_pos = positions + (size_t)d * runs_cap;
+    uint32_t* my_counts = counts + d * runs_cap;
+    uint32_t* my_pos = positions + d * runs_cap;
     // one sweep of a column; EMIT(pos) is called in increasing order of the column-major position
 #define DT_SEGM_SWEEP(EMIT)                                                                                              \
     {                                                                                                                    \
@@ -256,7 +265,7 @@ static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __res
         if (threadIdx.x == 0) { atomicMax(overflow, m); num_counts[d] = m; str_len[d] = 0; }
         return;
     }
-    uint8_t* my_str = strings + (size_t)d * str_cap;
+    uint8_t* my_str = strings + d * str_cap;
     for (int i = lo_i; i < hi_i; ++i) {
         long long x = (long long)my_counts[i];
         if (i > 2) x -= (long long)my_counts[i - 2];
@@ -272,21 +281,29 @@ static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __res
     if (threadIdx.x == 0) { num_counts[d] = m; str_len[d] = total_chars; }
 }
 
-// gathers the per-detection strings into one contiguous buffer; offsets[D+1] (exclusive scan of str_len)
+// offsets[0..D] = exclusive scan of str_len[0..D) (offsets[D] = total), one block: each thread sums a contiguous chunk, a block scan
+// of the chunk sums gives each chunk's start
+static __global__ void __launch_bounds__(1024) segm_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ offsets) {
+    __shared__ long long scratch[33];
+    const int chunk = (D + blockDim.x - 1) / blockDim.x;
+    const int lo = min((int)threadIdx.x * chunk, D), hi = min(lo + chunk, D);
+    long long sum = 0;
+    for (int i = lo; i < hi; ++i) sum += str_len[i];
+    long long total;
+    long long run = block_scan_value(sum, scratch, &total);
+    for (int i = lo; i < hi; ++i) { offsets[i] = run; run += str_len[i]; }
+    if (threadIdx.x == 0) offsets[D] = total;
+}
+
+// gathers the per-slot strings into one contiguous buffer at the scanned offsets; one warp per slot
 static __global__ void __launch_bounds__(256) segm_compact_kernel(const uint8_t* __restrict__ strings, const int* __restrict__ str_len, int D,
-                                                                  int str_cap, uint8_t* __restrict__ packed, long long* __restrict__ offsets) {
-    __shared__ long long s_off;
-    const int d = blockIdx.x;
-    if (threadIdx.x == 0) {
-        long long o = 0;
-        for (int i = 0; i < d; ++i) o += str_len[i];
-        s_off = o;
-        offsets[d] = o;
-        if (d == D - 1) offsets[D] = o + str_len[d];
-    }
-    __syncthreads();
+                                                                  int str_cap, const long long* __restrict__ offsets, uint8_t* __restrict__ packed) {
+    const int d = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (d >= D) return;
     const int n = str_len[d];
-    for (int i = threadIdx.x; i < n; i += blockDim.x) packed[s_off + i] = strings[(size_t)d * str_cap + i];
+    uint8_t* dst = packed + offsets[d];
+    const uint8_t* src = strings + (size_t)d * str_cap;
+    for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
 // pasted binary masks [D, im_h, im_w] uint8 (for callers that want the image-sized mask rather than its RLE)

@@ -447,6 +447,21 @@ class detector(torch.nn.Module):
             out["masks"] = m.view(B, cap, m.shape[-2], m.shape[-1])
         return out
 
+    def detect_images(self, ims, target_size=800, max_size=1333, canvas=None, with_masks=None):
+        """uint8 BGR images [H,W,3] of any sizes (numpy or CUDA tensors) -> one (scores_final, boxes_final, boxes_per_class, cls_segms)
+        per image, in input order: what the eval notebooks compute for that image alone (image_to_blob(fpn_on=True), forward,
+        postprocess_output, mask_head, segm_results at the original size), for the whole list in one detect() launch and one batched
+        paste + RLE.  cls_segms is None without masks.  canvas=None fits the largest image; a fixed (Hc, Wc) lets one engine and one
+        captured graph serve every list.  FPN models only, like detect() with per-image sizes."""
+        from ..utils import blob, result_utils
+        if not self.use_rpn_head:
+            raise RuntimeError("detect_images() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois)")
+        if self.family != "fpn":
+            raise NotImplementedError("detect_images: per-image sizes are built for the FPN models only")
+        data, sizes, scales, orig = blob.images_to_batch(ims, target_size, max_size, canvas)
+        out = self.detect(data, scaling_factor=scales, with_masks=with_masks, image_sizes=sizes, original_sizes=orig)
+        return result_utils.batch_results(out, orig, num_classes=self.N_classes)
+
     def _launch_detect(self, eng, images, scaling_factor, last, use_table):
         if not images.is_cuda:
             images = self._upload(eng, images)

@@ -3,6 +3,7 @@ current stream); all compute happens in detectorch_b200/csrc.  Every function re
 tensors -- there is no CPU path."""
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -180,6 +181,81 @@ def segm_rle(masks, classes, boxes, im_h, im_w, thresh=0.5, expanded=False, num_
     nmax = int(n_h.max()) if D else 0
     cnt_h = counts[:, :max(nmax, 1)].cpu().numpy().view("uint32")
     return [cnt_h[d, :n_h[d]].copy() for d in range(D)], [str_h[offs_h[d]:offs_h[d + 1]] for d in range(D)]
+
+
+def to_host(*ts):
+    """Device tensors -> numpy arrays of the same dtypes and shapes, through ONE device-to-host copy (and so one synchronisation)."""
+    ts = [t.contiguous() for t in ts]
+    flat = torch.cat([t.reshape(-1).view(torch.uint8) for t in ts]).cpu().numpy()
+    out, o = [], 0
+    for t in ts:
+        n = t.numel() * t.element_size()
+        out.append(flat[o:o + n].view(str(t.dtype).replace("torch.", "")).reshape(tuple(t.shape)))
+        o += n
+    return out
+
+
+def segm_image_sizes(im_sizes, B):
+    """Host (height, width) RLE canvas per image -> int64 numpy [B, 2]: int() of each value, as the notebooks pass int(h), int(w)."""
+    v = im_sizes.detach().cpu().numpy() if torch.is_tensor(im_sizes) else np.asarray(im_sizes)
+    if v.ndim != 2 or v.shape != (B, 2):
+        raise ValueError("expected one (height, width) per image: shape [%d, 2], got %s" % (B, tuple(v.shape)))
+    v = v.astype(np.float64)
+    if not np.all(np.isfinite(v)):
+        raise ValueError("image sizes must be finite")
+    sz = np.array([[int(h), int(w)] for h, w in v], dtype=np.int64).reshape(B, 2)
+    if np.any(sz < 1) or np.any(sz[:, 0] * sz[:, 1] >= 2 ** 32):
+        raise ValueError("image sizes must be at least 1 x 1 and below 2^32 pixels")
+    return sz
+
+
+def segm_rle_batch_device(masks, classes, boxes, num_dets, im_sizes, thresh=0.5, runs_cap=4096, extra=()):
+    """The launch half of segm_rle_batch: -> (packed strings on the device, host copies of [offsets int64 [B*cap+1], num_dets [B]] + the
+    `extra` device tensors), all read in one synchronisation (after a grow-and-redo, one more per redo)."""
+    _need_cuda(masks, classes, boxes, num_dets)
+    if masks.dim() not in (4, 5) or boxes.dim() != 3 or boxes.size(2) != 4:
+        raise ValueError("segm_rle_batch: masks must be [B,cap,M,M] or [B,cap,K,M,M] and boxes [B,cap,4]")
+    B, cap, M = masks.size(0), masks.size(1), masks.size(-1)
+    if tuple(boxes.shape[:2]) != (B, cap) or masks.size(-2) != M:
+        raise ValueError("segm_rle_batch: masks %s and boxes %s disagree" % (tuple(masks.shape), tuple(boxes.shape)))
+    if (masks.dim() == 5) != (classes is not None) or (classes is not None and tuple(classes.shape) != (B, cap)):
+        raise ValueError("segm_rle_batch: [B,cap,K,M,M] masks need classes [B,cap]; [B,cap,M,M] masks take none")
+    sz = segm_image_sizes(im_sizes, B)
+    K = masks.size(2) if masks.dim() == 5 else 1
+    dev = masks.device
+    masks, boxes = masks.contiguous().float(), boxes.contiguous().float()
+    if classes is not None:
+        classes = classes.contiguous().to(torch.int32)
+    nd = torch.full((B,), cap, dtype=torch.int32, device=dev) if num_dets is None else num_dets.contiguous().to(torch.int32)
+    if B * cap == 0:
+        host = to_host(nd, *extra)
+        return torch.empty((0,), dtype=torch.uint8, device=dev), [np.zeros((B * cap + 1,), np.int64)] + host
+    sizes = torch.from_numpy(sz.astype(np.int32)).to(dev)
+    L = _lib.lib()
+    while True:
+        ws = torch.empty((L.dt_segm_batch_workspace_bytes(B, cap, runs_cap),), dtype=torch.uint8, device=dev)
+        strings = torch.empty((L.dt_segm_batch_strings_bytes(B, cap, runs_cap),), dtype=torch.uint8, device=dev)
+        offs = torch.empty((B * cap + 1,), dtype=torch.int64, device=dev)
+        over = torch.zeros((1,), dtype=torch.int32, device=dev)
+        ok = L.dt_segm_rle_batch(_p(masks), _p(classes), K, M, _p(boxes), _p(nd), _p(sizes), B, cap, int(sz[:, 0].max()), int(sz[:, 1].max()),
+                                 float(thresh), runs_cap, _p(strings), _p(offs), _p(over), _p(ws), _stream())
+        _lib.check(ok, "dt_segm_rle_batch")
+        host = to_host(offs, over, nd, *extra)
+        need = int(host[1][0])
+        if need == 0:
+            return strings, [host[0], host[2]] + host[3:]
+        runs_cap = max(2 * runs_cap, need + 1)     # a detection needed more runs than provisioned: grow and redo
+
+
+def segm_rle_batch(masks, classes, boxes, num_dets, im_sizes, thresh=0.5, runs_cap=4096):
+    """Mask paste + COCO RLE of a batch of images on the device (lib/utils/result_utils.py:170-228 for every image at once).
+    masks [B,cap,M,M] (the selected class, detect()'s 'masks') or [B,cap,K,M,M] with classes int32 [B,cap] selecting the plane;
+    boxes [B,cap,4] fp32 image-space boxes; num_dets int32 [B] live slots per image (detect()'s 'counts'; None = all);
+    im_sizes host [B,2] (height, width) of each image's RLE canvas.  -> per image, a list of RLE strings (bytes), one per live slot."""
+    strings, (offs, nd) = segm_rle_batch_device(masks, classes, boxes, num_dets, im_sizes, thresh, runs_cap)
+    cap = masks.size(1)
+    str_h = strings[:int(offs[-1])].cpu().numpy().tobytes() if offs[-1] > 0 else b""
+    return [[str_h[offs[b * cap + d]:offs[b * cap + d + 1]] for d in range(min(max(int(nd[b]), 0), cap))] for b in range(masks.size(0))]
 
 
 def segm_paste(masks, classes, boxes, im_h, im_w, thresh=0.5, expanded=False, num_dets=None):

@@ -1,7 +1,8 @@
 """Mirror of the hot-path part of the reference lib/utils/result_utils.py: postprocess_output (:76-94)
 and box_results_with_nms_and_limit (:96-168), computed by the engine's on-device detection stage
 (decode with weights (10,10,5,5), clip, score > 0.05, per-class NMS 0.5, top-100) and returned in the
-reference's numpy structures; and of segm_results (:170-228): mask paste + COCO RLE on the device."""
+reference's numpy structures; and of segm_results (:170-228): mask paste + COCO RLE on the device.  batch_results gives both, per
+image, for a whole detector.detect() batch."""
 import numpy as np
 import torch
 
@@ -120,3 +121,41 @@ def segm_results(cls_boxes, masks, ref_boxes, im_h, im_w, num_classes=81, M=14, 
         cls_segms[j] = [{'size': [int(im_h), int(im_w)], 'counts': strings[k + i].decode()} for i in range(n_per_class[j])]
         k += n_per_class[j]
     return cls_segms
+
+
+def batch_results(out, original_sizes, num_classes=81, thresh_binarize=0.5):
+    """detector.detect()'s padded output dict -> per image (scores_final, boxes_final, boxes_per_class, cls_segms): exactly what
+    postprocess_output and then segm_results(cls_boxes, masks, boxes_final, int(h_orig), int(w_orig), M) return for that image alone.
+    original_sizes [B,2]: each image's un-scaled (height, width); int() of each value is the RLE canvas, as in the notebooks.
+    cls_segms is None when `out` has no masks (Faster R-CNN).  The masks are pasted and encoded on the device for the whole batch in
+    one launch; boxes, scores, classes, counts and the offsets of the strings come back in one copy, the strings in one more."""
+    from .. import ops
+    B, cap = int(out["boxes"].shape[0]), int(out["boxes"].shape[1])
+    sizes = ops.segm_image_sizes(original_sizes, B)           # validated before anything is launched
+    fields = (out["boxes"], out["scores"], out["classes"], out["counts"])
+    masks = out.get("masks")
+    if masks is None:
+        boxes, scores, classes, counts = ops.to_host(*fields)
+        offs = str_h = None
+    else:
+        strings, host = ops.segm_rle_batch_device(masks, None, out["boxes"], out["counts"], sizes, thresh_binarize, extra=fields)
+        offs, (boxes, scores, classes, counts) = host[0], host[2:]
+        str_h = strings[:int(offs[-1])].cpu().numpy().tobytes() if offs[-1] > 0 else b""
+    results = []
+    for b in range(B):
+        n = min(max(int(counts[b]), 0), cap)
+        bx, sc, cl = boxes[b, :n].copy(), scores[b, :n].copy(), classes[b, :n]
+        # the slots of an image are class-major (the engine's detection stage emits them class by class), which segm_results assumes;
+        # class j's rows are then one slice [bounds[j-1], bounds[j]) of the image's detections
+        if np.any(np.diff(cl) < 0) or np.any((cl < 1) | (cl >= num_classes)):
+            raise RuntimeError("batch_results: the detections of image %d are not grouped by class in 1..%d" % (b, num_classes - 1))
+        bounds = np.searchsorted(cl, np.arange(1, num_classes + 1))
+        dets = np.hstack((bx, sc[:, None])).astype(np.float32, copy=False)
+        cls_boxes = [[]] + [dets[bounds[j - 1]:bounds[j]] for j in range(1, num_classes)]
+        cls_segms = None
+        if str_h is not None:
+            size = [int(sizes[b, 0]), int(sizes[b, 1])]
+            segs = [{'size': list(size), 'counts': str_h[offs[b * cap + d]:offs[b * cap + d + 1]].decode()} for d in range(n)]
+            cls_segms = [[]] + [segs[bounds[j - 1]:bounds[j]] for j in range(1, num_classes)]
+        results.append((sc, bx, cls_boxes, cls_segms))
+    return results

@@ -115,6 +115,25 @@ int dt_segm_paste(const float* masks, const int* classes, int num_mask_classes, 
                   const int* expanded_boxes, const int* num_dets_dev, int max_dets, int im_h, int im_w, float thresh_binarize,
                   uint8_t* out, dt_stream_t stream);
 
+/* The same paste + RLE for a whole batch of images, each with its own canvas size and detection count: the padded outputs of the
+ * fused engine (det_boxes, det_classes, det_counts, masks / masks_full) go in as they are, one launch covers every (image, slot).
+ * dt_segm_rle is the one-image case of this code.
+ *   masks          [batch, cap, M, M] (the detected class), or [batch, cap, num_mask_classes, M, M] with classes [batch, cap] selecting
+ *                  the plane (classes NULL for the first layout)
+ *   boxes          [batch, cap, 4] fp32 image-space boxes (expanded by (M+2)/M and truncated on the device)
+ *   num_dets_dev   int32 [batch]: live slots of each image; slots at or past it produce empty strings
+ *   im_sizes       int32 [batch, 2]: (im_h, im_w) of each image's RLE canvas, each within max_im_h x max_im_w (the host-known maxima
+ *                  size the shared-memory tables; an entry outside [1, max] gives that image empty strings)
+ *   strings        dt_segm_batch_strings_bytes() bytes: the strings of slot s = b * cap + d back to back; str_offsets [batch*cap+1] int64
+ *   overflow       device int: 0, or the number of runs a slot needed when runs_cap (or its string staging) was too small: grow and redo
+ * Run lengths and their counts stay in the workspace (dt_segm_batch_workspace_bytes()).  Returns 0 for a mask size outside [1, 126],
+ * max_im_h * max_im_w >= 2^32, tables beyond the shared-memory limit, batch > 65535, runs_cap < 2 or a NULL pointer. */
+int64_t dt_segm_batch_workspace_bytes(int batch, int cap, int runs_cap);
+int64_t dt_segm_batch_strings_bytes(int batch, int cap, int runs_cap);
+int dt_segm_rle_batch(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes, const int* num_dets_dev,
+                      const int* im_sizes, int batch, int cap, int max_im_h, int max_im_w, float thresh_binarize, int runs_cap,
+                      uint8_t* strings, int64_t* str_offsets, int* overflow, void* workspace, dt_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Image pre-processing (the step right before the path, SURVEY.md 8f rank 3).
  * Replaces: lib/utils/blob.py:57-87 prep_im_for_blob (float32, minus pixel_means, cv2.resize(fx=fy=im_scale, INTER_LINEAR)) fused
