@@ -489,6 +489,9 @@ void plan_buffers(Engine* e) {
         add_buf(e, "masks", {D, M, M});
         add_buf(e, "masks_full", {D, NC, M, M});
     }
+    // Fast R-CNN on the FPN body: each image's pre-computed proposals in original-image coordinates, which the ST_COLLECT op scales,
+    // deduplicates and maps to levels into rois / roi_levels / roi_counts (Engine.set_proposals).  Last, so no other offset moves.
+    if (!f.c4 && !c.use_rpn) { add_buf(e, "fast_props", {B, post, 4}); add_buf(e, "fast_prop_counts", {B}, 1); }
 }
 
 // ---- program -----------------------------------------------------------------------------------
@@ -621,6 +624,15 @@ cudaError_t fn_proposals(Engine* e, cudaStream_t s) {
 }
 cudaError_t fn_collect(Engine* e, cudaStream_t s) {
     collect_kernel<<<e->cfg.batch, 1024, 0, s>>>(e->col);
+    return cudaGetLastError();
+}
+cudaError_t fn_fast_props(Engine* e, cudaStream_t s) {
+    FastPropsParams P;
+    P.boxes = e->buf("fast_props"); P.counts = e->buf<int>("fast_prop_counts");
+    P.im_info = e->im_info(); P.scaling_factor = e->scaling_factor;
+    P.top_n = e->cfg.post_nms_top_n; P.k_min = e->fam.lv_min; P.k_max = e->fam.lv_max;
+    P.rois = e->buf("rois"); P.levels = e->buf<int>("roi_levels"); P.roi_counts = e->buf<int>("roi_counts");
+    fast_props_kernel<<<e->cfg.batch, 1024, (size_t)P.top_n * 9, s>>>(P);
     return cudaGetLastError();
 }
 // per-image counts: padded rows carry zero boxes (collect_kernel) -> harmless, fully defined output
@@ -909,6 +921,7 @@ bool build_program(Engine* e) {
     }
     if (!f.c4) add_fpn(pb);
     if (c.use_rpn) add_rpn(pb);
+    else if (!f.c4) pb.fn(ST_COLLECT, fn_fast_props);      // forward() fills the RoIs itself and skips this stage
     pb.img_stride = 0;      // everything below is RoI-shaped
     // ---- RoIAlign in collected order (detector.py:259-270)
     e->roi_lv.num_levels = f.lv_max - f.lv_min + 1;

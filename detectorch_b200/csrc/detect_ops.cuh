@@ -3,6 +3,8 @@
 //   rpn_select_*_kernel, rpn_proposals_kernel, rpn_nms_scan_kernel  top-k + decode + clip + filter + NMS(0.7)   generate_proposals.py:31-122
 //   collect_kernel         merge levels, top-N, FPN level map           collect_and_distribute...py:84-128,
 //                                                                       multilevel_rois.py:41-53
+//   fast_props_kernel      pre-computed proposals -> scaled, deduplicated preprocess_sample.py:37-47,61-69,
+//                          RoIs in hash order + FPN level               multilevel_rois.py:19-39
 //   softmax_split_kernel   class softmax + split cls/bbox               detector.py:277-284
 //   det_class_kernel / det_limit_kernel  decode, clip, score>0.05, per-class NMS(0.5), top-100
 //                                                                       result_utils.py:76-168, boxes.py:150-208
@@ -573,6 +575,67 @@ static __global__ void __launch_bounds__(1024) collect_kernel(const __grid_const
             r[0] = (float)b; r[1] = r[2] = r[3] = r[4] = 0.f;
             P.levels[(size_t)b * P.top_n + i] = 0;
         }
+    }
+    if (threadIdx.x == 0) P.roi_counts[b] = m;
+}
+
+// ---------------------------------------------------------------------------------- pre-computed proposals (Fast R-CNN, FPN)
+// preprocess_sample.py:37-47,61-69 followed by add_multilevel_rois_for_test and the roi_original_idx restore of forward(), per image:
+// p = box * scale in fp32 (numpy multiplies the float32 roidb boxes by the Python-float scale in float32), the hash of the rounded
+// p / 16, np.unique(return_index=True) -- ascending hash, first occurrence of each -- and the FPN level of each surviving p.
+// numpy sums r0*1e3 + r1*1e6 + r2*1e9 + r3*1e12 in float64, where every term and partial sum is an exact integer while |r| < 8998
+// (the host rejects larger coordinates); an exact int64 key therefore has the same equalities and the same order.
+struct FastPropsParams {
+    const float* boxes;      // [B, top_n, 4] original-image coordinates
+    const int* counts;       // [B]
+    const float* im_info;    // per-image scaling factor (image_info), null = scaling_factor
+    float scaling_factor;
+    int top_n, k_min, k_max;
+    float* rois;             // [B, top_n, 5] (batch idx, x1,y1,x2,y2) in hash order; rows >= count are (b, 0, 0, 0, 0) as collect_kernel leaves them
+    int* levels;             // [B, top_n] level index (lvl - k_min)
+    int* roi_counts;         // [B] number of distinct hashes
+};
+
+// grid B, 1024 threads, dynamic shared memory top_n * 9 bytes.  At most ~1000 boxes per image: the stable sort is a rank count over
+// shared memory (the rank of a first occurrence = the number of first occurrences with a smaller key).
+static __global__ void __launch_bounds__(1024) fast_props_kernel(const __grid_constant__ FastPropsParams P) {
+    extern __shared__ long long keys[];                                        // [top_n]
+    unsigned char* first = reinterpret_cast<unsigned char*>(keys + P.top_n);   // [top_n]
+    const int b = blockIdx.x;
+    const int n = min(max(P.counts[b], 0), P.top_n);
+    const float scale = image_info(P.im_info, b, 1, 0, 0, P.scaling_factor).scale;
+    const float* bx = P.boxes + (size_t)b * P.top_n * 4;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        long long k = 0, w = 1000;
+#pragma unroll
+        for (int c = 0; c < 4; ++c, w *= 1000) k += (long long)rintf(__fmul_rn(__fmul_rn(bx[i * 4 + c], scale), 0.0625f)) * w;
+        keys[i] = k;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const long long k = keys[i];
+        bool f = true;
+        for (int j = 0; j < i && f; ++j) f = keys[j] != k;
+        first[i] = f;
+    }
+    __syncthreads();
+    int m = 0;
+    for (int base = 0; base < n; base += blockDim.x) m += __syncthreads_count(base + threadIdx.x < n && first[base + threadIdx.x]);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        if (!first[i]) continue;
+        const long long k = keys[i];
+        int u = 0;
+        for (int j = 0; j < n; ++j) u += first[j] & (keys[j] < k);
+        const float4 p = make_float4(__fmul_rn(bx[i * 4 + 0], scale), __fmul_rn(bx[i * 4 + 1], scale), __fmul_rn(bx[i * 4 + 2], scale),
+                                     __fmul_rn(bx[i * 4 + 3], scale));
+        float* r = P.rois + ((size_t)b * P.top_n + u) * 5;
+        r[0] = (float)b; r[1] = p.x; r[2] = p.y; r[3] = p.z; r[4] = p.w;
+        P.levels[(size_t)b * P.top_n + u] = fpn_level(p, P.k_min, P.k_max) - P.k_min;
+    }
+    for (int i = m + threadIdx.x; i < P.top_n; i += blockDim.x) {
+        float* r = P.rois + ((size_t)b * P.top_n + i) * 5;
+        r[0] = (float)b; r[1] = r[2] = r[3] = r[4] = 0.f;
+        P.levels[(size_t)b * P.top_n + i] = 0;
     }
     if (threadIdx.x == 0) P.roi_counts[b] = m;
 }

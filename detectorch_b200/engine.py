@@ -5,6 +5,7 @@ import ctypes
 import os
 import weakref
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -117,6 +118,22 @@ def fold_bn_running_stats(sd, eps=1e-5):
         out[pre + ".weight"] = (g * inv * (1.0 + eps) ** 0.5).float()
         out[pre + ".bias"] = (b - mean * g * inv).float()
     return out
+
+
+def pad_proposals(boxes_list, batch, cap):
+    """Per-image [n_b, 4] float32 boxes -> (float32 [batch, cap, 4] block with zero rows past n_b, int32 [batch] counts): the layout of
+    the engine's "fast_props" / "fast_prop_counts" buffers (no GPU needed)."""
+    if len(boxes_list) != batch:
+        raise ValueError("set_proposals: %d proposal arrays for %d images" % (len(boxes_list), batch))
+    block = np.zeros((batch, cap, 4), dtype=np.float32)
+    counts = np.zeros((batch,), dtype=np.int32)
+    for b, bx in enumerate(boxes_list):
+        bx = np.asarray(bx, dtype=np.float32).reshape(-1, 4)
+        if bx.shape[0] > cap:
+            raise ValueError("set_proposals: %d proposals for image %d exceed the engine capacity %d" % (bx.shape[0], b, cap))
+        block[b, :bx.shape[0]] = bx
+        counts[b] = bx.shape[0]
+    return block, counts
 
 
 class Engine:
@@ -276,6 +293,17 @@ class Engine:
     def clear_image_info(self):
         """Back to whole-canvas images with the scalar scaling factor."""
         _lib.check(self.L.dt_engine_use_image_info(self.h, 0), "dt_engine_use_image_info")
+
+    def set_proposals(self, boxes_list):
+        """Fast R-CNN on the FPN body (engine built with use_rpn=False): one float32 [n_b, 4] array of pre-computed proposals per image, in
+        original-image coordinates (the roidb's dbentry['boxes']).  Stage ST_COLLECT scales them by each image's scaling factor, removes
+        the duplicates as preprocess_sample does and writes rois / roi_levels / roi_counts.  Written on the current stream like
+        set_image_info, so a run still queued never sees them and a captured graph replays with the latest ones.  The caller validates
+        the boxes (detector.check_proposals)."""
+        block, counts = pad_proposals(boxes_list, self.cfg.batch, self.cfg.post_nms_top_n)
+        with torch.cuda.device(self.device):
+            self.buffer("fast_props").copy_(torch.from_numpy(block).pin_memory(), non_blocking=True)      # pinned blocks are not reused
+            self.buffer("fast_prop_counts").copy_(torch.from_numpy(counts).pin_memory(), non_blocking=True)   # before their copies ran
 
     def profile(self, image, scaling_factor=1.0, first=0, last=11):
         """One event-bracketed pass: list of (ms, algorithmic_flops, stage, block_n) per launch."""

@@ -405,7 +405,44 @@ class detector(torch.nn.Module):
                 raise ValueError("detect: original sizes must be positive")
         return net, sf, orig
 
-    def detect(self, images, scaling_factor=1.0, with_masks=None, image_sizes=None, original_sizes=None):
+    # Fast R-CNN batches: proposals per image (the engine's post_nms_top_n); |rint(box * scale / 16)| bound under which the float64 hash
+    # r0*1e3 + r1*1e6 + r2*1e9 + r3*1e12 of preprocess_sample.remove_dup_prop is exact (8998 * 1001001001000 < 2**53)
+    FAST_MAX_PROPOSALS = 1000
+    FAST_MAX_HASH_COORD = 8990
+
+    @staticmethod
+    def _check_proposals(proposals, scales):
+        """Host-side check of detect(proposals=): one float32 [n_b, 4] array (numpy or CPU tensor) of original-image boxes per image,
+        scales [B] the images' scaling factors.  -> list of float32 numpy arrays."""
+        if not isinstance(proposals, (list, tuple)):
+            raise TypeError("detect: proposals must be a list with one float32 [n, 4] array per image")
+        B = len(scales)
+        if len(proposals) != B:
+            raise ValueError("detect: %d proposal arrays for %d images" % (len(proposals), B))
+        out = []
+        for b, p in enumerate(proposals):
+            if torch.is_tensor(p):
+                p = p.detach().cpu().numpy()
+            if not isinstance(p, np.ndarray) or p.dtype != np.float32:
+                raise TypeError("detect: the proposals of image %d must be a float32 array (the roidb's boxes), got %s" %
+                                (b, getattr(p, "dtype", type(p).__name__)))
+            if p.ndim != 2 or p.shape[1] != 4:
+                raise ValueError("detect: the proposals of image %d must be [n, 4], got %s" % (b, tuple(p.shape)))
+            if p.shape[0] > detector.FAST_MAX_PROPOSALS:
+                raise ValueError("detect: %d proposals for image %d; at most %d per image" % (p.shape[0], b, detector.FAST_MAX_PROPOSALS))
+            if not np.all(np.isfinite(p)):
+                raise ValueError("detect: the proposals of image %d are not all finite" % b)
+            if np.any(p[:, 2] < p[:, 0]) or np.any(p[:, 3] < p[:, 1]):
+                raise ValueError("detect: the proposals of image %d must have x2 >= x1 and y2 >= y1" % b)
+            # the scaled coordinates exactly as preprocess_sample computes them (float32 boxes * float32 scale), then their hash digits
+            r = np.round((p * np.float32(scales[b])) * np.float32(0.0625))
+            if r.size and np.abs(r).max() > detector.FAST_MAX_HASH_COORD:
+                raise ValueError("detect: the proposals of image %d reach %g px after scaling; the duplicate hash is exact up to %d px" %
+                                 (b, float(np.abs(p * np.float32(scales[b])).max()), 16 * detector.FAST_MAX_HASH_COORD))
+            out.append(np.ascontiguousarray(p))
+        return out
+
+    def detect(self, images, scaling_factor=1.0, with_masks=None, image_sizes=None, original_sizes=None, proposals=None):
         """Fused path: images [B,3,H,W] -> dict of padded per-image detections (boxes [B,cap,4], scores, classes, counts,
         masks [B,cap,28,28] of the detected class).  No host synchronisation inside.
         `images` may live in (pinned) HOST memory: the upload then goes through two device staging buffers on a copy stream, so the
@@ -416,18 +453,35 @@ class detector(torch.nn.Module):
         slot -- its own im_list_to_blob(fpn_on=True) size, a multiple of 32 (utils.blob.images_to_batch builds such batches).
         `scaling_factor` may then be one value per image, and original_sizes [B,2] gives each image's un-scaled size for the final clip
         (default: size / scaling_factor).  Image b's results equal a batch-1 run of that image alone; the canvas outside the images is
-        ignored.  One captured graph serves every size mix on the same canvas."""
-        if not self.use_rpn_head:
-            raise RuntimeError("detect() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois)")
-        table = self._image_table(images.size(0), images.size(2), images.size(3), scaling_factor, image_sizes, original_sizes)
+        ignored.  One captured graph serves every size mix on the same canvas.
+
+        Fast R-CNN on the FPN body (eval_fast_FPN.ipynb's model): `proposals` is one float32 [n_b, 4] array per image of pre-computed
+        boxes in original-image coordinates (the roidb's dbentry['boxes'], at most 1000).  They are scaled, deduplicated and mapped to
+        the FPN levels on the device, as preprocess_sample(fpn_on=True) does on the host, and each image's detections equal
+        forward(image, [rois_fpn2..5], roi_original_idx) + postprocess_output of that image alone.  No masks."""
+        if proposals is not None:
+            if self.use_rpn_head:
+                raise ValueError("detect: proposals= is for the Fast R-CNN models; this model computes its own with the RPN")
+            if self.family != "fpn":
+                raise NotImplementedError("detect: batched Fast R-CNN is built for the FPN models only")
+        elif not self.use_rpn_head:
+            raise RuntimeError("detect() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois) or detect(proposals=)")
+        B = images.size(0)
+        table = self._image_table(B, images.size(2), images.size(3), scaling_factor, image_sizes, original_sizes)
         if table is not None and self.family != "fpn":
             raise NotImplementedError("detect: per-image sizes and scaling factors are built for the FPN models only")
-        eng = self.engine_for(images.size(0), images.size(2), images.size(3))
+        if proposals is not None:
+            proposals = self._check_proposals(proposals, np.full(B, float(scaling_factor)) if table is None else table[1])
+            eng = self.engine_for(B, images.size(2), images.size(3), post_nms_top_n=self.FAST_MAX_PROPOSALS)
+        else:
+            eng = self.engine_for(B, images.size(2), images.size(3))
         eng.set_original_size(0, 0)          # clip to the network input / scaling_factor (a previous postprocess_output may have set an image size)
         scaling_factor = float(scaling_factor) if table is None else 1.0      # with the table its per-image factors apply
         eng.last_scaling_factor = scaling_factor
         with_masks = self.use_mask_head if with_masks is None else with_masks
         last = ST_MASK_OUT if with_masks else ST_DETECT
+        if proposals is not None:
+            eng.set_proposals(proposals)     # on the current stream, like the table
         if table is not None:
             eng.set_image_info(*table)       # on the current stream, after every run already queued there
         try:
@@ -447,19 +501,24 @@ class detector(torch.nn.Module):
             out["masks"] = m.view(B, cap, m.shape[-2], m.shape[-1])
         return out
 
-    def detect_images(self, ims, target_size=800, max_size=1333, canvas=None, with_masks=None):
+    def detect_images(self, ims, target_size=800, max_size=1333, canvas=None, with_masks=None, proposals=None):
         """uint8 BGR images [H,W,3] of any sizes (numpy or CUDA tensors) -> one (scores_final, boxes_final, boxes_per_class, cls_segms)
         per image, in input order: what the eval notebooks compute for that image alone (image_to_blob(fpn_on=True), forward,
         postprocess_output, mask_head, segm_results at the original size), for the whole list in one detect() launch and one batched
         paste + RLE.  cls_segms is None without masks.  canvas=None fits the largest image; a fixed (Hc, Wc) lets one engine and one
-        captured graph serve every list.  FPN models only, like detect() with per-image sizes."""
+        captured graph serve every list.  FPN models only, like detect() with per-image sizes.
+        The Fast R-CNN FPN model takes `proposals`, one float32 [n_b, 4] array of original-image boxes per image (see detect()), and
+        returns what eval_fast_FPN.ipynb files per image: (scores_final, boxes_final, boxes_per_class, None)."""
         from ..utils import blob, result_utils
-        if not self.use_rpn_head:
-            raise RuntimeError("detect_images() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois)")
+        if proposals is not None and self.use_rpn_head:
+            raise ValueError("detect_images: proposals= is for the Fast R-CNN models; this model computes its own with the RPN")
+        if proposals is None and not self.use_rpn_head:
+            raise RuntimeError("detect_images() is the fused RPN path; Fast R-CNN configurations go through forward(image, rois) or "
+                               "detect_images(ims, proposals=)")
         if self.family != "fpn":
             raise NotImplementedError("detect_images: per-image sizes are built for the FPN models only")
         data, sizes, scales, orig = blob.images_to_batch(ims, target_size, max_size, canvas)
-        out = self.detect(data, scaling_factor=scales, with_masks=with_masks, image_sizes=sizes, original_sizes=orig)
+        out = self.detect(data, scaling_factor=scales, with_masks=with_masks, image_sizes=sizes, original_sizes=orig, proposals=proposals)
         return result_utils.batch_results(out, orig, num_classes=self.N_classes)
 
     def _launch_detect(self, eng, images, scaling_factor, last, use_table):

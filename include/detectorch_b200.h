@@ -203,7 +203,12 @@ typedef struct dt_engine_config {
                                     0 = separable / FMA fast path (fp32 re-association only, ~1e-7 relative) */
     int model_type;              /* 0 = R-50/101-FPN + RPN (+ '1up4convs' mask head); 1 = R-50/101-C4 (res5 head, 'upshare' mask head) */
     int use_rpn;                 /* 1 = Faster/Mask R-CNN (RPN head + proposal generation on the device), 0 = Fast R-CNN with pre-computed
-                                    proposals (eval_fast.ipynb / eval_fast_FPN.ipynb): the caller fills `rois` (+ `roi_levels` for FPN), `roi_counts` */
+                                    proposals (eval_fast.ipynb / eval_fast_FPN.ipynb): the caller fills `rois` (+ `roi_levels` for FPN), `roi_counts`.
+                                    FPN engines without the RPN can instead take the raw proposals: float32 "fast_props" [batch,
+                                    post_nms_top_n, 4] (original-image coordinates) and int32 "fast_prop_counts" [batch]; stage 4 then
+                                    scales them by each image's scaling factor, drops the duplicates of preprocess_sample.remove_dup_prop
+                                    (spatial scale 1/16) and writes the survivors in its order, with their FPN levels, to `rois` /
+                                    `roi_levels` / `roi_counts`.  The host must keep |box * scale / 16| below 8990 (exact hash). */
     int conv_kind;               /* 0 = three-term product on the kind::f16 pipe (fp16 hi/lo halves, default: twice the tf32 issue rate; an
                                     activation >= 65504 raises the int32 buffer "range_flag", which every run that starts at the first stage clears
                                     before it launches anything), 1 = 3xTF32 (no range limit) */
@@ -245,7 +250,7 @@ int dt_engine_set_original_size(dt_engine_t e, float orig_h, float orig_w);
  * batch-1 run of that image at its own size; the scaling_factor argument of dt_engine_run is ignored while the table is on.
  * enabled = 0 returns to whole-canvas images and the scalar scaling factor / dt_engine_set_original_size. */
 int dt_engine_use_image_info(dt_engine_t e, int enabled);
-/* stages: 0 trunk, 1 FPN, 2 RPN convs, 3 proposals, 4 collect, 5 RoIAlign(box), 6 box head, 7 detect (decode+NMS+limit),
+/* stages: 0 trunk, 1 FPN, 2 RPN convs, 3 proposals, 4 collect (FPN Fast R-CNN: pre-computed proposals -> RoIs), 5 RoIAlign(box), 6 box head, 7 detect (decode+NMS+limit),
  *         8 mask RoIs, 9 RoIAlign(mask), 10 mask convs, 11 mask output */
 int dt_engine_run(dt_engine_t e, const float* image_nchw, float scaling_factor, int first_stage, int last_stage, dt_stream_t stream);
 int dt_engine_count_launches(dt_engine_t e, int first_stage, int last_stage);
