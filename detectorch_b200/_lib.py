@@ -49,6 +49,13 @@ SIGNATURES = {
     "dt_conv2d_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                c_void_p, c_int, c_void_p]),
+    "dt_coco_gt_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
+    "dt_coco_gt_build": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
+    "dt_coco_eval_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int64]),
+    "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
+                             c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_void_p, c_void_p]),
 }
 
 

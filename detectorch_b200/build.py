@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libdetectorch_b200.so")
-SOURCES = ["capi_ops.cu", "capi_engine.cu"]
+SOURCES = ["capi_ops.cu", "capi_engine.cu", "capi_coco.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DNDEBUG"]
 
 

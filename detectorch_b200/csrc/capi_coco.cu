@@ -1,0 +1,56 @@
+// detectorch_b200 -- C-ABI entry points of the COCO evaluation (coco_eval.cuh; include/detectorch_b200.h).
+#include <stdio.h>
+
+#include "../../include/detectorch_b200.h"
+#include "coco_eval.cuh"
+#include "common.cuh"
+
+using namespace dt;
+
+extern "C" int64_t dt_coco_gt_workspace_bytes(int64_t num_parts, int64_t num_points, int64_t num_upsampled) {
+    if (num_parts < 0 || num_points < 0 || num_upsampled < 0) return 0;
+    return 4 * (num_points + 4 * num_upsampled + 3 * num_parts);
+}
+
+extern "C" int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t* parts, const double* xy, const uint32_t* ucounts,
+                                const char* chars, void* workspace, uint32_t* out_counts, uint32_t* tmp_counts, int64_t* out_len,
+                                double* out_box, dt_stream_t stream) {
+    if (num_anns < 0) { fprintf(stderr, "dt_coco_gt_build: negative annotation count\n"); return 0; }
+    if (num_anns == 0) return 1;
+    if (!anns || !parts || !out_counts || !tmp_counts || !out_len || !out_box) {
+        fprintf(stderr, "dt_coco_gt_build: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_gt_launch(num_anns, anns, parts, xy, ucounts, chars, reinterpret_cast<int*>(workspace), out_counts, tmp_counts,
+                                 out_len, out_box, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts,
+                                                int64_t num_order) {
+    if (num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 || num_gts < 0 || num_order < 0) return 0;
+    return (int64_t)coco_eval_ws(num_dets, num_chars, kept, num_ious, num_gts, num_order).total;
+}
+
+extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, const int64_t* pairs, const int64_t* cat_gt,
+                            const int64_t* cat_kept, const int64_t* order_off, int64_t num_dets, const double* det_f, const int64_t* det_i,
+                            const char* det_chars, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
+                            const double* gt_f, const int64_t* gt_i, const uint32_t* gt_counts, const double* params, double* precision,
+                            double* recall, double* scores, double* ious, void* workspace, dt_stream_t stream) {
+    if ((iou_type != 0 && iou_type != 1) || num_images < 0 || num_cats < 0 || num_active < 0 || num_dets < 0 || num_chars < 0 || kept < 0 ||
+        num_ious < 0 || num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || (int64_t)num_cats * 120 >= (1ll << 31)) {
+        fprintf(stderr, "dt_coco_eval: bad sizes\n");
+        return 0;
+    }
+    if (num_cats == 0) return 1;
+    if (!cat_gt || !cat_kept || !order_off || !params || !precision || !recall || !scores || (num_gts > 0 && (!gt_f || !gt_i)) ||
+        (iou_type == 1 && num_gts > 0 && !gt_counts) || (num_dets > 0 && (!pairs || !det_f || !det_i || !workspace)) ||
+        (iou_type == 1 && num_chars > 0 && !det_chars)) {
+        fprintf(stderr, "dt_coco_eval: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_eval_launch(iou_type, num_images, num_cats, num_active, pairs, cat_gt, cat_kept, order_off, num_dets, det_f, det_i,
+                                   det_chars, num_chars, kept, num_ious, num_gts, num_order, gt_f, gt_i, gt_counts, params, precision, recall,
+                                   scores, ious, workspace, (cudaStream_t)stream));
+    return 1;
+}

@@ -1,0 +1,490 @@
+// detectorch_b200 -- COCO box and mask evaluation on the device: pycocotools' COCOeval (iouType 'bbox' / 'segm', default Params)
+// restated kernel by kernel so that precision, recall and scores come out bit for bit as COCOeval.evaluate() + accumulate() give them.
+//
+//   coco_gt_kernel        one CTA per annotation: polygon -> RLE (maskApi rleFrPoly: x5 upsampling, edge walk, y-boundary points,
+//                         sort, run lengths) and union of the parts (rleMerge); uncompressed RLE copied; compressed RLE decoded;
+//                         rleToBbox of the result.  Runs once per ground-truth set.
+//   coco_det_rle_kernel   one thread per detection: rleFrString of its compressed string, maskUtils.area, rleToBbox.
+//   coco_pair_kernel      one CTA per (category, image) pair with detections: stable score sort cut to 100 (computeIoU), the IoU
+//                         matrix (bbIou / rleIou, double), then one thread per (area range, IoU threshold) runs evaluateImg's greedy
+//                         matching and writes a 2-bit state (matched, ignored) per detection.
+//   coco_rank_kernel      one thread per kept detection: its position in accumulate()'s stable sort by -score of the category's
+//                         detections concatenated in image order, for each maxDets cut.
+//   coco_accum_kernel     one thread per (category, area, maxDets, threshold): cumulative tp / fp, recall, the right-to-left
+//                         precision envelope and searchsorted(rc, recThrs, 'left'), in float64 as numpy computes them.
+//
+// Every product that feeds a sum is an explicit __dmul_rn / __dadd_rn: the C code it restates is compiled without contraction.
+// Pairs are ordered category-major, image-minor (COCOeval's evalImgs order), so a category's kept detections are one contiguous
+// range in image order, which is the concatenation accumulate() sorts.
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+namespace dt {
+
+constexpr int kCocoAreas = 4, kCocoThrs = 10, kCocoRecThrs = 101, kCocoMaxDets = 3, kCocoKeep = 100;
+constexpr int kCocoStates = kCocoAreas * kCocoThrs;   // per kept detection: one state byte per (area range, threshold)
+// params block (double): area ranges [4][2], IoU thresholds already clipped to 1 - 1e-10 [10], recall thresholds [101]
+constexpr int kCocoParAreas = 0, kCocoParThrs = 8, kCocoParRec = 18, kCocoParams = 119;
+// annotation table (int64 per annotation): kind, h, w, first part, number of parts, output offset
+constexpr int kCocoAnnCols = 6;
+enum { kCocoPoly = 0, kCocoCounts = 1, kCocoString = 2 };
+// part table (int64 per part): first element (xy pair / count / char), number of elements, int32 workspace offset, upsampled points
+// of a polygon (maskApi's m after the edge walk; the host counts it from the same rounding).  A polygon part of k points and m
+// upsampled points takes k + 4 m + 3 ints of workspace.
+constexpr int kCocoPartCols = 4;
+// ground truth in pair order: f64 [box x y w h, area, rle box x y w h]; i64 [rle offset, rle length, h, w, iscrowd, id != 0]
+constexpr int kCocoGtF = 9, kCocoGtI = 6;
+// detections in pair order: f64 [score, box x y w h]; i64 [char offset, char count, h, w]
+constexpr int kCocoDetF = 5, kCocoDetI = 4;
+// active pair table (int64): pair index (category * images + image), first detection, D, first gt, G, first kept slot, first IoU
+constexpr int kCocoPairCols = 7;
+
+// x86 cvttsd2si: truncation, and INT_MIN for NaN or out of range (what the host build of maskApi.c does with (int) of a double)
+__host__ __device__ __forceinline__ int coco_trunc(double v) {
+    return (v >= -2147483648.0 && v < 2147483648.0) ? (int)v : (int)0x80000000;
+}
+
+__device__ __forceinline__ uint32_t coco_umin(uint32_t a, uint32_t b) { return a < b ? a : b; }
+__device__ __forceinline__ uint32_t coco_umax(uint32_t a, uint32_t b) { return a > b ? a : b; }
+
+// maskApi rleToBbox of one RLE (uint arithmetic as in C)
+__device__ void coco_rle_box(const uint32_t* cnts, int64_t m, uint32_t h, uint32_t w, double* bb) {
+    m = (m / 2) * 2;
+    if (m == 0) { bb[0] = bb[1] = bb[2] = bb[3] = 0; return; }
+    uint32_t xs = w, ys = h, xe = 0, ye = 0, cc = 0;
+    for (int64_t j = 0; j < m; j++) {
+        cc += cnts[j];
+        const uint32_t t = cc - (uint32_t)(j % 2), y = t % h, x = (t - y) / h;
+        xs = coco_umin(xs, x); xe = coco_umax(xe, x); ys = coco_umin(ys, y); ye = coco_umax(ye, y);
+    }
+    bb[0] = xs; bb[2] = (double)(uint32_t)(xe - xs + 1);
+    bb[1] = ys; bb[3] = (double)(uint32_t)(ye - ys + 1);
+}
+
+// maskApi bbIou of one (detection, gt) pair, xywh
+__device__ __forceinline__ double coco_bb_iou(const double* D, const double* G, bool crowd) {
+    const double ga = __dmul_rn(G[2], G[3]), da = __dmul_rn(D[2], D[3]);
+    const double w = __dsub_rn(fmin(__dadd_rn(D[2], D[0]), __dadd_rn(G[2], G[0])), fmax(D[0], G[0]));
+    if (w <= 0) return 0;
+    const double h = __dsub_rn(fmin(__dadd_rn(D[3], D[1]), __dadd_rn(G[3], G[1])), fmax(D[1], G[1]));
+    if (h <= 0) return 0;
+    const double i = __dmul_rn(w, h), u = crowd ? da : __dsub_rn(__dadd_rn(da, ga), i);
+    return __ddiv_rn(i, u);
+}
+
+// maskApi rleIou of one pair: box IoU first, the run merge only where the boxes overlap
+__device__ double coco_rle_iou(const uint32_t* dc, int64_t dm, const double* dbox, int64_t dh, int64_t dw, const uint32_t* gc, int64_t gm,
+                               const double* gbox, int64_t gh, int64_t gw, bool crowd) {
+    const double o = coco_bb_iou(dbox, gbox, crowd);
+    if (!(o > 0)) return o;
+    if (dh != gh || dw != gw) return -1;
+    uint32_t ca = dc[0], cb = gc[0], c, ct = 1, i = 0, u = 0;
+    int64_t a = 1, b = 1;
+    bool va = false, vb = false;
+    while (ct > 0) {
+        c = coco_umin(ca, cb);
+        if (va || vb) { u += c; if (va && vb) i += c; }
+        ct = 0;
+        ca -= c; if (!ca && a < dm) { ca = dc[a++]; va = !va; } ct += ca;
+        cb -= c; if (!cb && b < gm) { cb = gc[b++]; vb = !vb; } ct += cb;
+    }
+    if (i == 0) u = 1;
+    else if (crowd) { u = 0; for (int64_t j = 1; j < dm; j += 2) u += dc[j]; }
+    return __ddiv_rn((double)i, (double)u);
+}
+
+// maskApi rleFrString of one string: returns the number of counts written to cnts
+__device__ int64_t coco_rle_from_string(const char* s, int64_t len, uint32_t* cnts) {
+    int64_t m = 0, p = 0;
+    while (p < len) {
+        long long x = 0;
+        int k = 0, more = 1;
+        while (more) {
+            const int c = s[p] - 48;
+            x |= (long long)(int)((c & 0x1f) << (5 * k));
+            more = c & 0x20; p++; k++;
+            if (!more && (c & 0x10)) x |= (long long)(int)(0xffffffffu << (5 * k));
+        }
+        if (m > 2) x += (long long)cnts[m - 2];
+        cnts[m++] = (uint32_t)x;
+    }
+    return m;
+}
+
+// maskApi rleMerge step (union) of A and B into out: returns the number of counts
+__device__ int64_t coco_rle_union(const uint32_t* A, int64_t am, const uint32_t* B, int64_t bm, uint32_t* out) {
+    uint32_t ca = A[0], cb = B[0], c, cc = 0, ct = 1;
+    int v = 0, va = 0, vb = 0, vp;
+    int64_t a = 1, b = 1, m = 0;
+    while (ct > 0) {
+        c = coco_umin(ca, cb); cc += c; ct = 0;
+        ca -= c; if (!ca && a < am) { ca = A[a++]; va = !va; } ct += ca;
+        cb -= c; if (!cb && b < bm) { cb = B[b++]; vb = !vb; } ct += cb;
+        vp = v; v = va || vb;
+        if (v != vp || ct == 0) { out[m++] = cc; cc = 0; }
+    }
+    return m;
+}
+
+__device__ __forceinline__ int coco_up(double v) { return coco_trunc(__dadd_rn(__dmul_rn(5.0, v), .5)); }
+
+// rleFrPoly of one polygon of k points, cooperatively by the CTA.  ws: the part's int32 workspace (k + 4 m_up + 3 ints, m_up the
+// number of upsampled boundary points); thread 0 gets the part's run lengths at *out (inside ws) and their number in *out_m.
+__device__ void coco_poly_rle(const double* xy, int k, uint32_t h, uint32_t w, int* ws, int64_t m_up, uint32_t** out, int64_t* out_m) {
+    __shared__ int s_n;
+    int* eoff = ws;                          // k + 1 edge offsets into the upsampled points
+    int* u = eoff + k + 1;
+    int* v = u + m_up;
+    uint32_t* a = reinterpret_cast<uint32_t*>(v + m_up);   // y-boundary points, then h * w      (m_up + 1)
+    uint32_t* srt = a + m_up + 1;                           // sorted, then differenced and packed (m_up + 1)
+    const int tid = threadIdx.x, nt = blockDim.x;
+    if (tid == 0) {
+        int o = 0;
+        for (int j = 0; j < k; j++) {
+            eoff[j] = o;
+            const int j1 = j + 1 < k ? j + 1 : 0;
+            const int dx = abs(coco_up(xy[2 * j1]) - coco_up(xy[2 * j])), dy = abs(coco_up(xy[2 * j1 + 1]) - coco_up(xy[2 * j + 1]));
+            o += (int)coco_umax((uint32_t)dx, (uint32_t)dy) + 1;
+        }
+        eoff[k] = o;
+        s_n = 0;
+    }
+    __syncthreads();
+    const int m = eoff[k];
+    for (int i = tid; i < m; i += nt) {
+        int lo = 0, hi = k - 1;              // the edge j with eoff[j] <= i < eoff[j + 1]
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (eoff[mid] <= i) lo = mid; else hi = mid - 1; }
+        const int j = lo, d = i - eoff[j], j1 = j + 1 < k ? j + 1 : 0;
+        int xs = coco_up(xy[2 * j]), xe = coco_up(xy[2 * j1]), ys = coco_up(xy[2 * j + 1]), ye = coco_up(xy[2 * j1 + 1]);
+        const int dx = abs(xe - xs), dy = abs(ys - ye);
+        const bool flip = (dx >= dy && xs > xe) || (dx < dy && ys > ye);
+        if (flip) { int t = xs; xs = xe; xe = t; t = ys; ys = ye; ye = t; }
+        const double s = dx >= dy ? __ddiv_rn((double)(ye - ys), (double)dx) : __ddiv_rn((double)(xe - xs), (double)dy);
+        if (dx >= dy) {
+            const int t = flip ? dx - d : d;
+            u[i] = t + xs; v[i] = coco_trunc(__dadd_rn(__dadd_rn((double)ys, __dmul_rn(s, (double)t)), .5));
+        } else {
+            const int t = flip ? dy - d : d;
+            v[i] = t + ys; u[i] = coco_trunc(__dadd_rn(__dadd_rn((double)xs, __dmul_rn(s, (double)t)), .5));
+        }
+    }
+    __syncthreads();
+    // y-boundary points and downsampling; their order does not matter (they are sorted next)
+    for (int j = 1 + tid; j < m; j += nt) {
+        if (u[j] == u[j - 1]) continue;
+        double xd = (double)(u[j] < u[j - 1] ? u[j] : u[j] - 1);
+        xd = (xd + .5) / 5.0 - .5;
+        if (floor(xd) != xd || xd < 0 || xd > (double)(w - 1)) continue;
+        double yd = (double)(v[j] < v[j - 1] ? v[j] : v[j - 1]);
+        yd = (yd + .5) / 5.0 - .5;
+        if (yd < 0) yd = 0; else if (yd > (double)h) yd = h;
+        yd = ceil(yd);
+        a[atomicAdd(&s_n, 1)] = (uint32_t)((int)xd * (int)h + (int)yd);
+    }
+    __syncthreads();
+    const int n = s_n + 1;
+    if (tid == 0) a[n - 1] = h * w;
+    __syncthreads();
+    for (int i = tid; i < n; i += nt) {      // rank sort (equal values keep their index order: the sorted multiset is unique)
+        const uint32_t x = a[i];
+        int r = 0;
+        for (int j = 0; j < n; j++) r += (a[j] < x) || (a[j] == x && j < i);
+        srt[r] = x;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        uint32_t p = 0;
+        for (int j = 0; j < n; j++) { const uint32_t t = srt[j]; srt[j] -= p; p = t; }
+        int j = 0, mm = 0;
+        srt[mm++] = srt[j++];
+        while (j < n) {
+            if (srt[j] > 0) srt[mm++] = srt[j++];
+            else { j++; if (j < n) srt[mm - 1] += srt[j++]; }
+        }
+        *out = srt; *out_m = mm;
+    }
+    __syncthreads();
+}
+
+// one CTA per annotation.  out_cnts / tmp_cnts: same layout, capacity per annotation = the distance to the next one's offset
+__global__ void coco_gt_kernel(const int64_t* __restrict__ ann, const int64_t* __restrict__ parts, const double* __restrict__ xy,
+                               const uint32_t* __restrict__ ucounts, const char* __restrict__ chars, int* __restrict__ ws,
+                               uint32_t* __restrict__ out_cnts, uint32_t* __restrict__ tmp_cnts, int64_t* __restrict__ out_len,
+                               double* __restrict__ out_box) {
+    const int64_t* A = ann + (int64_t)blockIdx.x * kCocoAnnCols;
+    const int kind = (int)A[0], np_ = (int)A[4];
+    const uint32_t h = (uint32_t)A[1], w = (uint32_t)A[2];
+    const int64_t p0 = A[3], off = A[5];
+    uint32_t* out = out_cnts + off;
+    uint32_t* tmp = tmp_cnts + off;
+    __shared__ int64_t s_m;
+    if (kind == kCocoPoly) {
+        for (int p = 0; p < np_; p++) {
+            const int64_t* P = parts + (p0 + p) * kCocoPartCols;
+            uint32_t* r; int64_t rm;
+            coco_poly_rle(xy + 2 * P[0], (int)P[1], h, w, ws + P[2], P[3], &r, &rm);
+            if (threadIdx.x == 0) {
+                if (p == 0) { for (int64_t j = 0; j < rm; j++) out[j] = r[j]; s_m = rm; }
+                else {
+                    const int64_t mm = coco_rle_union(out, s_m, r, rm, tmp);
+                    for (int64_t j = 0; j < mm; j++) out[j] = tmp[j];
+                    s_m = mm;
+                }
+            }
+            __syncthreads();
+        }
+    } else if (threadIdx.x == 0) {
+        const int64_t* P = parts + p0 * kCocoPartCols;
+        if (kind == kCocoCounts) {
+            for (int64_t j = 0; j < P[1]; j++) out[j] = ucounts[P[0] + j];
+            s_m = P[1];
+        } else {
+            s_m = coco_rle_from_string(chars + P[0], P[1], out);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        out_len[blockIdx.x] = s_m;
+        coco_rle_box(out, s_m, h, w, out_box + 4 * (int64_t)blockIdx.x);
+    }
+}
+
+// one thread per detection: decoded counts at the detection's char offset (a count takes at least one char)
+__global__ void coco_det_rle_kernel(int64_t n, const int64_t* __restrict__ det_i, const char* __restrict__ chars, uint32_t* __restrict__ cnts,
+                                    int64_t* __restrict__ det_m, double* __restrict__ det_area, double* __restrict__ det_box) {
+    const int64_t d = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n) return;
+    const int64_t* I = det_i + d * kCocoDetI;
+    uint32_t* c = cnts + I[0];
+    const int64_t m = coco_rle_from_string(chars + I[0], I[1], c);
+    uint32_t area = 0;
+    for (int64_t j = 1; j < m; j += 2) area += c[j];
+    det_m[d] = m;
+    det_area[d] = (double)area;
+    coco_rle_box(c, m, (uint32_t)I[2], (uint32_t)I[3], det_box + 4 * d);
+}
+
+struct CocoEvalArgs {
+    int segm, num_images;
+    const int64_t* pairs;
+    const double* det_f; const int64_t* det_i;
+    const uint32_t* det_cnts; const int64_t* det_m; const double* det_area; const double* det_rbox;
+    const double* gt_f; const int64_t* gt_i; const uint32_t* gt_cnts;
+    const double* par;
+    int* kept_det;            // [kept] detection index of each kept slot
+    int* kept_rank;           // [kept] rank within its pair
+    double* kept_score;       // [kept]
+    uint8_t* state;           // [kept][40] bit 0 matched (to a gt of non-zero id), bit 1 ignored
+    double* iou;              // [sum D' G]
+    uint8_t* gtm;             // [gts][40]
+};
+
+__device__ __forceinline__ bool coco_out(double area, const double* rng) { return area < rng[0] || area > rng[1]; }
+
+// one CTA per (category, image) pair that has detections
+__global__ void coco_pair_kernel(CocoEvalArgs p) {
+    const int64_t* T = p.pairs + (int64_t)blockIdx.x * kCocoPairCols;
+    const int64_t d0 = T[1], D = T[2], g0 = T[3], G = T[4], k0 = T[5], i0 = T[6];
+    const int64_t Dk = D < kCocoKeep ? D : kCocoKeep;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    // computeIoU: np.argsort(-score, kind='mergesort'), cut to maxDets[-1]
+    for (int64_t i = tid; i < D; i += nt) {
+        const double s = p.det_f[(d0 + i) * kCocoDetF];
+        int64_t r = 0;
+        for (int64_t j = 0; j < D; j++) {
+            const double sj = p.det_f[(d0 + j) * kCocoDetF];
+            r += (sj > s) || (sj == s && j < i);
+        }
+        if (r < kCocoKeep) { p.kept_det[k0 + r] = (int)(d0 + i); p.kept_rank[k0 + r] = (int)r; p.kept_score[k0 + r] = s; }
+    }
+    __syncthreads();
+    for (int64_t e = tid; e < Dk * G; e += nt) {
+        const int64_t dr = e / G, g = e % G, d = p.kept_det[k0 + dr], gi = g0 + g;
+        const bool crowd = p.gt_i[gi * kCocoGtI + 4] != 0;
+        double o;
+        if (p.segm) {
+            const int64_t* DI = p.det_i + d * kCocoDetI;
+            const int64_t* GI = p.gt_i + gi * kCocoGtI;
+            o = coco_rle_iou(p.det_cnts + DI[0], p.det_m[d], p.det_rbox + 4 * d, DI[2], DI[3], p.gt_cnts + GI[0], GI[1], p.gt_f + gi * kCocoGtF + 5,
+                             GI[2], GI[3], crowd);
+        } else {
+            o = coco_bb_iou(p.det_f + d * kCocoDetF + 1, p.gt_f + gi * kCocoGtF, crowd);
+        }
+        p.iou[i0 + dr * G + g] = o;
+    }
+    __syncthreads();
+    // evaluateImg per (area range, threshold): gts ignore-last (stable), greedy matching in score order
+    for (int c = tid; c < kCocoStates; c += nt) {
+        const int ar = c / kCocoThrs, t = c % kCocoThrs;
+        const double* rng = p.par + kCocoParAreas + 2 * ar;
+        uint8_t* gm = p.gtm + g0 * kCocoStates + (int64_t)c * G;
+        for (int64_t g = 0; g < G; g++) gm[g] = 0;
+        for (int64_t dr = 0; dr < Dk; dr++) {
+            double best = p.par[kCocoParThrs + t];
+            int64_t m = -1;
+            bool m_ig = false;
+            for (int pass = 0; pass < 2; pass++) {
+                for (int64_t g = 0; g < G; g++) {
+                    const int64_t* GI = p.gt_i + (g0 + g) * kCocoGtI;
+                    const bool ig = GI[4] != 0 || coco_out(p.gt_f[(g0 + g) * kCocoGtF + 4], rng);
+                    if ((int)ig != pass) continue;
+                    if (gm[g] && !GI[4]) continue;
+                    if (m > -1 && !m_ig && ig) goto matched;
+                    const double o = p.iou[i0 + dr * G + g];
+                    if (o < best) continue;
+                    best = o; m = g; m_ig = ig;
+                }
+            }
+        matched:
+            bool hit = false, dig = false;
+            if (m > -1) {
+                dig = m_ig;
+                hit = p.gt_i[(g0 + m) * kCocoGtI + 5] != 0;
+                gm[m] = 1;
+            }
+            const int64_t d = p.kept_det[k0 + dr];
+            const double area = p.segm ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
+            if (!hit && coco_out(area, rng)) dig = true;
+            p.state[(k0 + dr) * kCocoStates + c] = (uint8_t)((hit ? 1 : 0) | (dig ? 2 : 0));
+        }
+    }
+}
+
+// accumulate(): position of each kept detection in the stable -score sort of its category, per maxDets cut.
+// order_off [3][K + 1]: start of category k's list for cut m; cat_kept [K + 1]: the category's kept slots
+__global__ void coco_rank_kernel(int64_t kept, int K, const int64_t* __restrict__ cat_kept, const int64_t* __restrict__ order_off,
+                                 const int* __restrict__ kept_rank, const double* __restrict__ kept_score, int* __restrict__ order) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= kept) return;
+    int lo = 0, hi = K - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (cat_kept[mid] <= e) lo = mid; else hi = mid - 1; }
+    const int k = lo;
+    const double s = kept_score[e];
+    const int r = kept_rank[e];
+    int64_t pos[kCocoMaxDets] = {0, 0, 0};
+    const int cut[kCocoMaxDets] = {1, 10, 100};
+    for (int64_t j = cat_kept[k]; j < cat_kept[k + 1]; j++) {
+        const double sj = kept_score[j];
+        if ((sj > s) || (sj == s && j < e)) {
+            const int rj = kept_rank[j];
+            pos[0] += rj < cut[0]; pos[1] += rj < cut[1]; pos[2] += rj < cut[2];
+        }
+    }
+    for (int m = 0; m < kCocoMaxDets; m++)
+        if (r < cut[m]) order[order_off[m * (K + 1) + k] + pos[m]] = (int)e;
+}
+
+// one thread per (category, area range, maxDets, threshold).  precision / scores [T, R, K, A, M], recall [T, K, A, M]
+__global__ void coco_accum_kernel(int K, const int64_t* __restrict__ cat_gt, const double* __restrict__ gt_f, const int64_t* __restrict__ gt_i,
+                                  const int64_t* __restrict__ order_off, const int* __restrict__ order, const double* __restrict__ kept_score,
+                                  const uint8_t* __restrict__ state, const double* __restrict__ par, double* __restrict__ precision,
+                                  double* __restrict__ recall, double* __restrict__ scores) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= K * kCocoAreas * kCocoMaxDets * kCocoThrs) return;
+    const int t = idx % kCocoThrs, m = (idx / kCocoThrs) % kCocoMaxDets, a = (idx / (kCocoThrs * kCocoMaxDets)) % kCocoAreas;
+    const int k = idx / (kCocoThrs * kCocoMaxDets * kCocoAreas);
+    const int A = kCocoAreas, M = kCocoMaxDets, R = kCocoRecThrs;
+    const double* rng = par + kCocoParAreas + 2 * a;
+    const double* rec = par + kCocoParRec;
+    const int64_t cell = ((int64_t)k * A + a) * M + m;
+    double* prec = precision + (int64_t)t * R * K * A * M + cell;     // + r * K * A * M
+    double* sco = scores + (int64_t)t * R * K * A * M + cell;
+    const int64_t rstride = (int64_t)K * A * M;
+    int64_t npig = 0;
+    for (int64_t g = cat_gt[k]; g < cat_gt[k + 1]; g++) npig += !(gt_i[g * kCocoGtI + 4] != 0 || coco_out(gt_f[g * kCocoGtF + 4], rng));
+    if (npig == 0) {
+        for (int r = 0; r < R; r++) { prec[r * rstride] = -1; sco[r * rstride] = -1; }
+        recall[(int64_t)t * K * A * M + cell] = -1;
+        return;
+    }
+    const int* list = order + order_off[m * (K + 1) + k];
+    const int64_t nd = order_off[m * (K + 1) + k + 1] - order_off[m * (K + 1) + k];
+    const int sc = a * kCocoThrs + t;
+    int64_t tp = 0, fp = 0;
+    for (int64_t i = 0; i < nd; i++) {
+        const uint8_t st = state[(int64_t)list[i] * kCocoStates + sc];
+        if (!(st & 2)) { if (st & 1) tp++; else fp++; }
+    }
+    const double np_ = (double)npig, eps = 2.220446049250313e-16;   // np.spacing(1)
+    recall[(int64_t)t * K * A * M + cell] = nd ? __ddiv_rn((double)tp, np_) : 0.0;
+    int r = R - 1;
+    const double rc_last = nd ? __ddiv_rn((double)tp, np_) : 0.0;
+    // searchsorted(rc, recThrs, 'left') == nd: precision and score stay 0
+    while (r >= 0 && (nd == 0 || rec[r] > rc_last)) { prec[r * rstride] = 0; sco[r * rstride] = 0; r--; }
+    double env = 0;
+    for (int64_t i = nd - 1; i >= 0; i--) {
+        const double pr = __ddiv_rn((double)tp, __dadd_rn(__dadd_rn((double)fp, (double)tp), eps));
+        env = (i == nd - 1 || !(env > pr)) ? pr : env;     // pr[i-1] = pr[i] if pr[i] > pr[i-1]
+        const uint8_t st = state[(int64_t)list[i] * kCocoStates + sc];
+        if (!(st & 2)) { if (st & 1) tp--; else fp--; }
+        const double rc_prev = __ddiv_rn((double)tp, np_);
+        const double s = kept_score[list[i]];
+        while (r >= 0 && (i == 0 || rec[r] > rc_prev)) { prec[r * rstride] = env; sco[r * rstride] = s; r--; }
+    }
+}
+
+// workspace of dt_coco_eval, 256-byte aligned pieces
+struct CocoEvalWs {
+    size_t det_cnts, det_m, det_area, det_rbox, kept_det, kept_rank, kept_score, state, iou, gtm, order, total;
+};
+inline CocoEvalWs coco_eval_ws(int64_t n_det, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt, int64_t n_order) {
+    CocoEvalWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) / 256 * 256; return at; };
+    w.det_cnts = take(4 * (size_t)n_chars);
+    w.det_m = take(8 * (size_t)n_det);
+    w.det_area = take(8 * (size_t)n_det);
+    w.det_rbox = take(32 * (size_t)n_det);
+    w.kept_det = take(4 * (size_t)kept);
+    w.kept_rank = take(4 * (size_t)kept);
+    w.kept_score = take(8 * (size_t)kept);
+    w.state = take((size_t)kCocoStates * kept);
+    w.iou = take(8 * (size_t)n_iou);
+    w.gtm = take((size_t)kCocoStates * n_gt);
+    w.order = take(4 * (size_t)n_order);
+    w.total = o;
+    return w;
+}
+
+inline cudaError_t coco_gt_launch(int n_ann, const int64_t* ann, const int64_t* parts, const double* xy, const uint32_t* ucounts,
+                                  const char* chars, int* ws, uint32_t* out_cnts, uint32_t* tmp_cnts, int64_t* out_len, double* out_box,
+                                  cudaStream_t st) {
+    coco_gt_kernel<<<n_ann, 128, 0, st>>>(ann, parts, xy, ucounts, chars, ws, out_cnts, tmp_cnts, out_len, out_box);
+    return cudaGetLastError();
+}
+
+inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_active, const int64_t* pairs, const int64_t* cat_gt,
+                                    const int64_t* cat_kept, const int64_t* order_off, int64_t n_det, const double* det_f,
+                                    const int64_t* det_i, const char* det_chars, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt,
+                                    int64_t n_order, const double* gt_f, const int64_t* gt_i, const uint32_t* gt_cnts, const double* par,
+                                    double* precision, double* recall, double* scores, double* ious, void* workspace, cudaStream_t st) {
+    const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order);
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    CocoEvalArgs p;
+    p.segm = segm; p.num_images = num_images; p.pairs = pairs;
+    p.det_f = det_f; p.det_i = det_i;
+    p.det_cnts = reinterpret_cast<uint32_t*>(ws + L.det_cnts); p.det_m = reinterpret_cast<int64_t*>(ws + L.det_m);
+    p.det_area = reinterpret_cast<double*>(ws + L.det_area); p.det_rbox = reinterpret_cast<double*>(ws + L.det_rbox);
+    p.gt_f = gt_f; p.gt_i = gt_i; p.gt_cnts = gt_cnts; p.par = par;
+    p.kept_det = reinterpret_cast<int*>(ws + L.kept_det); p.kept_rank = reinterpret_cast<int*>(ws + L.kept_rank);
+    p.kept_score = reinterpret_cast<double*>(ws + L.kept_score); p.state = ws + L.state;
+    p.iou = ious ? ious : reinterpret_cast<double*>(ws + L.iou); p.gtm = ws + L.gtm;
+    int* order = reinterpret_cast<int*>(ws + L.order);
+    if (segm && n_det > 0) {
+        coco_det_rle_kernel<<<(unsigned)((n_det + 127) / 128), 128, 0, st>>>(n_det, det_i, det_chars, const_cast<uint32_t*>(p.det_cnts), const_cast<int64_t*>(p.det_m), const_cast<double*>(p.det_area), const_cast<double*>(p.det_rbox));
+    }
+    if (n_active > 0) {
+        coco_pair_kernel<<<n_active, 128, 0, st>>>(p);
+    }
+    if (kept > 0) {
+        coco_rank_kernel<<<(unsigned)((kept + 255) / 256), 256, 0, st>>>(kept, K, cat_kept, order_off, p.kept_rank, p.kept_score, order);
+    }
+    const int cells = K * kCocoAreas * kCocoMaxDets * kCocoThrs;
+    if (cells > 0) {
+        coco_accum_kernel<<<(cells + 127) / 128, 128, 0, st>>>(K, cat_gt, gt_f, gt_i, order_off, order, p.kept_score, p.state, par, precision, recall, scores);
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace dt

@@ -1,0 +1,478 @@
+"""COCO box and mask evaluation on the device: pycocotools' COCOeval ('bbox' / 'segm', default Params) without its per-(image,
+category) Python loops.  Precision, recall and scores are bit-identical to COCOeval.evaluate() + accumulate() run on the results
+file that lib/utils/json_dataset_evaluator.py would write; no file is written.
+
+    gt = CocoGroundTruth("instances_minival2014.json")   # or the annotation dict; GT masks are built once, on the device
+    E = evaluate(gt, detector.detect_images(ims), "segm")  # or evaluate(gt, all_boxes, "bbox") / evaluate(gt, all_boxes, "segm", all_segms)
+    E.stats, E.eval["precision"]                          # summarize()'s 12 numbers, [T, R, K, A, M]
+
+The host only checks and flattens the annotations and results into arrays (csrc/coco_eval.cuh documents their layout); everything
+numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before anything is launched."""
+import json
+import math
+
+import numpy as np
+import torch
+
+from .. import _lib
+
+# COCOeval's Params.setDetParams
+IOU_THRS = np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)
+REC_THRS = np.linspace(.0, 1.00, int(np.round((1.00 - .0) / .01)) + 1, endpoint=True)
+MAX_DETS = [1, 10, 100]
+AREA_RNG = [[0 ** 2, 1e5 ** 2], [0 ** 2, 32 ** 2], [32 ** 2, 96 ** 2], [96 ** 2, 1e5 ** 2]]
+AREA_LBL = ['all', 'small', 'medium', 'large']
+KIND_POLY, KIND_COUNTS, KIND_STRING = 0, 1, 2
+_GT_BUDGET_INTS = 1 << 26        # GT masks are built in chunks of at most this much int32 workspace + output
+_COORD_MAX = 1e8                 # polygon coordinates: x5 upsampled to int32 by maskApi
+
+
+def _params():
+    p = np.zeros(119, np.float64)
+    p[0:8] = np.array(AREA_RNG, np.float64).reshape(-1)
+    p[8:18] = [min([t, 1 - 1e-10]) for t in IOU_THRS]
+    p[18:] = REC_THRS
+    return p
+
+
+def _p(t):
+    return None if t is None else t.data_ptr()
+
+
+def _stream(dev):
+    return torch.cuda.current_stream(dev).cuda_stream
+
+
+def _int(v, what):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+        raise ValueError("%s must be an integer, got %r" % (what, v))
+    return int(v)
+
+
+def _num(v, what):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not math.isfinite(float(v)):
+        raise ValueError("%s must be a finite number, got %r" % (what, v))
+    return float(v)
+
+
+def _size(seg, what):
+    sz = seg.get('size')
+    if not isinstance(sz, (list, tuple)) or len(sz) != 2:
+        raise ValueError("%s: RLE 'size' must be [h, w]" % what)
+    h, w = _int(sz[0], what + " size"), _int(sz[1], what + " size")
+    if h < 1 or w < 1 or h * w >= 2 ** 32:
+        raise ValueError("%s: RLE size %dx%d outside [1, 2^32) pixels" % (what, h, w))
+    return h, w
+
+
+def _check_strings(buf, lens, what):
+    """maskApi rleFrString reads 6-bit chars 48..111, a value ends on a char without bit 0x20; values are kept to <= 6 chars (< 2^30)."""
+    if len(buf) == 0:
+        return
+    b = np.frombuffer(buf, np.uint8).astype(np.int32)
+    if b.min() < 48 or b.max() > 111:
+        raise ValueError("%s: RLE string with a character outside '0'..'o'" % what)
+    cont = ((b - 48) & 0x20) != 0
+    ends = np.cumsum(lens)[lens > 0] - 1
+    if np.any(cont[ends]):
+        raise ValueError("%s: RLE string ends inside a value" % what)
+    stops = np.flatnonzero(~cont)
+    if np.max(np.diff(np.concatenate([[-1], stops])) - 1) > 5:
+        raise ValueError("%s: RLE string with a value longer than 6 characters" % what)
+
+
+def _as_bytes(c, what):
+    if isinstance(c, str):
+        try:
+            return c.encode('ascii')
+        except UnicodeEncodeError:
+            raise ValueError("%s: RLE string is not ASCII" % what) from None
+    if isinstance(c, (bytes, bytearray)):
+        return bytes(c)
+    raise ValueError("%s: RLE 'counts' must be a string, bytes or a list of integers" % what)
+
+
+def _upsampled_points(xy):
+    """maskApi rleFrPoly's m: points of the x5 upsampled boundary ((int)(5 x + .5), then max(|dx|, |dy|) + 1 per edge)."""
+    q = np.trunc(5.0 * xy + 0.5).astype(np.int64).reshape(-1, 2)
+    d = np.abs(q - np.roll(q, -1, axis=0))
+    return int(np.sum(np.maximum(d[:, 0], d[:, 1]) + 1))
+
+
+class CocoGroundTruth:
+    """The ground truth of a COCO annotation set (dict or json path) on the device, reusable across evaluations.  Images, categories
+    and annotations are taken as pycocotools' COCO indexes them; annotations of unknown images or categories are left out, as
+    COCOeval's getAnnIds does.  Polygon / uncompressed RLE / RLE masks are converted to RLE on the device (COCO.annToRLE)."""
+
+    def __init__(self, annotations, device=None):
+        if isinstance(annotations, str):
+            with open(annotations) as f:
+                annotations = json.load(f)
+        if not isinstance(annotations, dict):
+            raise ValueError("annotations must be a COCO annotation dict or the path of one")
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        ds = annotations
+        imgs, cats, anns = ds.get('images', []), ds.get('categories', []), ds.get('annotations', [])
+        self.image_hw = {}
+        for im in imgs:
+            i = _int(im.get('id'), "image id")
+            if i in self.image_hw:
+                raise ValueError("duplicate image id %d" % i)
+            h, w = _int(im.get('height'), "image %d height" % i), _int(im.get('width'), "image %d width" % i)
+            if h < 1 or w < 1 or h * w >= 2 ** 32:
+                raise ValueError("image %d: size %dx%d outside [1, 2^32) pixels" % (i, h, w))
+            self.image_hw[i] = (h, w)
+        self.category_ids = [_int(c.get('id'), "category id") for c in cats]       # dataset order: JsonDataset's contiguous classes
+        if len(set(self.category_ids)) != len(self.category_ids):
+            raise ValueError("duplicate category id")
+        self.img_ids = sorted(self.image_hw)                                          # COCOeval params.imgIds / catIds
+        self.cat_ids = sorted(self.category_ids)
+        I, K = len(self.img_ids), len(self.cat_ids)
+        img_index = {v: n for n, v in enumerate(self.img_ids)}
+        cat_index = {v: n for n, v in enumerate(self.cat_ids)}
+        seen, kept = set(), []
+        for a in anns:
+            aid = _int(a.get('id'), "annotation id")
+            if aid in seen:
+                raise ValueError("duplicate annotation id %d" % aid)
+            seen.add(aid)
+            i, k = img_index.get(a.get('image_id')), cat_index.get(a.get('category_id'))
+            if i is not None and k is not None:
+                kept.append((k * I + i, a))
+        order = sorted(range(len(kept)), key=lambda n: kept[n][0])                  # stable: annotation order within a pair
+        G = len(kept)
+        self.num_images, self.num_cats, self.num_gts = I, K, G
+        gt_f = np.zeros((G, 9), np.float64)
+        gt_i = np.zeros((G, 6), np.int64)
+        keys = np.zeros(G, np.int64)
+        segs = []
+        for n, o in enumerate(order):
+            key, a = kept[o]
+            what = "annotation %r" % a['id']
+            keys[n] = key
+            bb = a.get('bbox')
+            if not isinstance(bb, (list, tuple)) or len(bb) != 4:
+                raise ValueError("%s: bbox must be [x, y, w, h]" % what)
+            gt_f[n, :4] = [_num(v, what + " bbox") for v in bb]
+            gt_f[n, 4] = _num(a.get('area'), what + " area")
+            crowd = a.get('iscrowd')
+            if crowd not in (0, 1) or isinstance(crowd, float):
+                raise ValueError("%s: iscrowd must be 0 or 1, got %r" % (what, crowd))
+            h, w = self.image_hw[self.img_ids[key % I]]
+            gt_i[n, 2:6] = [h, w, int(crowd), int(a['id'] != 0)]
+            segs.append((a.get('segmentation'), h, w, what))
+        self.keys = keys
+        self.ann_ids = [kept[o][1]['id'] for o in order]                             # annotation ids in pair order
+        self.cat_gt = np.searchsorted(keys // max(I, 1), np.arange(K + 1)).astype(np.int64) if I else np.zeros(K + 1, np.int64)
+        self.has_masks = all(s[0] is not None for s in segs)
+        self._gt_f, self._gt_i = gt_f, gt_i
+        self.gt_counts = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        if self.has_masks and G:
+            self._build_masks(segs)
+        self.gt_f = torch.from_numpy(self._gt_f).to(self.device)
+        self.gt_i = torch.from_numpy(self._gt_i).to(self.device)
+
+    def _build_masks(self, segs):
+        """Flatten every mask into the annotation / part tables, check it, then convert on the device in bounded chunks."""
+        G = len(segs)
+        ann = np.zeros((G, 6), np.int64)
+        parts, xy, ucounts, chars = [], [], [], []
+        nxy = ncnt = nch = 0
+        ws_ints, out_cap = np.zeros(G, np.int64), np.zeros(G, np.int64)
+        for n, (seg, h, w, what) in enumerate(segs):
+            if isinstance(seg, list):
+                if len(seg) == 0 or not all(isinstance(p, (list, tuple)) for p in seg):
+                    raise ValueError("%s: polygon segmentation must be a non-empty list of coordinate lists" % what)
+                # maskUtils.frPyObjects takes a first entry of 4 numbers for a box list and fails on it (frBbox wants an array)
+                polys = []
+                for p in seg:
+                    if len(p) < 6 or len(p) % 2:
+                        raise ValueError("%s: a polygon needs an even number (>= 6) of coordinates" % what)
+                    polys.append(np.array([_num(v, what + " polygon") for v in p], np.float64))
+                ann[n, :5] = [KIND_POLY, h, w, len(parts), len(polys)]
+                for q in polys:
+                    if np.abs(q).max() > _COORD_MAX:
+                        raise ValueError("%s: polygon coordinate beyond %g" % (what, _COORD_MAX))
+                    k, m = len(q) // 2, _upsampled_points(q)
+                    if m >= 2 ** 31 // 4:
+                        raise ValueError("%s: polygon too long" % what)
+                    parts.append([nxy, k, int(ws_ints[n]), m])
+                    ws_ints[n] += k + 4 * m + 3
+                    out_cap[n] += m + 2
+                    xy.append(q); nxy += k
+                out_cap[n] += len(polys)
+            elif isinstance(seg, dict) and 'counts' in seg and 'size' in seg:
+                rh, rw = _size(seg, what)
+                c = seg['counts']
+                if isinstance(c, list):
+                    v = np.array([_int(x, what + " counts") for x in c], np.int64)
+                    if v.size and (v.min() < 0 or v.max() >= 2 ** 32):
+                        raise ValueError("%s: RLE count outside [0, 2^32)" % what)
+                    ann[n, :5] = [KIND_COUNTS, rh, rw, len(parts), 1]
+                    parts.append([ncnt, len(v), 0, 0]); ucounts.append(v.astype(np.uint32)); ncnt += len(v)
+                    out_cap[n] = max(len(v), 1)
+                else:
+                    s = _as_bytes(c, what)
+                    _check_strings(s, np.array([len(s)]), what)
+                    ann[n, :5] = [KIND_STRING, rh, rw, len(parts), 1]
+                    parts.append([nch, len(s), 0, 0]); chars.append(s); nch += len(s)
+                    out_cap[n] = max(len(s), 1)
+                self._gt_i[n, 2:4] = [rh, rw]
+            else:
+                raise ValueError("%s: segmentation must be polygons or an RLE dict with 'size' and 'counts'" % what)
+        parts = np.array(parts, np.int64).reshape(-1, 4)
+        dev = self.device
+        L = _lib.lib()
+        xy_d = torch.from_numpy(np.concatenate(xy) if xy else np.zeros(2)).to(dev)
+        uc_d = torch.from_numpy((np.concatenate(ucounts) if ucounts else np.zeros(1, np.uint32)).view(np.int32)).to(dev)
+        ch_d = torch.from_numpy(np.frombuffer(b"".join(chars) or b"\0", np.uint8).copy()).to(dev)
+        # chunks of annotations whose workspace + 2 output buffers fit the budget (a single larger annotation gets a chunk of its own)
+        cost = ws_ints + 2 * out_cap
+        lens, outs = np.zeros(G, np.int64), []
+        n0 = 0
+        while n0 < G:
+            n1 = n0 + 1
+            tot = cost[n0]
+            while n1 < G and tot + cost[n1] <= _GT_BUDGET_INTS:
+                tot += cost[n1]; n1 += 1
+            a = ann[n0:n1].copy()
+            a[:, 5] = np.concatenate([[0], np.cumsum(out_cap[n0:n1])[:-1]])
+            p0, p1 = a[0, 3], (a[-1, 3] + a[-1, 4])
+            pt = parts[p0:p1].copy()
+            a[:, 3] -= p0
+            poly = a[:, 0] == KIND_POLY
+            # workspace offsets of the chunk's polygon parts: per annotation, after the previous annotations'
+            wbase = np.concatenate([[0], np.cumsum(ws_ints[n0:n1])[:-1]])
+            for r in np.flatnonzero(poly):
+                pt[a[r, 3]:a[r, 3] + a[r, 4], 2] += wbase[r]
+            ncap = int(out_cap[n0:n1].sum())
+            ws = torch.empty((max(int(ws_ints[n0:n1].sum()), 1),), dtype=torch.int32, device=dev)
+            out = torch.empty((ncap,), dtype=torch.int32, device=dev)
+            tmp = torch.empty((ncap,), dtype=torch.int32, device=dev)
+            olen = torch.empty((n1 - n0,), dtype=torch.int64, device=dev)
+            obox = torch.empty((n1 - n0, 4), dtype=torch.float64, device=dev)
+            a_d, p_d = torch.from_numpy(a).to(dev), torch.from_numpy(pt).to(dev)
+            _lib.check(L.dt_coco_gt_build(n1 - n0, _p(a_d), _p(p_d), _p(xy_d), _p(uc_d), _p(ch_d), _p(ws), _p(out), _p(tmp), _p(olen), _p(obox),
+                                          _stream(dev)), "dt_coco_gt_build")
+            ln = olen.cpu().numpy()
+            lens[n0:n1] = ln
+            self._gt_f[n0:n1, 5:9] = obox.cpu().numpy()
+            starts = torch.from_numpy(a[:, 5]).to(dev)
+            ln_d = torch.from_numpy(ln).to(dev)
+            idx = torch.repeat_interleave(starts, ln_d) + (torch.arange(int(ln.sum()), device=dev) -
+                                                           torch.repeat_interleave(torch.cumsum(ln_d, 0) - ln_d, ln_d))
+            outs.append(out[idx])
+            n0 = n1
+        self._gt_i[:, 0] = np.concatenate([[0], np.cumsum(lens)[:-1]])
+        self._gt_i[:, 1] = lens
+        self.gt_counts = torch.cat(outs) if int(lens.sum()) else torch.zeros((1,), dtype=torch.int32, device=dev)
+
+    def rles(self):
+        """The GT masks as pycocotools would hold them after COCO.annToRLE, in pair order: uint32 run lengths per annotation."""
+        c = self.gt_counts.cpu().numpy().view(np.uint32)
+        return [c[o:o + n].copy() for o, n in self._gt_i[:, :2]]
+
+
+class Params:
+    """The parts of COCOeval's Params that evaluation results refer to."""
+
+    def __init__(self, gt, iou_type):
+        self.imgIds, self.catIds = list(gt.img_ids), list(gt.cat_ids)
+        self.iouThrs, self.recThrs = IOU_THRS.copy(), REC_THRS.copy()
+        self.maxDets, self.areaRng, self.areaRngLbl = list(MAX_DETS), [list(a) for a in AREA_RNG], list(AREA_LBL)
+        self.useCats, self.iouType = 1, iou_type
+
+
+class CocoEvalResult:
+    """What a COCOeval object holds after evaluate() + accumulate() (+ summarize() for .stats): .params, .eval, .stats."""
+
+    def __init__(self, params, precision, recall, scores):
+        self.params = params
+        T, R, K, A, M = precision.shape
+        self.eval = {'params': params, 'counts': [T, R, K, A, M], 'precision': precision, 'recall': recall, 'scores': scores}
+        self.stats = self._stats(verbose=False)
+
+    def summarize(self):
+        self.stats = self._stats(verbose=True)
+
+    def _stats(self, verbose):
+        p = self.params
+
+        def one(ap=1, iouThr=None, areaRng='all', maxDets=100):
+            aind = [i for i, aRng in enumerate(p.areaRngLbl) if aRng == areaRng]
+            mind = [i for i, mDet in enumerate(p.maxDets) if mDet == maxDets]
+            s = self.eval['precision'] if ap == 1 else self.eval['recall']
+            if iouThr is not None:
+                s = s[np.where(iouThr == p.iouThrs)[0]]
+            s = s[:, :, :, aind, mind] if ap == 1 else s[:, :, aind, mind]
+            mean_s = -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+            if verbose:
+                iouStr = '{:0.2f}:{:0.2f}'.format(p.iouThrs[0], p.iouThrs[-1]) if iouThr is None else '{:0.2f}'.format(iouThr)
+                print(' {:<18} {} @[ IoU={:<9} | area={:>6s} | maxDets={:>3d} ] = {:0.3f}'.format(
+                    'Average Precision' if ap == 1 else 'Average Recall', '(AP)' if ap == 1 else '(AR)', iouStr, areaRng, maxDets, mean_s))
+            return mean_s
+        m = p.maxDets
+        stats = np.zeros((12,))
+        stats[0] = one(1)
+        stats[1] = one(1, iouThr=.5, maxDets=m[2])
+        stats[2] = one(1, iouThr=.75, maxDets=m[2])
+        stats[3] = one(1, areaRng='small', maxDets=m[2])
+        stats[4] = one(1, areaRng='medium', maxDets=m[2])
+        stats[5] = one(1, areaRng='large', maxDets=m[2])
+        stats[6] = one(0, maxDets=m[0])
+        stats[7] = one(0, maxDets=m[1])
+        stats[8] = one(0, maxDets=m[2])
+        stats[9] = one(0, areaRng='small', maxDets=m[2])
+        stats[10] = one(0, areaRng='medium', maxDets=m[2])
+        stats[11] = one(0, areaRng='large', maxDets=m[2])
+        return stats
+
+
+def _per_class(gt, results, all_segms, iou_type):
+    """results -> (all_boxes, all_segms) indexed [contiguous class][image]: detect_images / batch_results' per-image tuples are filed
+    the way extend_results files them."""
+    if isinstance(results, (list, tuple)) and len(results) and isinstance(results[0], tuple):
+        if all_segms is not None:
+            raise ValueError("per-image results carry their masks; all_segms is for all_boxes input")
+        if len(results) != gt.num_images:
+            raise ValueError("%d per-image results for %d images" % (len(results), gt.num_images))
+        if any(len(r) != 4 for r in results):
+            raise ValueError("per-image results are (scores, boxes, boxes_per_class, segms_per_class) tuples")
+        nc = max(len(r[2]) for r in results)
+        boxes = [[[] for _ in results] for _ in range(nc)]
+        segms = [[[] for _ in results] for _ in range(nc)]
+        for i, r in enumerate(results):
+            for j in range(1, len(r[2])):
+                boxes[j][i] = r[2][j]
+                if r[3] is not None:
+                    segms[j][i] = r[3][j]
+                elif iou_type == 'segm':
+                    raise ValueError("segm evaluation of results without masks")
+        return boxes, segms
+    if iou_type == 'segm' and all_segms is None:
+        raise ValueError("segm evaluation of all_boxes needs all_segms")
+    return results, all_segms
+
+
+def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids):
+    """_write_coco_{bbox,segms}_results_file + COCO.loadRes, as arrays: one row per result in the file's order (class-major, images in
+    sorted-id order), bbox = xyxy_to_xywh of the float64 boxes (+1 width), score = the float64 of the stored value."""
+    I = gt.num_images
+    cat_index = {v: n for n, v in enumerate(gt.cat_ids)}
+    segm = iou_type == 'segm'
+    keys, dets, strs, hw = [], [], [], []
+    for j in range(1, len(category_ids) + 1):
+        if j >= len(all_boxes):
+            break
+        k = cat_index[category_ids[j - 1]]
+        per_img = all_boxes[j]
+        if len(per_img) != I:
+            raise ValueError("class %d: %d entries for %d images" % (j, len(per_img), I))
+        if segm and (j >= len(all_segms) or len(all_segms[j]) != I):
+            raise ValueError("class %d: all_segms does not have one entry per image" % j)
+        for i in range(I):
+            d = per_img[i]
+            if isinstance(d, list) and len(d) == 0:
+                continue
+            d = np.asarray(d)
+            if d.ndim != 2 or d.shape[1] != 5:
+                raise ValueError("class %d image %d: detections must be an N x 5 array" % (j, i))
+            n = d.shape[0]
+            keys.append((k * I + i, n))
+            dets.append(d)
+            if segm:
+                rles = all_segms[j][i]
+                if len(rles) < n:
+                    raise ValueError("class %d image %d: %d masks for %d detections" % (j, i, len(rles), n))
+                for r in rles[:n]:
+                    if not isinstance(r, dict) or 'counts' not in r or 'size' not in r:
+                        raise ValueError("class %d image %d: RLE dicts with 'size' and 'counts' expected" % (j, i))
+                    sz, c = r['size'], r['counts']
+                    hw.append(sz)
+                    strs.append(c.encode() if isinstance(c, str) else _as_bytes(c, "class %d image %d mask" % (j, i)))
+    # the float64 view of each stored value, then xyxy_to_xywh (+1) -- elementwise, so done once over the concatenation
+    d = np.concatenate([x.astype(np.float64) for x in dets]) if dets else np.zeros((0, 5))
+    if not np.all(np.isfinite(d)):
+        raise ValueError("non-finite box or score in the results")
+    N = len(d)
+    key = np.repeat(np.array([a for a, _ in keys], np.int64), [n for _, n in keys]) if keys else np.zeros(0, np.int64)
+    det_f = np.zeros((N, 5), np.float64)
+    det_i = np.zeros((N, 4), np.int64)
+    det_f[:, 0] = d[:, -1]
+    det_f[:, 1:5] = np.hstack((d[:, 0:2], d[:, 2:4] - d[:, 0:2] + 1))
+    chars = b""
+    if segm and N:
+        sizes = np.array(hw, dtype=object)
+        if sizes.ndim != 2 or sizes.shape[1] != 2 or not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in sizes.flat):
+            raise ValueError("results: RLE 'size' must be [h, w] integers")
+        sizes = sizes.astype(np.int64)
+        if np.any(sizes < 1) or np.any(sizes[:, 0] * sizes[:, 1] >= 2 ** 32):
+            raise ValueError("results: RLE size outside [1, 2^32) pixels")
+        lens = np.fromiter((len(s) for s in strs), np.int64, N)
+        try:
+            chars = b"".join(strs)
+        except TypeError:
+            raise ValueError("results: RLE 'counts' must be strings") from None
+        _check_strings(chars, lens, "results")
+        det_i[:, 0] = np.concatenate([[0], np.cumsum(lens)[:-1]])
+        det_i[:, 1] = lens
+        det_i[:, 2:4] = sizes
+    order = np.argsort(key, kind='stable')
+    return key[order], det_f[order], det_i[order], chars
+
+
+def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False):
+    """COCOeval(gt, loadRes(results file), iou_type).evaluate() + accumulate() on the device -> CocoEvalResult.
+    results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), or the notebooks' all_boxes
+    [class][image] (with all_segms [class][image] for 'segm').  category_ids: json id of contiguous class j (1-based) at j - 1;
+    default: the dataset's category order, as JsonDataset builds its classes.  keep_ious: also return COCOeval's .ious, {(image id,
+    category id): [min(D, 100), G] array} for the pairs with detections and GTs."""
+    if iou_type not in ('bbox', 'segm'):
+        raise ValueError("iou_type must be 'bbox' or 'segm'")
+    if not isinstance(gt, CocoGroundTruth):
+        raise TypeError("gt must be a CocoGroundTruth")
+    if iou_type == 'segm' and not gt.has_masks:
+        raise ValueError("segm evaluation: some ground-truth annotations have no segmentation")
+    category_ids = list(gt.category_ids if category_ids is None else category_ids)
+    if any(c not in set(gt.cat_ids) for c in category_ids):
+        raise ValueError("category_ids names a category the ground truth does not have")
+    boxes, segms = _per_class(gt, results, all_segms, iou_type)
+    key, det_f, det_i, chars = _flatten_results(gt, boxes, segms, iou_type, category_ids)
+    I, K, N = gt.num_images, gt.num_cats, len(key)
+    # (category, image) pairs with detections
+    pk, pstart, pcount = np.unique(key, return_index=True, return_counts=True)
+    g0 = np.searchsorted(gt.keys, pk, 'left')
+    gn = np.searchsorted(gt.keys, pk, 'right') - g0
+    kept = np.minimum(pcount, MAX_DETS[-1])
+    pairs = np.zeros((len(pk), 7), np.int64)
+    pairs[:, 0], pairs[:, 1], pairs[:, 2], pairs[:, 3], pairs[:, 4] = pk, pstart, pcount, g0, gn
+    pairs[:, 5] = np.concatenate([[0], np.cumsum(kept)[:-1]])
+    pairs[:, 6] = np.concatenate([[0], np.cumsum(kept * gn)[:-1]])
+    pcat = pk // max(I, 1)
+    cat_kept = np.concatenate([[0], np.cumsum(np.bincount(pcat, weights=kept, minlength=K)[:K].astype(np.int64))])
+    order_off = np.zeros((3, K + 1), np.int64)
+    base = 0
+    for m, cut in enumerate(MAX_DETS):
+        c = np.bincount(pcat, weights=np.minimum(pcount, cut), minlength=K)[:K].astype(np.int64)
+        order_off[m] = base + np.concatenate([[0], np.cumsum(c)])
+        base = order_off[m, -1]
+    n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(base)
+    dev = gt.device
+    T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
+    prec = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
+    rec = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
+    scr = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
+    L = _lib.lib()
+    up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, gt.cat_gt, cat_kept, order_off, det_f, det_i, _params())]
+    ch = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
+    ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious else None
+    ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, len(chars), n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
+    _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, len(pk), _p(up[0]), _p(up[1]), _p(up[2]), _p(up[3]), N, _p(up[4]),
+                              _p(up[5]), _p(ch), len(chars), n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f), _p(gt.gt_i), _p(gt.gt_counts),
+                              _p(up[6]), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
+    E = CocoEvalResult(Params(gt, iou_type), prec.cpu().numpy(), rec.cpu().numpy(), scr.cpu().numpy())
+    if keep_ious:
+        iv = ious.cpu().numpy()
+        E.ious = {(gt.img_ids[k % I], gt.cat_ids[k // I]): iv[o:o + d * g].reshape(d, g)
+                  for k, d, g, o in zip(pk, kept, gn, pairs[:, 6]) if g > 0}
+    return E

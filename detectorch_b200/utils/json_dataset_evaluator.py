@@ -1,0 +1,55 @@
+"""evaluate_boxes / evaluate_masks of the reference's lib/utils/json_dataset_evaluator.py (:40-64, :128-146) on the device: the same
+signatures and the same COCOeval numbers (coco_eval.evaluate), without writing, reloading or keeping a results file.  A notebook
+switches with one import line:
+    from detectorch_b200.utils.json_dataset_evaluator import evaluate_boxes, evaluate_masks
+json_dataset.COCO.dataset supplies the ground truth (built on the device once per json_dataset, kept on it); its classes /
+category_to_id_map give the json category id of each contiguous class, as _write_coco_*_results_file uses them."""
+import logging
+
+import numpy as np
+
+from . import coco_eval
+
+logger = logging.getLogger(__name__)
+
+
+def _ground_truth(json_dataset):
+    gt = getattr(json_dataset, "_device_coco_gt", None)
+    if gt is None:
+        gt = coco_eval.CocoGroundTruth(json_dataset.COCO.dataset)
+        json_dataset._device_coco_gt = gt
+    return gt
+
+
+def _category_ids(json_dataset):
+    return [json_dataset.category_to_id_map[c] for c in json_dataset.classes if c != '__background__']
+
+
+def _evaluate(json_dataset, all_boxes, all_segms, iou_type):
+    # Only do evaluation on non-test sets (annotations are undisclosed on test), as the reference
+    if json_dataset.name.find('test') != -1:
+        return None
+    E = coco_eval.evaluate(_ground_truth(json_dataset), all_boxes, iou_type, all_segms, category_ids=_category_ids(json_dataset))
+    _log_detection_eval_metrics(E)
+    return E
+
+
+def evaluate_masks(json_dataset, all_boxes, all_segms, output_dir, use_salt=True, cleanup=False):
+    """-> the evaluation ('segm'): .eval['precision' | 'recall' | 'scores'], .stats, .params.  output_dir / use_salt / cleanup are
+    accepted for the reference's signature; nothing is written."""
+    return _evaluate(json_dataset, all_boxes, all_segms, 'segm')
+
+
+def evaluate_boxes(json_dataset, all_boxes, output_dir, use_salt=True, cleanup=False):
+    """-> the evaluation ('bbox'), as evaluate_masks."""
+    return _evaluate(json_dataset, all_boxes, None, 'bbox')
+
+
+def _log_detection_eval_metrics(E):
+    ind_lo = np.where(np.isclose(E.params.iouThrs, 0.5))[0][0]
+    ind_hi = np.where(np.isclose(E.params.iouThrs, 0.95))[0][0]
+    precision = E.eval['precision'][ind_lo:(ind_hi + 1), :, :, 0, 2]
+    ap = np.mean(precision[precision > -1]) if np.any(precision > -1) else -1
+    logger.info('~~~~ Mean and per-category AP @ IoU=[0.50,0.95] ~~~~')
+    logger.info('{:.1f}'.format(100 * ap))
+    E.summarize()

@@ -259,6 +259,36 @@ int dt_engine_count_launches(dt_engine_t e, int first_stage, int last_stage);
 int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_factor, int first_stage, int last_stage, dt_stream_t stream,
                       float* ms_out, double* flops_out, int* stage_out, int* block_n_out, int cap);
 
+/* ---------------------------------------------------------------------------------------------
+ * COCO box / mask evaluation (pycocotools COCOeval, iouType 'bbox' or 'segm', default Params), bit for bit.
+ * Table layouts are the constants at the top of detectorch_b200/csrc/coco_eval.cuh.
+ * dt_coco_gt_build: ground-truth masks -> RLE, one CTA per annotation.
+ *   anns [num_anns, 6] int64      kind (0 polygon parts, 1 uncompressed counts, 2 compressed string), h, w, first part, parts, output offset
+ *   parts [.., 4] int64           first element of xy (point pairs) / ucounts / chars, its element count, int32 workspace offset, and for a
+ *                                 polygon the number of upsampled boundary points (k points, m of them: k + 4 m + 3 ints of workspace)
+ *   out_counts / tmp_counts       uint32 run lengths at each annotation's offset (capacity: up to the next annotation's offset)
+ *   out_len [num_anns] int64, out_box [num_anns, 4] double (rleToBbox)
+ * dt_coco_eval: one evaluation of a detection set against a built ground truth, grouped by (category, image) pair in
+ *   category-major order.  iou_type 0 bbox, 1 segm.
+ *   pairs [num_active, 7]         pair index, first detection, D, first gt, G, first kept slot (min(D, 100) per pair), first IoU (min(D,100) G)
+ *   cat_gt / cat_kept [K+1]       each category's gt range / kept-slot range; order_off [3, K+1] each category's list for maxDets 1, 10, 100
+ *   det_f [num_dets, 5] double    score, x, y, w, h;  det_i [num_dets, 4] int64: char offset, char count, h, w (segm strings in det_chars)
+ *   gt_f [num_gts, 9] double      bbox x y w h, area, RLE box;  gt_i [num_gts, 6] int64: RLE offset, length, h, w, iscrowd, id != 0
+ *   params [119] double           area ranges [4][2], IoU thresholds min(t, 1 - 1e-10) [10], recall thresholds [101]
+ *   precision / scores [10, 101, K, 4, 3], recall [10, K, 4, 3] double
+ *   ious                          optional [num_ious] double: each pair's IoU matrix [min(D, 100), G] (detections in score order, gts in
+ *                                 annotation order) at its first IoU; NULL keeps them in the workspace
+ * Both return 0 on bad sizes or a NULL pointer. */
+int64_t dt_coco_gt_workspace_bytes(int64_t num_parts, int64_t num_points, int64_t num_upsampled);
+int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t* parts, const double* xy, const uint32_t* ucounts, const char* chars,
+                     void* workspace, uint32_t* out_counts, uint32_t* tmp_counts, int64_t* out_len, double* out_box, dt_stream_t stream);
+int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order);
+int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, const int64_t* pairs, const int64_t* cat_gt, const int64_t* cat_kept,
+                 const int64_t* order_off, int64_t num_dets, const double* det_f, const int64_t* det_i, const char* det_chars, int64_t num_chars,
+                 int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order, const double* gt_f, const int64_t* gt_i,
+                 const uint32_t* gt_counts, const double* params, double* precision, double* recall, double* scores, double* ious, void* workspace,
+                 dt_stream_t stream);
+
 /* library / build info */
 const char* dt_version(void);
 
