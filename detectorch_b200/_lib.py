@@ -52,6 +52,7 @@ SIGNATURES = {
     "dt_coco_gt_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
     "dt_coco_gt_build": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
+    "dt_coco_det_check": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_coco_eval_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int64]),
     "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                              c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

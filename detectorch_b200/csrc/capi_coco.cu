@@ -26,6 +26,14 @@ extern "C" int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t
     return 1;
 }
 
+extern "C" int dt_coco_det_check(int64_t num_dets, const int64_t* det_i, const char* det_chars, uint8_t* bad, dt_stream_t stream) {
+    if (num_dets < 0) { fprintf(stderr, "dt_coco_det_check: negative detection count\n"); return 0; }
+    if (num_dets == 0) return 1;
+    if (!det_i || !det_chars || !bad) { fprintf(stderr, "dt_coco_det_check: null argument\n"); return 0; }
+    DT_CHECK_CUDA(coco_det_check_launch(num_dets, det_i, det_chars, bad, (cudaStream_t)stream));
+    return 1;
+}
+
 extern "C" int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts,
                                                 int64_t num_order) {
     if (num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 || num_gts < 0 || num_order < 0) return 0;

@@ -265,6 +265,40 @@ __global__ void coco_det_rle_kernel(int64_t n, const int64_t* __restrict__ det_i
     coco_rle_box(c, m, (uint32_t)I[2], (uint32_t)I[3], det_box + 4 * d);
 }
 
+// one thread per detection string: bad[d] = 1 when rleFrString's uint32 counts of it do not sum to h * w.  rleIou walks two masks'
+// runs until both end, so a mask whose runs cover another number of pixels than its partner's never ends (in maskApi as here); the
+// host refuses such results before dt_coco_eval.  Same decode as coco_rle_from_string, keeping only the last two counts.
+__global__ void coco_det_check_kernel(int64_t n, const int64_t* __restrict__ det_i, const char* __restrict__ chars, uint8_t* __restrict__ bad) {
+    const int64_t d = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n) return;
+    const int64_t* I = det_i + d * kCocoDetI;
+    const char* s = chars + I[0];
+    const int64_t len = I[1];
+    int64_t m = 0, p = 0;
+    uint32_t c2 = 0, c1 = 0;                 // counts m - 2 and m - 1
+    uint64_t tot = 0;
+    while (p < len) {
+        long long x = 0;
+        int k = 0, more = 1;
+        while (more) {
+            const int c = s[p] - 48;
+            x |= (long long)(int)((c & 0x1f) << (5 * k));
+            more = c & 0x20; p++; k++;
+            if (!more && (c & 0x10)) x |= (long long)(int)(0xffffffffu << (5 * k));
+        }
+        if (m > 2) x += (long long)c2;
+        const uint32_t cnt = (uint32_t)x;
+        tot += cnt;
+        c2 = c1; c1 = cnt; m++;
+    }
+    bad[d] = tot != (uint64_t)I[2] * (uint64_t)I[3];
+}
+
+inline cudaError_t coco_det_check_launch(int64_t n, const int64_t* det_i, const char* chars, uint8_t* bad, cudaStream_t st) {
+    coco_det_check_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, det_i, chars, bad);
+    return cudaGetLastError();
+}
+
 struct CocoEvalArgs {
     int segm, num_images;
     const int64_t* pairs;

@@ -7,7 +7,8 @@ file that lib/utils/json_dataset_evaluator.py would write; no file is written.
     E.stats, E.eval["precision"]                          # summarize()'s 12 numbers, [T, R, K, A, M]
 
 The host only checks and flattens the annotations and results into arrays (csrc/coco_eval.cuh documents their layout); everything
-numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before anything is launched."""
+numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before the evaluation is
+launched (segm results' run sums are checked by a small kernel first)."""
 import json
 import math
 
@@ -79,6 +80,77 @@ def _check_strings(buf, lens, what):
     stops = np.flatnonzero(~cont)
     if np.max(np.diff(np.concatenate([[-1], stops])) - 1) > 5:
         raise ValueError("%s: RLE string with a value longer than 6 characters" % what)
+
+
+_SUM_BLOCK_CHARS = 1 << 20      # _string_sums works on blocks of whole strings of about this many chars (bounded temporaries)
+
+
+def _string_sums(buf, lens):
+    """The sum of the run lengths rleFrString decodes from each string (buf already passed _check_strings).  Linear in the chars,
+    per-value temporaries only: chars 48..79 end a value; a value is its 5-bit groups, sign-extended from bit 4 of its last char;
+    count m > 2 is its value plus count m - 2, in uint32."""
+    lens = np.asarray(lens, np.int64)
+    sums = np.zeros(len(lens), np.int64)
+    if len(buf) == 0:
+        return sums
+    b = np.frombuffer(buf, np.uint8)
+    ends = np.cumsum(lens)
+    s0 = 0
+    while s0 < len(lens):
+        c0 = ends[s0] - lens[s0]
+        s1 = max(int(np.searchsorted(ends, c0 + _SUM_BLOCK_CHARS, 'right')), s0 + 1)
+        sums[s0:s1] = _string_sums_block(b[c0:ends[s1 - 1]], lens[s0:s1])
+        s0 = s1
+    return sums
+
+
+def _string_sums_block(b, lens):
+    """One block (< 2^31 chars): 32-bit arithmetic throughout, uint32 sums wrap as the C counts do."""
+    stops = np.flatnonzero(b < 80).astype(np.int32)
+    if len(stops) == 0:
+        return np.zeros(len(lens), np.int64)
+    nv = np.diff(np.searchsorted(stops, np.cumsum(lens)), prepend=0).astype(np.int32)     # values per string
+    # the last char holds the top 5-bit group, sign-extended from its bit 4; the lower groups of the few longer values are added
+    v = b[stops].astype(np.int32) - 48
+    v -= (v & 0x10) << 1
+    nch = np.diff(stops, prepend=np.int32(-1))
+    i = np.flatnonzero(nch > 1)
+    if len(i):
+        n, s = nch[i], stops[i] - nch[i] + 1
+        top = v[i] << (5 * (n - 1))
+        for k in range(5):
+            j = np.flatnonzero(n - 1 > k)
+            top[j] += ((b[s[j] + k].astype(np.int32) - 48) & 0x1f) << (5 * k)
+        v[i] = top
+    u = v.view(np.uint32)
+    vfirst = (np.cumsum(nv) - nv).astype(np.int32)
+    first = np.repeat(vfirst, nv)                                            # each value's string's first value
+    idx = np.arange(len(v), dtype=np.int32)
+    odd, even = ((idx ^ first) & 1) == 1, ((idx ^ first) & 1) == 0
+    even &= idx != first
+    # counts 1, 3, 5.. and 2, 4, 6.. are running sums of their values, restarted at each string; count 0 stands alone
+    p = np.zeros(len(v) + 1, np.uint32)
+    q = np.zeros(len(v) + 1, np.uint32)
+    np.cumsum(np.where(odd, u, np.uint32(0)), dtype=np.uint32, out=p[1:])
+    np.cumsum(np.where(even, u, np.uint32(0)), dtype=np.uint32, out=q[1:])
+    cnt = np.where(odd, p[1:] - p[first], np.where(even, q[1:] - q[first], u))
+    out = np.zeros(len(lens), np.int64)
+    full = nv > 0
+    out[full] = np.add.reduceat(cnt, vfirst[full], dtype=np.int64)
+    return out
+
+
+def _check_sums(sums, h, w, what):
+    """rleIou and rleMerge walk two masks' runs together until both end: runs that do not cover h * w pixels never end."""
+    bad = np.flatnonzero(np.asarray(sums) != np.asarray(h, np.int64) * np.asarray(w, np.int64))
+    if len(bad):
+        raise ValueError("%s: RLE counts do not sum to h * w (mask %d)" % (what, bad[0]))
+
+
+_MASK_PIXELS = 1 << 29           # pycocotools keeps GT masks as strings (polygons and uncompressed counts too): a count or count
+                                 # difference outside [-2^29, 2^29) takes 7 chars, and rleFrString decodes some of those with int
+                                 # shifts that overflow (-1 << 35 for negative ones, a last group of 2 or more << 30).  Masks of fewer
+                                 # pixels never need 7 chars; larger polygon images are refused, larger counts checked one by one.
 
 
 def _as_bytes(c, what):
@@ -189,6 +261,8 @@ class CocoGroundTruth:
                     if len(p) < 6 or len(p) % 2:
                         raise ValueError("%s: a polygon needs an even number (>= 6) of coordinates" % what)
                     polys.append(np.array([_num(v, what + " polygon") for v in p], np.float64))
+                if h * w >= _MASK_PIXELS:
+                    raise ValueError("%s: polygon on an image of %dx%d, 2^29 pixels or more" % (what, h, w))
                 ann[n, :5] = [KIND_POLY, h, w, len(parts), len(polys)]
                 for q in polys:
                     if np.abs(q).max() > _COORD_MAX:
@@ -208,12 +282,18 @@ class CocoGroundTruth:
                     v = np.array([_int(x, what + " counts") for x in c], np.int64)
                     if v.size and (v.min() < 0 or v.max() >= 2 ** 32):
                         raise ValueError("%s: RLE count outside [0, 2^32)" % what)
+                    _check_sums([v.sum()], rh, rw, what)
+                    # frPyObjects stores them as a string: count m > 2 as its difference to count m - 2, in at most 6 chars
+                    d = np.concatenate([v[:3], v[3:] - v[1:-2]])
+                    if d.size and (d.max() >= _MASK_PIXELS or d.min() < -_MASK_PIXELS):
+                        raise ValueError("%s: RLE count difference outside [-2^29, 2^29)" % what)
                     ann[n, :5] = [KIND_COUNTS, rh, rw, len(parts), 1]
                     parts.append([ncnt, len(v), 0, 0]); ucounts.append(v.astype(np.uint32)); ncnt += len(v)
                     out_cap[n] = max(len(v), 1)
                 else:
                     s = _as_bytes(c, what)
                     _check_strings(s, np.array([len(s)]), what)
+                    _check_sums(_string_sums(s, np.array([len(s)])), rh, rw, what)
                     ann[n, :5] = [KIND_STRING, rh, rw, len(parts), 1]
                     parts.append([nch, len(s), 0, 0]); chars.append(s); nch += len(s)
                     out_cap[n] = max(len(s), 1)
@@ -228,6 +308,7 @@ class CocoGroundTruth:
         ch_d = torch.from_numpy(np.frombuffer(b"".join(chars) or b"\0", np.uint8).copy()).to(dev)
         # chunks of annotations whose workspace + 2 output buffers fit the budget (a single larger annotation gets a chunk of its own)
         cost = ws_ints + 2 * out_cap
+        self._mask_cost = cost
         lens, outs = np.zeros(G, np.int64), []
         n0 = 0
         while n0 < G:
@@ -465,6 +546,13 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
     L = _lib.lib()
     up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, gt.cat_gt, cat_kept, order_off, det_f, det_i, _params())]
     ch = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
+    if iou_type == 'segm' and N:
+        # runs that do not cover h * w pixels would make rleIou's merge loop forever: decoded and summed on the device, refused here
+        bad = torch.empty((N,), dtype=torch.uint8, device=dev)
+        _lib.check(L.dt_coco_det_check(N, _p(up[5]), _p(ch), _p(bad), _stream(dev)), "dt_coco_det_check")
+        nb = torch.nonzero(bad).flatten()[:1].cpu().numpy()
+        if len(nb):
+            raise ValueError("results: RLE counts of result %d (in (category, image) order) do not sum to h * w" % nb[0])
     ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious else None
     ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, len(chars), n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
     _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, len(pk), _p(up[0]), _p(up[1]), _p(up[2]), _p(up[3]), N, _p(up[4]),

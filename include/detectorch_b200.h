@@ -278,7 +278,10 @@ int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_fact
  *   precision / scores [10, 101, K, 4, 3], recall [10, K, 4, 3] double
  *   ious                          optional [num_ious] double: each pair's IoU matrix [min(D, 100), G] (detections in score order, gts in
  *                                 annotation order) at its first IoU; NULL keeps them in the workspace
- * Both return 0 on bad sizes or a NULL pointer. */
+ * dt_coco_det_check: bad [num_dets] uint8, 1 where a segm detection's string (det_i / det_chars as for dt_coco_eval) decodes to
+ *   counts that do not sum to h * w.  rleIou never ends on such a mask, so dt_coco_eval must not be given one.
+ * All return 0 on bad sizes or a NULL pointer. */
+int dt_coco_det_check(int64_t num_dets, const int64_t* det_i, const char* det_chars, uint8_t* bad, dt_stream_t stream);
 int64_t dt_coco_gt_workspace_bytes(int64_t num_parts, int64_t num_points, int64_t num_upsampled);
 int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t* parts, const double* xy, const uint32_t* ucounts, const char* chars,
                      void* workspace, uint32_t* out_counts, uint32_t* tmp_counts, int64_t* out_len, double* out_box, dt_stream_t stream);

@@ -70,6 +70,11 @@ def _ds(**ann):
     dict(segmentation=dict(size=[10, 10], counts=[3, -1])), dict(segmentation=dict(size=[10], counts=[3])),
     dict(segmentation=dict(size=[10, 10], counts="0p")), dict(segmentation=dict(size=[10, 10], counts="0\x7f1")),
     dict(segmentation=dict(size=[10, 10], counts="0" + "P" * 6 + "1")), dict(segmentation="x"), dict(id=1.5),
+    # runs that do not cover the mask: rleIou's merge of two such masks never ends
+    dict(segmentation=dict(size=[10, 10], counts=[3, 5])), dict(segmentation=dict(size=[10, 10], counts="35")),
+    dict(segmentation=dict(size=[10, 10], counts=[])), dict(segmentation=dict(size=[10, 10], counts=[90, 20])),
+    # a count difference of 2^29: 7 chars in pycocotools' string form
+    dict(segmentation=dict(size=[30000, 30000], counts=[0, 900000000])),
 ])
 def test_malformed_annotations_raise(bad):
     from detectorch_b200.utils import coco_eval
@@ -81,7 +86,8 @@ def test_malformed_datasets_raise():
     from detectorch_b200.utils import coco_eval
     ds = _ds()
     for bad in (dict(ds, images=ds['images'] * 2), dict(ds, categories=ds['categories'] * 2), dict(ds, annotations=ds['annotations'] * 2),
-                dict(ds, images=[dict(id=1, height=0, width=10)])):
+                dict(ds, images=[dict(id=1, height=0, width=10)]),
+                dict(ds, images=[dict(id=1, height=23171, width=23171)])):      # a polygon on 2^29 pixels: its RLE may need 7-char values
         with pytest.raises(ValueError):
             coco_eval.CocoGroundTruth(bad, device='cpu')
     with pytest.raises(ValueError):
