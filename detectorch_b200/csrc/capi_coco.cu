@@ -1,9 +1,11 @@
-// detectorch_b200 -- C-ABI entry points of the COCO evaluation (coco_eval.cuh; include/detectorch_b200.h).
+// detectorch_b200 -- C-ABI entry points of the COCO evaluation (coco_eval.cuh) and of the proposal recall (proposal_recall.cuh);
+// include/detectorch_b200.h.
 #include <stdio.h>
 
 #include "../../include/detectorch_b200.h"
 #include "coco_eval.cuh"
 #include "common.cuh"
+#include "proposal_recall.cuh"
 
 using namespace dt;
 
@@ -60,5 +62,39 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
     DT_CHECK_CUDA(coco_eval_launch(iou_type, num_images, num_cats, num_active, pairs, cat_gt, cat_kept, order_off, num_dets, det_f, det_i,
                                    det_chars, num_chars, kept, num_ious, num_gts, num_order, gt_f, gt_i, gt_counts, params, precision, recall,
                                    scores, ious, workspace, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int64_t dt_proposal_recall_smem_bytes(int max_gts, int64_t max_props) {
+    if (max_gts < 0 || max_props < 0 || max_gts > (1 << 24) || max_props > (1ll << 36)) return 0;
+    return (int64_t)proposal_recall_smem(max_gts, (int)((max_props + 31) / 32));
+}
+
+extern "C" int dt_proposal_recall(int num_images, int num_combos, const int64_t* prop_off, const float* props, const int64_t* gt_off,
+                                  const float* gts, const double* gt_area, const double* area_rng, const int64_t* limits,
+                                  const int64_t* out_off, int max_gts, int64_t max_props, double* out, int* flag, dt_stream_t stream) {
+    if (num_images < 0 || num_combos < 0 || num_combos > 65535 || max_gts < 0 || max_props < 0 || max_props > (1ll << 36)) {
+        fprintf(stderr, "dt_proposal_recall: bad sizes\n");
+        return 0;
+    }
+    if (num_images == 0 || num_combos == 0) return 1;
+    if (!prop_off || !gt_off || !area_rng || !limits || !out_off || !flag || (max_props > 0 && !props) || (max_gts > 0 && (!gts || !gt_area || !out))) {
+        fprintf(stderr, "dt_proposal_recall: null argument\n");
+        return 0;
+    }
+    const int words = (int)((max_props + 31) / 32);
+    if (proposal_recall_smem(max_gts, words) > 227 * 1024) {
+        fprintf(stderr, "dt_proposal_recall: %d ground-truth boxes and %lld proposals in one image exceed shared memory\n", max_gts,
+                (long long)max_props);
+        return 0;
+    }
+    if (max_gts == 0) return 1;
+    RecallParams P;
+    P.num_images = num_images;
+    P.prop_off = prop_off; P.props = reinterpret_cast<const float4*>(props);
+    P.gt_off = gt_off; P.gts = reinterpret_cast<const float4*>(gts); P.gt_area = gt_area;
+    P.area_rng = area_rng; P.limits = limits; P.out_off = out_off; P.out = out; P.flag = flag;
+    P.max_gts = max_gts; P.row_words = words;
+    DT_CHECK_CUDA(proposal_recall_launch(P, num_combos, (cudaStream_t)stream));
     return 1;
 }

@@ -1177,6 +1177,20 @@ int dt_engine_profile(dt_engine_t h, const float* image_nchw, float scaling_fact
     return (int)sel.size();
 }
 
+// The proposals of the last run (FPN engine with the RPN, run through ST_COLLECT): boxes [batch, post_nms_top_n, 4] in original-image
+// coordinates and scores [batch, post_nms_top_n], zero past each image's roi_counts.  One launch on `stream`; graph-capturable.
+int dt_engine_proposals(dt_engine_t h, float* boxes, float* scores, dt_stream_t stream) {
+    Engine* e = reinterpret_cast<Engine*>(h);
+    if (!e->bound || e->cfg.model_type != 0 || !e->cfg.use_rpn) {
+        fprintf(stderr, "[detectorch_b200] engine: proposals are built for the FPN engine with the RPN\n");
+        return 0;
+    }
+    if (!boxes || !scores || ((uintptr_t)boxes & 15)) { fprintf(stderr, "[detectorch_b200] engine: proposals: bad output pointer\n"); return 0; }
+    collect_outputs_kernel<<<e->cfg.batch, 256, 0, (cudaStream_t)stream>>>(e->col, e->im_info(), e->scaling_factor, boxes, scores);
+    DT_CHECK_CUDA(cudaGetLastError());
+    return 1;
+}
+
 // number of kernel launches stages [first,last] issue (bench.py's gpu_launches)
 int dt_engine_count_launches(dt_engine_t h, int first_stage, int last_stage) {
     Engine* e = reinterpret_cast<Engine*>(h);

@@ -3,6 +3,7 @@
 //   rpn_select_*_kernel, rpn_proposals_kernel, rpn_nms_scan_kernel  top-k + decode + clip + filter + NMS(0.7)   generate_proposals.py:31-122
 //   collect_kernel         merge levels, top-N, FPN level map           collect_and_distribute...py:84-128,
 //                                                                       multilevel_rois.py:41-53
+//   collect_outputs_kernel collected RoIs / scale + their RPN scores       result_utils.py:77 (propose_images only)
 //   fast_props_kernel      pre-computed proposals -> scaled, deduplicated preprocess_sample.py:37-47,61-69,
 //                          RoIs in hash order + FPN level               multilevel_rois.py:19-39
 //   softmax_split_kernel   class softmax + split cls/bbox               detector.py:277-284
@@ -577,6 +578,28 @@ static __global__ void __launch_bounds__(1024) collect_kernel(const __grid_const
         }
     }
     if (threadIdx.x == 0) P.roi_counts[b] = m;
+}
+
+// The collected RoIs in original-image coordinates (rois / scaling_factor in fp32, as postprocess_output divides them) and each one's
+// RPN score, read through the collect's sort order (v0 after the sort); rows >= roi_counts[b] are zero.  Not part of the engine
+// program: dt_engine_proposals launches it after a run that ended at ST_COLLECT.  grid B
+static __global__ void collect_outputs_kernel(const __grid_constant__ CollectParams P, const float* __restrict__ im_info, float scaling_factor,
+                                              float* __restrict__ out_boxes, float* __restrict__ out_scores) {
+    const int b = blockIdx.x;
+    const int cap = P.L * P.post_nms;
+    const int m = P.roi_counts[b];
+    const float s = image_info(im_info, b, 1, 0, 0, scaling_factor).scale;
+    for (int i = threadIdx.x; i < P.top_n; i += blockDim.x) {
+        float4 box = make_float4(0.f, 0.f, 0.f, 0.f);
+        float score = 0.f;
+        if (i < m) {
+            const float* r = P.rois + ((size_t)b * P.top_n + i) * 5;
+            box = make_float4(__fdiv_rn(r[1], s), __fdiv_rn(r[2], s), __fdiv_rn(r[3], s), __fdiv_rn(r[4], s));
+            score = P.scores[(size_t)b * cap + P.v0[(size_t)b * cap + i]];
+        }
+        reinterpret_cast<float4*>(out_boxes)[(size_t)b * P.top_n + i] = box;
+        out_scores[(size_t)b * P.top_n + i] = score;
+    }
 }
 
 // ---------------------------------------------------------------------------------- pre-computed proposals (Fast R-CNN, FPN)

@@ -305,6 +305,19 @@ class Engine:
             self.buffer("fast_props").copy_(torch.from_numpy(block).pin_memory(), non_blocking=True)      # pinned blocks are not reused
             self.buffer("fast_prop_counts").copy_(torch.from_numpy(counts).pin_memory(), non_blocking=True)   # before their copies ran
 
+    def proposals(self, boxes, scores):
+        """After a run through ST_COLLECT (FPN engine with the RPN): the collected RoIs / each image's scaling factor into boxes
+        float32 [batch, post_nms_top_n, 4] and their RPN scores into scores float32 [batch, post_nms_top_n] (dt_engine_proposals), on the
+        current stream; rows past roi_counts are zero."""
+        R = (self.cfg.batch, self.cfg.post_nms_top_n)
+        for t, shape in ((boxes, R + (4,)), (scores, R)):
+            if not t.is_cuda or t.device != self.device or t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != shape:
+                raise ValueError("Engine.proposals: outputs must be contiguous float32 %s / %s tensors on %s" % (R + (4,), R, self.device))
+        f = self.L.dt_engine_proposals
+        f.restype, f.argtypes = ctypes.c_int, [ctypes.c_void_p] * 4
+        with torch.cuda.device(self.device):
+            _lib.check(f(self.h, boxes.data_ptr(), scores.data_ptr(), self._stream()), "dt_engine_proposals")
+
     def profile(self, image, scaling_factor=1.0, first=0, last=11):
         """One event-bracketed pass: list of (ms, algorithmic_flops, stage, block_n) per launch."""
         cap = 512

@@ -23,7 +23,7 @@ import torchvision.models as models
 import collections
 import os
 
-from ..engine import Engine, engine_owning, ST_TRUNK, ST_FPN, ST_ROI_BOX, ST_BOX_HEAD, ST_DETECT, ST_MASK_ROI_FEAT, ST_MASK_OUT
+from ..engine import Engine, engine_owning, ST_TRUNK, ST_FPN, ST_COLLECT, ST_ROI_BOX, ST_BOX_HEAD, ST_DETECT, ST_MASK_ROI_FEAT, ST_MASK_OUT
 
 
 def caffe2_blob_name(key):
@@ -520,6 +520,57 @@ class detector(torch.nn.Module):
         data, sizes, scales, orig = blob.images_to_batch(ims, target_size, max_size, canvas)
         out = self.detect(data, scaling_factor=scales, with_masks=with_masks, image_sizes=sizes, original_sizes=orig, proposals=proposals)
         return result_utils.batch_results(out, orig, num_classes=self.N_classes)
+
+    def propose_images(self, ims, target_size=800, max_size=1333, canvas=None):
+        """uint8 BGR images [H,W,3] of any sizes -> one (boxes float32 [n, 4], scores float32 [n]) per image, in input order: the RPN
+        proposals that forward() of that image alone collects (top post_nms_top_n by score, in that order), boxes divided by the image's
+        scaling factor as postprocess_output divides the RoIs (original-image coordinates), scores their RPN objectness.  One engine
+        run through the collect stage for the whole list (no box head); from the second call on a captured CUDA graph replays it.
+        FPN models with the RPN only: the Fast R-CNN models raise RuntimeError, the C4 models NotImplementedError."""
+        from ..utils import blob
+        from .. import ops
+        if self.family != "fpn":
+            raise NotImplementedError("propose_images: per-image sizes are built for the FPN models only")
+        if not self.use_rpn_head:
+            raise RuntimeError("propose_images: this Fast R-CNN model has no RPN; its proposals come from a file")
+        data, sizes, scales, orig = blob.images_to_batch(ims, target_size, max_size, canvas)
+        B, Hc, Wc = data.size(0), data.size(2), data.size(3)
+        table = self._image_table(B, Hc, Wc, scales, sizes, orig)
+        eng = self.engine_for(B, Hc, Wc)
+        st = getattr(eng, "_proposal_state", None)
+        if st is None:
+            R = eng.cfg.post_nms_top_n
+            with torch.cuda.device(eng.device):
+                st = {"input": torch.empty((B, 3, Hc, Wc), dtype=torch.float32, device=eng.device),
+                      "boxes": torch.empty((B, R, 4), dtype=torch.float32, device=eng.device),
+                      "scores": torch.empty((B, R), dtype=torch.float32, device=eng.device), "graph": None, "seen": 0}
+            eng._proposal_state = st
+
+        def step():
+            eng.run(st["input"], 1.0, ST_TRUNK, ST_COLLECT)
+            eng.proposals(st["boxes"], st["scores"])
+
+        eng.last_scaling_factor = 1.0
+        eng.set_image_info(*table)           # on the current stream, after every run already queued there
+        try:
+            with torch.cuda.device(eng.device):
+                st["input"].copy_(data)      # a fixed input address: the captured graph reads it
+                if st["graph"] is None and st["seen"] >= 1 and self.capture_graphs:
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        step()
+                    st["graph"] = g
+                st["seen"] += 1
+                if st["graph"] is not None:
+                    st["graph"].replay()
+                else:
+                    step()
+        finally:
+            eng.clear_image_info()
+        boxes, scores, counts, flag = ops.to_host(st["boxes"], st["scores"], eng.buffer("roi_counts"), eng.buffer("range_flag"))
+        if int(flag[0]) != 0:
+            eng.check_range()
+        return [(boxes[b, :int(counts[b])].copy(), scores[b, :int(counts[b])].copy()) for b in range(B)]
 
     def _launch_detect(self, eng, images, scaling_factor, last, use_table):
         if not images.is_cuda:

@@ -564,3 +564,126 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
         E.ious = {(gt.img_ids[k % I], gt.cat_ids[k // I]): iv[o:o + d * g].reshape(d, g)
                   for k, d, g, o in zip(pk, kept, gn, pairs[:, 6]) if g > 0}
     return E
+
+
+# ------------------------------------------------------------------------------------------------------------ proposal recall
+# evaluate_box_proposals' area ranges (json_dataset_evaluator.py:247-264), both bounds inclusive
+PROPOSAL_AREAS = {'all': [0 ** 2, 1e5 ** 2], 'small': [0 ** 2, 32 ** 2], 'medium': [32 ** 2, 96 ** 2], 'large': [96 ** 2, 1e5 ** 2],
+                  '96-128': [96 ** 2, 128 ** 2], '128-256': [128 ** 2, 256 ** 2], '256-512': [256 ** 2, 512 ** 2], '512-inf': [512 ** 2, 1e5 ** 2]}
+_BOX_COORD_MAX = 1e15            # |coordinate| bound that keeps every float32 area and union of bbox_overlaps finite
+_AREA_DTYPES = (np.float32, np.float64, np.int32, np.int64)
+
+
+def _entry_arrays(n, e):
+    what = "roidb entry %d" % n
+    if not isinstance(e, dict) or any(k not in e for k in ('boxes', 'gt_classes', 'is_crowd', 'seg_areas')):
+        raise ValueError("%s: needs 'boxes', 'gt_classes', 'is_crowd' and 'seg_areas'" % what)
+    boxes, cls, crowd, areas = (np.asarray(e[k]) for k in ('boxes', 'gt_classes', 'is_crowd', 'seg_areas'))
+    if boxes.ndim != 2 or boxes.shape[1] != 4 or not (np.issubdtype(boxes.dtype, np.floating) or np.issubdtype(boxes.dtype, np.integer)):
+        raise ValueError("%s: boxes must be a numeric [n, 4] array" % what)
+    r = boxes.shape[0]
+    if cls.shape != (r,) or not np.issubdtype(cls.dtype, np.integer):
+        raise ValueError("%s: gt_classes must be an integer array of one value per box" % what)
+    if crowd.shape != (r,) or not (crowd.dtype == np.bool_ or np.issubdtype(crowd.dtype, np.integer)):
+        raise ValueError("%s: is_crowd must be a bool or integer array of one value per box" % what)
+    if areas.shape != (r,) or areas.dtype.type not in _AREA_DTYPES:
+        raise ValueError("%s: seg_areas must be a float32 / float64 / int32 / int64 array of one value per box" % what)
+    return boxes, cls, crowd, areas
+
+
+def _proposal_tables(roidb):
+    """roidb -> (prop_off, props, gt_off, gts, gt_area): per image its proposals (gt_classes == 0 rows, in order) and its ground truth
+    (gt_classes > 0, not crowd), boxes as float32 as bbox_overlaps is given them.  Malformed entries raise ValueError."""
+    props, gts, areas = [], [], []
+    np_i, ng_i = np.zeros(len(roidb), np.int64), np.zeros(len(roidb), np.int64)
+    for n, e in enumerate(roidb):
+        boxes, cls, crowd, area = _entry_arrays(n, e)
+        g = (cls > 0) & (crowd == 0)
+        p = cls == 0
+        b = boxes.astype(np.float32, copy=False)
+        props.append(b[p]); gts.append(b[g]); areas.append(area[g].astype(np.float64))
+        np_i[n], ng_i[n] = props[-1].shape[0], gts[-1].shape[0]
+    props = np.ascontiguousarray(np.concatenate(props) if props else np.zeros((0, 4), np.float32), np.float32)
+    gts = np.ascontiguousarray(np.concatenate(gts) if gts else np.zeros((0, 4), np.float32), np.float32)
+    gt_area = np.concatenate(areas) if areas else np.zeros(0)
+    for what, b in (("proposal", props), ("ground-truth", gts)):
+        if b.size and not (np.all(np.isfinite(b)) and np.abs(b).max() <= _BOX_COORD_MAX):
+            raise ValueError("roidb: a %s box is not finite or has a coordinate beyond %g" % (what, _BOX_COORD_MAX))
+    off = lambda c: np.concatenate([[0], np.cumsum(c)]).astype(np.int64)
+    return off(np_i), props, off(ng_i), gts, gt_area
+
+
+def _limit(v):
+    if v is None:
+        return -1
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 0:
+        raise ValueError("proposal limit must be None or a non-negative integer, got %r" % (v,))
+    return int(v)
+
+
+def box_proposal_recall(roidb, areas=('all', 'small', 'medium', 'large'), limits=(100, 1000), thresholds=None, device=None):
+    """Detectron's evaluate_box_proposals(json_dataset, roidb, thresholds, area, limit) for every (area, limit) combination at once
+    -> {(area, limit): {'ar', 'recalls', 'thresholds', 'gt_overlaps', 'num_pos'}}, each dict equal to what the reference returns.
+    roidb: entries with 'boxes' (ground truth then proposals), 'gt_classes' (0 for a proposal), 'is_crowd' and 'seg_areas', as
+    JsonDataset.get_roidb(gt=True, proposal_file=...) builds them.  The greedy matching of every (image, combination) runs in one
+    CUDA launch; the host sorts the overlaps and counts them against the thresholds as the reference does."""
+    areas, limits = list(areas), list(limits)
+    for a in areas:
+        if a not in PROPOSAL_AREAS:
+            raise ValueError("Unknown area range: {}".format(a))
+    combos = [(a, l) for a in areas for l in limits]
+    lims = np.array([_limit(l) for _, l in combos], np.int64)
+    rng = np.array([PROPOSAL_AREAS[a] for a, _ in combos], np.float64).reshape(-1, 2)
+    prop_off, props, gt_off, gts, gt_area = _proposal_tables(roidb)
+    I, C = len(prop_off) - 1, len(combos)
+    np_i, ng_i = np.diff(prop_off), np.diff(gt_off)
+    img_of_gt = np.repeat(np.arange(I), ng_i)
+    # GTs inside each range per image (the kernel selects the same ones), outputs only for images with proposals
+    sel = np.zeros((C, I), np.int64)
+    for c in range(C):
+        m = (gt_area >= rng[c, 0]) & (gt_area <= rng[c, 1])
+        sel[c] = np.bincount(img_of_gt[m], minlength=I)
+    outlen = np.where(np_i[None, :] > 0, sel, 0)
+    out_off = np.concatenate([[0], np.cumsum(outlen.reshape(-1))]).astype(np.int64)
+    total = int(out_off[-1])
+    max_gts = int(ng_i.max()) if I else 0
+    max_props = int(np_i.max()) if I else 0
+    L = _lib.lib()
+    smem = L.dt_proposal_recall_smem_bytes(max_gts, max_props)
+    if smem == 0 or smem > 227 * 1024:
+        raise ValueError("box_proposal_recall: %d ground-truth boxes and %d proposals in one image do not fit one CTA's shared memory" %
+                         (max_gts, max_props))
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    ov = np.zeros(0)
+    if total and I:
+        up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (prop_off, props.reshape(-1) if props.size else np.zeros(4, np.float32),
+                                                                           gt_off, gts.reshape(-1), gt_area, rng.reshape(-1), lims, out_off[:-1])]
+        out = torch.empty((total,), dtype=torch.float64, device=dev)
+        flag = torch.zeros((1,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.dt_proposal_recall(I, C, _p(up[0]), _p(up[1]), _p(up[2]), _p(up[3]), _p(up[4]), _p(up[5]), _p(up[6]), _p(up[7]),
+                                            max_gts, max_props, _p(out), _p(flag), _stream(dev)), "dt_proposal_recall")
+        f = int(flag.item())
+        if f & 2:
+            raise ValueError("roidb: a proposal and a ground-truth box whose union is 0 (bbox_overlaps divides by zero)")
+        if f & 1:
+            raise ValueError("roidb: a recorded overlap below 0 (the reference asserts gt_ovr >= 0)")
+        ov = out.cpu().numpy()
+    res = {}
+    for c, key in enumerate(combos):
+        gt_overlaps = np.sort(ov[out_off[c * I]:out_off[(c + 1) * I]])
+        res[key] = _recall_summary(gt_overlaps, int(sel[c].sum()), thresholds)
+    return res
+
+
+def _recall_summary(gt_overlaps, num_pos, thresholds):
+    """json_dataset_evaluator.py:308-319 on the sorted overlaps."""
+    if thresholds is None:
+        step = 0.05
+        thresholds = np.arange(0.5, 0.95 + 1e-5, step)
+    recalls = np.zeros_like(thresholds)
+    # compute recall for each iou threshold
+    for i, t in enumerate(thresholds):
+        recalls[i] = (gt_overlaps >= t).sum() / float(num_pos)
+    ar = recalls.mean()
+    return {'ar': ar, 'recalls': recalls, 'thresholds': thresholds, 'gt_overlaps': gt_overlaps, 'num_pos': num_pos}

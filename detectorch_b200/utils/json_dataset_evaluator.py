@@ -3,7 +3,8 @@ signatures and the same COCOeval numbers (coco_eval.evaluate), without writing, 
 switches with one import line:
     from detectorch_b200.utils.json_dataset_evaluator import evaluate_boxes, evaluate_masks
 json_dataset.COCO.dataset supplies the ground truth (built on the device once per json_dataset, kept on it); its classes /
-category_to_id_map give the json category id of each contiguous class, as _write_coco_*_results_file uses them."""
+category_to_id_map give the json category id of each contiguous class, as _write_coco_*_results_file uses them.
+evaluate_box_proposals (:238-320) is the proposal recall of coco_eval.box_proposal_recall, one (area, limit) combination."""
 import logging
 
 import numpy as np
@@ -53,3 +54,11 @@ def _log_detection_eval_metrics(E):
     logger.info('~~~~ Mean and per-category AP @ IoU=[0.50,0.95] ~~~~')
     logger.info('{:.1f}'.format(100 * ap))
     E.summarize()
+
+
+def evaluate_box_proposals(json_dataset, roidb, thresholds=None, area='all', limit=None):
+    """Detectron's proposal recall (AR over IoU thresholds for one area range and proposal limit) -> {'ar', 'recalls', 'thresholds',
+    'gt_overlaps', 'num_pos'}, equal to the reference's; the greedy matching runs on the device.  An unknown area raises ValueError."""
+    if area not in coco_eval.PROPOSAL_AREAS:
+        raise ValueError('Unknown area range: {}'.format(area))
+    return coco_eval.box_proposal_recall(roidb, [area], [limit], thresholds)[(area, limit)]

@@ -254,6 +254,11 @@ int dt_engine_use_image_info(dt_engine_t e, int enabled);
  *         8 mask RoIs, 9 RoIAlign(mask), 10 mask convs, 11 mask output */
 int dt_engine_run(dt_engine_t e, const float* image_nchw, float scaling_factor, int first_stage, int last_stage, dt_stream_t stream);
 int dt_engine_count_launches(dt_engine_t e, int first_stage, int last_stage);
+/* the RPN proposals of the last run through stage 4 (FPN engine with the RPN; 0 otherwise): boxes [batch, post_nms_top_n, 4] float32
+ * = the collected RoIs / each image's scaling factor (fp32 division, original-image coordinates), scores [batch, post_nms_top_n] float32
+ * = their RPN objectness, in the collect's order; rows past roi_counts are zero.  boxes 16-byte aligned.  Launched on `stream`, not
+ * part of the engine program (a run to the detections never pays for it). */
+int dt_engine_proposals(dt_engine_t e, float* boxes, float* scores, dt_stream_t stream);
 /* measurement aid: one pass with a CUDA-event pair around every launch on `stream` (synchronises at the end);
  * per-op milliseconds, algorithmic FLOPs (0 for non-GEMM ops), stage id, BLOCK_N (0 for non-GEMM ops) */
 int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_factor, int first_stage, int last_stage, dt_stream_t stream,
@@ -291,6 +296,22 @@ int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, con
                  int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order, const double* gt_f, const int64_t* gt_i,
                  const uint32_t* gt_counts, const double* params, double* precision, double* recall, double* scores, double* ious, void* workspace,
                  dt_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Proposal recall (Detectron's evaluate_box_proposals), bit for bit.  One CTA per (image, combination); every combination of
+ * (area range, proposal limit) in one launch.
+ *   prop_off / gt_off [I+1] int64  each image's range in props [NP, 4] / gts [NG, 4] (float32 x1 y1 x2 y2; gts: gt_classes > 0, not crowd)
+ *   gt_area [NG] double            seg_areas
+ *   area_rng [C, 2] double         inclusive range; limits [C] int64 (< 0: no limit)
+ *   out_off [C, I] int64           first output of (combination, image): the image's GTs in the range when it has proposals, else none
+ *   max_gts / max_props            the largest gt / proposal count of one image (shared-memory sizing)
+ *   out double                     each GT's recorded overlap, in assignment order, 0 past the last round
+ *   flag int (zeroed by the caller) bit 0: a chosen overlap < 0 (the reference asserts), bit 1: a union of 0 (it divides by zero)
+ * dt_proposal_recall_smem_bytes: the dynamic shared memory one CTA needs (the launch refuses more than 227 KB). */
+int64_t dt_proposal_recall_smem_bytes(int max_gts, int64_t max_props);
+int dt_proposal_recall(int num_images, int num_combos, const int64_t* prop_off, const float* props, const int64_t* gt_off, const float* gts,
+                       const double* gt_area, const double* area_rng, const int64_t* limits, const int64_t* out_off, int max_gts,
+                       int64_t max_props, double* out, int* flag, dt_stream_t stream);
 
 /* library / build info */
 const char* dt_version(void);
