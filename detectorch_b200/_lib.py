@@ -57,6 +57,12 @@ SIGNATURES = {
     "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                              c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "dt_coco_results_append": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                       c_void_p, c_void_p, c_void_p]),
+    "dt_coco_results_count": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
+    "dt_coco_results_write": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_proposal_recall_smem_bytes": (c_int64, [c_int, c_int64]),
     "dt_proposal_recall": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64,
                                    c_void_p, c_void_p, c_void_p]),

@@ -65,6 +65,56 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
     return 1;
 }
 
+extern "C" int dt_coco_results_append(int batch, int cap, int num_classes, const float* boxes, const float* scores, const int* classes,
+                                      const int* counts, const int64_t* images, const int64_t* str_offs, int64_t char_base, float* rec_f,
+                                      int64_t* rec_i, int* err, dt_stream_t stream) {
+    if (batch < 0 || cap < 0 || num_classes < 1 || char_base < 0) { fprintf(stderr, "dt_coco_results_append: bad sizes\n"); return 0; }
+    if ((int64_t)batch * cap == 0) return 1;
+    if (!boxes || !scores || !classes || !counts || !images || !rec_f || !rec_i || !err) {
+        fprintf(stderr, "dt_coco_results_append: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_results_append_launch(batch, cap, num_classes, boxes, scores, classes, counts, images, str_offs, char_base, rec_f, rec_i,
+                                             err, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int dt_coco_results_count(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k,
+                                     const int* ord_i, int num_images, int num_cats, const int64_t* gt_keys, int64_t num_gts, int* bin_cnt,
+                                     int64_t* scan_in, int* nonfinite, dt_stream_t stream) {
+    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0) {
+        fprintf(stderr, "dt_coco_results_count: bad sizes\n");
+        return 0;
+    }
+    if ((num_records > 0 && (!rec_f || !rec_i || !cls_k || !ord_i || !nonfinite)) ||
+        ((int64_t)num_images * num_cats > 0 && (!bin_cnt || !scan_in || (num_gts > 0 && !gt_keys)))) {
+        fprintf(stderr, "dt_coco_results_count: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_results_count_launch(num_records, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, gt_keys, num_gts, bin_cnt,
+                                            scan_in, nonfinite, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int dt_coco_results_write(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k,
+                                     const int* ord_i, int num_images, int num_cats, const int64_t* scan, const int64_t* gt_keys, int64_t num_gts,
+                                     int64_t* det_key, double* det_f, int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off,
+                                     dt_stream_t stream) {
+    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0) {
+        fprintf(stderr, "dt_coco_results_write: bad sizes\n");
+        return 0;
+    }
+    const bool bins = (int64_t)num_images * num_cats > 0;
+    if ((num_records > 0 && (!rec_f || !rec_i || !cls_k || !ord_i || (bins && (!det_key || !det_f || !det_i)))) || !cat_kept || !order_off ||
+        (bins && (!scan || (num_gts > 0 && !gt_keys)))) {
+        fprintf(stderr, "dt_coco_results_write: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_results_write_launch(bins ? num_records : 0, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, scan, gt_keys,
+                                            num_gts, det_key, det_f, det_i, pairs, cat_kept, order_off, (cudaStream_t)stream));
+    return 1;
+}
+
 extern "C" int64_t dt_proposal_recall_smem_bytes(int max_gts, int64_t max_props) {
     if (max_gts < 0 || max_props < 0 || max_gts > (1 << 24) || max_props > (1ll << 36)) return 0;
     return (int64_t)proposal_recall_smem(max_gts, (int)((max_props + 31) / 32));

@@ -521,4 +521,179 @@ inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_activ
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------ device-resident results
+// utils.coco_eval.DeviceResults keeps detect() batches on the device as raw records, one per (image, slot) of each batch, in the order
+// they were added.  At evaluate() they are flattened into the det_f / det_i / pairs / cat_kept / order_off tables of dt_coco_eval, in
+// the order the host conversion gives them: by key = k * I + i (category index k, image index i), slot order inside a key.
+//
+//   coco_results_append_kernel   one thread per (image, slot) of a batch: the record, the slot's rank inside its class in the image,
+//                                and the batch_results checks (class in 1..num_classes-1, slots grouped by class) as an error flag.
+//   coco_results_count_kernel    one thread per record: the last record of each (image, class) group writes the group's size to its
+//                                (category, image) bin; records of live slots with non-finite values set a flag.
+//   coco_results_bins_kernel     one thread per bin: D, D > 0, min(D, 10), min(D, 100) and min(D, 100) G for the scans (torch.cumsum).
+//   coco_results_scatter_kernel  one thread per record: its det_f / det_i row at its bin's start + its rank (a counting sort).
+//   coco_results_pairs_kernel    one thread per bin: the pair row of a non-empty bin at its rank among them; one thread per category:
+//                                cat_kept and order_off from the scans at the category's first bin.
+// Each (category, image) bin is filled by one class of one image (category ids are distinct), so no two groups share a bin and the
+// only atomics are the integer error flags.
+// record: f32 [x1, y1, x2, y2, score]; i64 [image ordinal (-1: dead slot), class, rank in class, char offset, char count, h, w]
+constexpr int kCocoRecF = 5, kCocoRecI = 7;
+// the bin scans, int64 [5][K I] inclusive: D, D > 0 (= min(D, 1)), min(D, 10), min(D, 100), min(D, 100) G
+constexpr int kCocoScanRows = 5;
+
+__device__ __forceinline__ int64_t coco_lower_bound(const int64_t* a, int64_t n, int64_t v, bool upper) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (a[mid] < v || (upper && a[mid] == v)) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// images [B, 3] int64: ordinal, h, w; str_offs [B cap + 1] the batch's string offsets (NULL without masks), placed at char_base.
+// err[0] |= 1 and err[1] = min ordinal of an image whose live classes are outside 1..num_classes-1 or not grouped.
+__global__ void coco_results_append_kernel(int B, int cap, int num_classes, const float* __restrict__ boxes, const float* __restrict__ scores,
+                                           const int* __restrict__ classes, const int* __restrict__ counts, const int64_t* __restrict__ images,
+                                           const int64_t* __restrict__ str_offs, int64_t char_base, float* __restrict__ rec_f,
+                                           int64_t* __restrict__ rec_i, int* __restrict__ err) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)B * cap) return;
+    const int b = (int)(e / cap), d = (int)(e % cap);
+    const int n = min(max(counts[b], 0), cap);
+    int64_t* R = rec_i + e * kCocoRecI;
+    float* F = rec_f + e * kCocoRecF;
+    if (d >= n) {
+        R[0] = -1;
+        for (int j = 1; j < kCocoRecI; j++) R[j] = 0;
+        for (int j = 0; j < kCocoRecF; j++) F[j] = 0.f;
+        return;
+    }
+    const int* cl = classes + (int64_t)b * cap;
+    const int c = cl[d];
+    const int64_t* im = images + 3 * (int64_t)b;
+    if (c < 1 || c >= num_classes || (d > 0 && cl[d - 1] > c)) {
+        atomicOr(err, 1);
+        atomicMin(err + 1, (int)im[0]);
+    }
+    int r = 0;
+    while (r < d && cl[d - 1 - r] == c) r++;
+    R[0] = im[0]; R[1] = c; R[2] = r;
+    if (str_offs) {
+        R[3] = char_base + str_offs[e]; R[4] = str_offs[e + 1] - str_offs[e]; R[5] = im[1]; R[6] = im[2];
+    } else {
+        R[3] = R[4] = R[5] = R[6] = 0;
+    }
+    for (int j = 0; j < 4; j++) F[j] = boxes[4 * e + j];
+    F[4] = scores[e];
+}
+
+// the category index of a record (-1: dead slot, or a class without a category); cls_k [num_cls], ord_i [ordinals] -> gt image index
+__device__ __forceinline__ int coco_rec_cat(const int64_t* R, int num_cls, const int* cls_k) {
+    const int64_t o = R[0], c = R[1];
+    if (o < 0 || c < 0 || c >= num_cls) return -1;
+    return cls_k[c];
+}
+
+__global__ void coco_results_count_kernel(int64_t n, const float* __restrict__ rec_f, const int64_t* __restrict__ rec_i, int num_cls,
+                                          const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, int* __restrict__ bin_cnt,
+                                          int* __restrict__ nonfinite) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int64_t* R = rec_i + r * kCocoRecI;
+    const int k = coco_rec_cat(R, num_cls, cls_k);
+    if (k < 0) return;
+    const float* F = rec_f + r * kCocoRecF;
+    bool fin = true;
+    for (int j = 0; j < kCocoRecF; j++) fin = fin && isfinite(F[j]);
+    if (!fin) atomicOr(nonfinite, 1);
+    const bool last = r + 1 == n || R[kCocoRecI] != R[0] || R[kCocoRecI + 1] != R[1];
+    if (last) bin_cnt[(int64_t)k * I + ord_i[R[0]]] = (int)R[2] + 1;
+}
+
+__global__ void coco_results_bins_kernel(int64_t nb, const int* __restrict__ bin_cnt, const int64_t* __restrict__ gt_keys, int64_t G,
+                                         int64_t* __restrict__ vals) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    const int64_t D = bin_cnt[b];
+    int64_t gn = 0;
+    if (D > 0) gn = coco_lower_bound(gt_keys, G, b, true) - coco_lower_bound(gt_keys, G, b, false);
+    const int64_t kept = D < kCocoKeep ? D : kCocoKeep;
+    vals[b] = D;
+    vals[nb + b] = D > 0;
+    vals[2 * nb + b] = D < 10 ? D : 10;
+    vals[3 * nb + b] = kept;
+    vals[4 * nb + b] = kept * gn;
+}
+
+// det_f: (score, x1, y1, x2 - x1 + 1, y2 - y1 + 1), each term the double of the stored float, as the host's float64 arithmetic
+__global__ void coco_results_scatter_kernel(int64_t n, const float* __restrict__ rec_f, const int64_t* __restrict__ rec_i, int num_cls,
+                                            const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, const int64_t* __restrict__ scan,
+                                            int64_t* __restrict__ det_key, double* __restrict__ det_f, int64_t* __restrict__ det_i) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int64_t* R = rec_i + r * kCocoRecI;
+    const int k = coco_rec_cat(R, num_cls, cls_k);
+    if (k < 0) return;
+    const int64_t key = (int64_t)k * I + ord_i[R[0]];
+    const int64_t pos = (key > 0 ? scan[key - 1] : 0) + R[2];
+    const float* F = rec_f + r * kCocoRecF;
+    const double x1 = F[0], y1 = F[1], x2 = F[2], y2 = F[3];
+    double* D = det_f + pos * kCocoDetF;
+    D[0] = (double)F[4]; D[1] = x1; D[2] = y1;
+    D[3] = __dadd_rn(__dsub_rn(x2, x1), 1.0); D[4] = __dadd_rn(__dsub_rn(y2, y1), 1.0);
+    int64_t* DI = det_i + pos * kCocoDetI;
+    DI[0] = R[3]; DI[1] = R[4]; DI[2] = R[5]; DI[3] = R[6];
+    det_key[pos] = key;
+}
+
+__global__ void coco_results_pairs_kernel(int K, int I, const int64_t* __restrict__ scan, const int64_t* __restrict__ gt_keys, int64_t G,
+                                          int64_t* __restrict__ pairs, int64_t* __restrict__ cat_kept, int64_t* __restrict__ order_off) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t nb = (int64_t)K * I;
+    auto excl = [&](int row, int64_t b) -> int64_t { return b > 0 ? scan[row * nb + b - 1] : 0; };
+    if (t < nb) {
+        const int64_t d0 = excl(0, t), D = scan[t] - d0;
+        if (D > 0) {
+            const int64_t g0 = coco_lower_bound(gt_keys, G, t, false), g1 = coco_lower_bound(gt_keys, G, t, true);
+            int64_t* P = pairs + excl(1, t) * kCocoPairCols;
+            P[0] = t; P[1] = d0; P[2] = D; P[3] = g0; P[4] = g1 - g0; P[5] = excl(3, t); P[6] = excl(4, t);
+        }
+    }
+    if (t <= K) {
+        const int64_t b = t * I;                  // category t's first bin; t == K: the totals
+        const int64_t T1 = excl(1, nb), T2 = excl(2, nb);
+        cat_kept[t] = excl(3, b);
+        order_off[t] = excl(1, b);
+        order_off[(K + 1) + t] = T1 + excl(2, b);
+        order_off[2 * (K + 1) + t] = T1 + T2 + excl(3, b);
+    }
+}
+
+inline cudaError_t coco_results_append_launch(int B, int cap, int num_classes, const float* boxes, const float* scores, const int* classes,
+                                              const int* counts, const int64_t* images, const int64_t* str_offs, int64_t char_base, float* rec_f,
+                                              int64_t* rec_i, int* err, cudaStream_t st) {
+    const int64_t n = (int64_t)B * cap;
+    coco_results_append_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(B, cap, num_classes, boxes, scores, classes, counts, images, str_offs,
+                                                                           char_base, rec_f, rec_i, err);
+    return cudaGetLastError();
+}
+
+inline cudaError_t coco_results_count_launch(int64_t n, const float* rec_f, const int64_t* rec_i, int num_cls, const int* cls_k, const int* ord_i,
+                                             int I, int K, const int64_t* gt_keys, int64_t G, int* bin_cnt, int64_t* vals, int* nonfinite,
+                                             cudaStream_t st) {
+    const int64_t nb = (int64_t)K * I;
+    if (n > 0) coco_results_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, bin_cnt, nonfinite);
+    if (nb > 0) coco_results_bins_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(nb, bin_cnt, gt_keys, G, vals);
+    return cudaGetLastError();
+}
+
+inline cudaError_t coco_results_write_launch(int64_t n, const float* rec_f, const int64_t* rec_i, int num_cls, const int* cls_k, const int* ord_i,
+                                             int I, int K, const int64_t* scan, const int64_t* gt_keys, int64_t G, int64_t* det_key, double* det_f,
+                                             int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off, cudaStream_t st) {
+    const int64_t nb = (int64_t)K * I, nt = nb > K + 1 ? nb : K + 1;
+    if (n > 0) coco_results_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, scan, det_key, det_f, det_i);
+    coco_results_pairs_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(K, I, scan, gt_keys, G, pairs, cat_kept, order_off);
+    return cudaGetLastError();
+}
+
 }  // namespace dt

@@ -5,6 +5,7 @@ file that lib/utils/json_dataset_evaluator.py would write; no file is written.
     gt = CocoGroundTruth("instances_minival2014.json")   # or the annotation dict; GT masks are built once, on the device
     E = evaluate(gt, detector.detect_images(ims), "segm")  # or evaluate(gt, all_boxes, "bbox") / evaluate(gt, all_boxes, "segm", all_segms)
     E.stats, E.eval["precision"]                          # summarize()'s 12 numbers, [T, R, K, A, M]
+    acc = DeviceResults(); acc.add(detector.detect(...), image_ids, original_sizes=orig); evaluate(gt, acc, "segm")   # no host copy
 
 The host only checks and flattens the annotations and results into arrays (csrc/coco_eval.cuh documents their layout); everything
 numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before the evaluation is
@@ -243,6 +244,7 @@ class CocoGroundTruth:
             self._build_masks(segs)
         self.gt_f = torch.from_numpy(self._gt_f).to(self.device)
         self.gt_i = torch.from_numpy(self._gt_i).to(self.device)
+        self.keys_d = torch.from_numpy(keys).to(self.device)                        # DeviceResults looks pairs' gts up on the device
 
     def _build_masks(self, segs):
         """Flatten every mask into the annotation / part tables, check it, then convert on the device in bounded chunks."""
@@ -504,8 +506,8 @@ def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids):
 
 def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False):
     """COCOeval(gt, loadRes(results file), iou_type).evaluate() + accumulate() on the device -> CocoEvalResult.
-    results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), or the notebooks' all_boxes
-    [class][image] (with all_segms [class][image] for 'segm').  category_ids: json id of contiguous class j (1-based) at j - 1;
+    results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), the notebooks' all_boxes
+    [class][image] (with all_segms [class][image] for 'segm'), or a DeviceResults (flattened on the device, on gt's device).  category_ids: json id of contiguous class j (1-based) at j - 1;
     default: the dataset's category order, as JsonDataset builds its classes.  keep_ious: also return COCOeval's .ious, {(image id,
     category id): [min(D, 100), G] array} for the pairs with detections and GTs."""
     if iou_type not in ('bbox', 'segm'):
@@ -517,10 +519,27 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
     category_ids = list(gt.category_ids if category_ids is None else category_ids)
     if any(c not in set(gt.cat_ids) for c in category_ids):
         raise ValueError("category_ids names a category the ground truth does not have")
+    if isinstance(results, DeviceResults):
+        if all_segms is not None:
+            raise ValueError("a DeviceResults carries its masks; all_segms is for all_boxes input")
+        f = _flatten_device(gt, results, iou_type, category_ids)
+        return _evaluate_tables(gt, iou_type, None, f['pairs'], f['cat_kept'], f['order_off'], f['det_f'], f['det_i'], f['chars'],
+                                f['num_chars'], f['num_kept'], f['num_ious'], f['num_order'], keep_ious)
     boxes, segms = _per_class(gt, results, all_segms, iou_type)
     key, det_f, det_i, chars = _flatten_results(gt, boxes, segms, iou_type, category_ids)
-    I, K, N = gt.num_images, gt.num_cats, len(key)
-    # (category, image) pairs with detections
+    pairs, cat_kept, order_off = _pair_tables(gt, key)
+    kept, gn = np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
+    n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(order_off[-1, -1])
+    dev = gt.device
+    up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, cat_kept, order_off, det_f, det_i)]
+    ch = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
+    return _evaluate_tables(gt, iou_type, pairs, *up, ch, len(chars), n_kept, n_iou, n_order, keep_ious)
+
+
+def _pair_tables(gt, key):
+    """dt_coco_eval's tables of the (category, image) pairs with detections, for results sorted by key = k * I + i -> (pairs [P, 7]:
+    key, first detection, D, first gt, G, first kept slot, first IoU; cat_kept [K + 1]; order_off [3, K + 1])."""
+    I, K = gt.num_images, gt.num_cats
     pk, pstart, pcount = np.unique(key, return_index=True, return_counts=True)
     g0 = np.searchsorted(gt.keys, pk, 'left')
     gn = np.searchsorted(gt.keys, pk, 'right') - g0
@@ -537,33 +556,219 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
         c = np.bincount(pcat, weights=np.minimum(pcount, cut), minlength=K)[:K].astype(np.int64)
         order_off[m] = base + np.concatenate([[0], np.cumsum(c)])
         base = order_off[m, -1]
-    n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(base)
+    return pairs, cat_kept, order_off
+
+
+def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_f_d, det_i_d, ch, num_chars, n_kept, n_iou, n_order, keep_ious):
+    """dt_coco_eval on the flattened results, already on gt's device (pairs: their host copy, or None to read it back for keep_ious)."""
+    I, K, N = gt.num_images, gt.num_cats, int(det_f_d.shape[0])
     dev = gt.device
     T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
     prec = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
     rec = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
     scr = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
     L = _lib.lib()
-    up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, gt.cat_gt, cat_kept, order_off, det_f, det_i, _params())]
-    ch = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
+    cat_gt_d, par_d = (torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (gt.cat_gt, _params()))
     if iou_type == 'segm' and N:
         # runs that do not cover h * w pixels would make rleIou's merge loop forever: decoded and summed on the device, refused here
         bad = torch.empty((N,), dtype=torch.uint8, device=dev)
-        _lib.check(L.dt_coco_det_check(N, _p(up[5]), _p(ch), _p(bad), _stream(dev)), "dt_coco_det_check")
+        _lib.check(L.dt_coco_det_check(N, _p(det_i_d), _p(ch), _p(bad), _stream(dev)), "dt_coco_det_check")
         nb = torch.nonzero(bad).flatten()[:1].cpu().numpy()
         if len(nb):
             raise ValueError("results: RLE counts of result %d (in (category, image) order) do not sum to h * w" % nb[0])
     ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious else None
-    ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, len(chars), n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
-    _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, len(pk), _p(up[0]), _p(up[1]), _p(up[2]), _p(up[3]), N, _p(up[4]),
-                              _p(up[5]), _p(ch), len(chars), n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f), _p(gt.gt_i), _p(gt.gt_counts),
-                              _p(up[6]), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
+    ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, num_chars, n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
+    _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, int(pairs_d.shape[0]), _p(pairs_d), _p(cat_gt_d), _p(cat_kept_d),
+                              _p(order_off_d), N, _p(det_f_d), _p(det_i_d), _p(ch), num_chars, n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f),
+                              _p(gt.gt_i), _p(gt.gt_counts), _p(par_d), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
     E = CocoEvalResult(Params(gt, iou_type), prec.cpu().numpy(), rec.cpu().numpy(), scr.cpu().numpy())
     if keep_ious:
+        if pairs is None:
+            pairs = pairs_d.cpu().numpy()
+        pk, kept, gn = pairs[:, 0], np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
         iv = ious.cpu().numpy()
         E.ious = {(gt.img_ids[k % I], gt.cat_ids[k // I]): iv[o:o + d * g].reshape(d, g)
                   for k, d, g, o in zip(pk, kept, gn, pairs[:, 6]) if g > 0}
     return E
+
+
+# ------------------------------------------------------------------------------------------------------------ device-resident results
+_INT32_MAX = 2 ** 31 - 1
+
+
+def _pinned_upload(a, dev):
+    """A small host table -> device, copied from pinned memory without synchronising the host."""
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+
+
+class DeviceResults:
+    """detect() outputs accumulated on the device, for evaluate(gt, acc, 'bbox' | 'segm') without bringing any detection to the host:
+
+        acc = DeviceResults()
+        for ...:
+            out = model.detect(blob, scaling_factor=scales, image_sizes=sizes, original_sizes=orig)
+            acc.add(out, image_ids, original_sizes=orig)     # json image id of each image of the batch
+        E = evaluate(gt, acc, 'segm')
+
+    The evaluation equals evaluate(gt, per_image_results, ...) where image i holds what batch_results returned for it (images never
+    added have no detections).  add() only enqueues work on the current stream: detect()'s buffers may be overwritten by the next call
+    straight away.  Without masks it does not synchronise the host; with masks it pastes and encodes them as batch_results does (one
+    synchronisation) and keeps the strings in a device char buffer.  Each add keeps B * cap records of 76 bytes (+ the strings).
+    evaluate() takes K * I bins (K categories, I images of the ground truth) of 84 bytes each: an int32 counter and 5 int64 values with
+    their scans, 34 MB for 80 x 5000.  Device-side problems (classes not grouped or out of range, non-finite values) are raised by
+    evaluate().  The category ids given to evaluate() must be distinct, so that each (category, image) bin holds one class's slots."""
+    _MIN_RECORDS = 1 << 12          # initial capacities; both buffers then grow geometrically
+    _MIN_CHARS = 1 << 20
+
+    def __init__(self, device=None):
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if dev.type != 'cuda':
+            raise ValueError("DeviceResults lives on a CUDA device, got %s" % dev)
+        self.device = torch.device('cuda', torch.cuda.current_device() if dev.index is None else dev.index)
+        self.image_ids = []                 # json id of each image ordinal, in the order added
+        self._ordinal = {}
+        self._where = []                    # per ordinal: (position in its detect() batch, num_classes of its add)
+        self._num_records = self._num_chars = 0
+        self._num_classes = 1
+        self._all_masks = True
+        self._rec_f = self._rec_i = self._chars = None
+        with torch.cuda.device(self.device):
+            self._err = _pinned_upload(np.array([0, _INT32_MAX], np.int32), self.device)
+
+    def __len__(self):
+        return len(self.image_ids)
+
+    def _reserve(self, records, chars):
+        dev, n = self.device, self._num_records
+        if self._rec_f is None or records > self._rec_f.shape[0]:
+            cap = max(records, 2 * (0 if self._rec_f is None else self._rec_f.shape[0]), self._MIN_RECORDS)
+            f = torch.empty((cap, 5), dtype=torch.float32, device=dev)
+            i = torch.empty((cap, 7), dtype=torch.int64, device=dev)
+            if n:
+                f[:n].copy_(self._rec_f[:n]); i[:n].copy_(self._rec_i[:n])
+            self._rec_f, self._rec_i = f, i
+        if chars and (self._chars is None or chars > self._chars.shape[0]):
+            cap = max(chars, 2 * (0 if self._chars is None else self._chars.shape[0]), self._MIN_CHARS)
+            c = torch.empty((cap,), dtype=torch.uint8, device=dev)
+            if self._num_chars:
+                c[:self._num_chars].copy_(self._chars[:self._num_chars])
+            self._chars = c
+
+    def add(self, out, image_ids, original_sizes=None, num_classes=81):
+        """Append one detect() output (boxes [B,cap,4], scores, classes, counts and optionally masks [B,cap,M,M]) for the images
+        image_ids (one json id each, never added before).  original_sizes [B,2] (host): each image's RLE canvas, int() of each value as
+        in batch_results; required with masks.  num_classes: the model's, classes must lie in 1..num_classes-1."""
+        from .. import ops
+        if not isinstance(out, dict) or any(k not in out for k in ('boxes', 'scores', 'classes', 'counts')):
+            raise ValueError("add: expected detect()'s output dict with 'boxes', 'scores', 'classes' and 'counts'")
+        boxes, scores, classes, counts, masks = out['boxes'], out['scores'], out['classes'], out['counts'], out.get('masks')
+        tensors = [boxes, scores, classes, counts] + ([masks] if masks is not None else [])
+        if not all(torch.is_tensor(t) and t.device == self.device for t in tensors):
+            raise ValueError("add: detect() output must be tensors on %s" % self.device)
+        if boxes.dim() != 3 or boxes.size(2) != 4:
+            raise ValueError("add: boxes must be [B, cap, 4], got %s" % (tuple(boxes.shape),))
+        B, cap = int(boxes.size(0)), int(boxes.size(1))
+        if tuple(scores.shape) != (B, cap) or tuple(classes.shape) != (B, cap) or tuple(counts.shape) != (B,):
+            raise ValueError("add: scores / classes must be [%d, %d] and counts [%d]" % (B, cap, B))
+        if masks is not None and (masks.dim() != 4 or tuple(masks.shape[:2]) != (B, cap)):
+            raise ValueError("add: masks must be [%d, %d, M, M] (the detected class's mask)" % (B, cap))
+        num_classes = _int(num_classes, "num_classes")
+        if num_classes < 1:
+            raise ValueError("add: num_classes must be at least 1")
+        if isinstance(image_ids, (str, bytes)) or torch.is_tensor(image_ids):
+            raise ValueError("add: image_ids must be a sequence of integer json ids")
+        ids = [_int(v, "image id") for v in image_ids]
+        if len(ids) != B:
+            raise ValueError("add: %d image ids for %d images" % (len(ids), B))
+        if len(set(ids)) != B:
+            raise ValueError("add: an image id is repeated in this batch")
+        again = [v for v in ids if v in self._ordinal]
+        if again:
+            raise ValueError("add: image id %d was already added" % again[0])
+        if masks is not None and original_sizes is None:
+            raise ValueError("add: masks need original_sizes, each image's (height, width) RLE canvas")
+        sizes = ops.segm_image_sizes(original_sizes, B) if original_sizes is not None else np.zeros((B, 2), np.int64)
+        o0, n0 = len(self.image_ids), self._num_records
+        L = _lib.lib()
+        with torch.cuda.device(self.device):
+            offs_d, nch = None, 0
+            if masks is not None:
+                strings, host = ops.segm_rle_batch_device(masks, None, boxes, counts, sizes)
+                nch = int(host[0][-1])
+                self._reserve(n0 + B * cap, self._num_chars + nch)
+                if nch:
+                    self._chars[self._num_chars:self._num_chars + nch].copy_(strings[:nch])
+                offs_d = _pinned_upload(host[0].astype(np.int64), self.device)
+            else:
+                self._reserve(n0 + B * cap, 0)
+            table = np.concatenate([np.arange(o0, o0 + B, dtype=np.int64)[:, None], sizes.astype(np.int64)], 1)
+            img_d = _pinned_upload(table, self.device)
+            bx, sc = boxes.contiguous().float(), scores.contiguous().float()
+            cl, ct = classes.contiguous().to(torch.int32), counts.contiguous().to(torch.int32)
+            _lib.check(L.dt_coco_results_append(B, cap, num_classes, _p(bx), _p(sc), _p(cl), _p(ct), _p(img_d), _p(offs_d), self._num_chars,
+                                                _p(self._rec_f[n0:]), _p(self._rec_i[n0:]), _p(self._err), _stream(self.device)),
+                       "dt_coco_results_append")
+        for b, v in enumerate(ids):
+            self._ordinal[v] = o0 + b
+            self._where.append((b, num_classes))
+        self.image_ids += ids
+        self._num_records += B * cap
+        self._num_chars += nch
+        self._num_classes = max(self._num_classes, num_classes)
+        self._all_masks = self._all_masks and masks is not None
+
+
+def _flatten_device(gt, acc, iou_type, category_ids):
+    """_flatten_results + _pair_tables for a DeviceResults, on the device: -> dict of device tensors key [N], det_f [N, 5], det_i [N, 4]
+    (char offsets into acc's buffer `chars`), pairs [P, 7], cat_kept [K + 1], order_off [3, K + 1], and the sizes dt_coco_eval takes.
+    Host checks raise ValueError before anything is launched; the device's error flags come back with the sizes, in one copy."""
+    if acc.device != gt.device:
+        raise ValueError("the results are on %s, the ground truth on %s" % (acc.device, gt.device))
+    if iou_type == 'segm' and not acc._all_masks:
+        raise ValueError("segm evaluation of results without masks")
+    if len(set(category_ids)) != len(category_ids):
+        raise ValueError("category_ids must be distinct to evaluate a DeviceResults")
+    img_index = {v: n for n, v in enumerate(gt.img_ids)}
+    unknown = [v for v in acc.image_ids if v not in img_index]
+    if unknown:
+        raise ValueError("image id %d was added to the results but is not an image of the ground truth" % unknown[0])
+    ord_i = np.array([img_index[v] for v in acc.image_ids] or [0], np.int32)
+    cat_index = {v: n for n, v in enumerate(gt.cat_ids)}
+    nc = acc._num_classes
+    cls_k = np.full(nc, -1, np.int32)
+    for j in range(1, min(len(category_ids) + 1, nc)):        # classes past category_ids are dropped, as the host loop's break drops them
+        cls_k[j] = cat_index[category_ids[j - 1]]
+    I, K = gt.num_images, gt.num_cats
+    nb, n, dev = I * K, acc._num_records, gt.device
+    L = _lib.lib()
+    rec_f, rec_i = (acc._rec_f, acc._rec_i) if n else (None, None)
+    with torch.cuda.device(dev):
+        cls_d, ord_d = torch.from_numpy(cls_k).to(dev), torch.from_numpy(ord_i).to(dev)
+        nonfinite = torch.zeros((1,), dtype=torch.int32, device=dev)
+        cnt = torch.zeros((nb,), dtype=torch.int32, device=dev) if nb else None
+        vals = torch.empty((5, nb), dtype=torch.int64, device=dev) if nb else None
+        _lib.check(L.dt_coco_results_count(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(gt.keys_d), gt.num_gts, _p(cnt), _p(vals),
+                                           _p(nonfinite), _stream(dev)), "dt_coco_results_count")
+        scan = torch.cumsum(vals, 1) if nb else None
+        totals = scan[:, -1] if nb else torch.zeros((5,), dtype=torch.int64, device=dev)
+        tail = torch.cat([totals, acc._err.to(torch.int64), nonfinite.to(torch.int64)]).cpu().numpy()
+        if tail[5]:
+            b, ncls = acc._where[int(tail[6])]
+            raise RuntimeError("batch_results: the detections of image %d are not grouped by class in 1..%d" % (b, ncls - 1))
+        if tail[7]:
+            raise ValueError("non-finite box or score in the results")
+        N, P, c10, n_kept, n_iou = (int(v) for v in tail[:5])
+        key = torch.empty((max(N, 1),), dtype=torch.int64, device=dev)
+        det_f = torch.empty((max(N, 1), 5), dtype=torch.float64, device=dev)
+        det_i = torch.empty((max(N, 1), 4), dtype=torch.int64, device=dev)
+        pairs = torch.empty((max(P, 1), 7), dtype=torch.int64, device=dev)
+        cat_kept = torch.empty((K + 1,), dtype=torch.int64, device=dev)
+        order_off = torch.empty((3, K + 1), dtype=torch.int64, device=dev)
+        _lib.check(L.dt_coco_results_write(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(scan), _p(gt.keys_d), gt.num_gts, _p(key),
+                                           _p(det_f), _p(det_i), _p(pairs), _p(cat_kept), _p(order_off), _stream(dev)), "dt_coco_results_write")
+    chars = acc._chars if acc._chars is not None else torch.zeros((1,), dtype=torch.uint8, device=dev)
+    return dict(key=key[:N], det_f=det_f[:N], det_i=det_i[:N], pairs=pairs[:P], cat_kept=cat_kept, order_off=order_off, chars=chars,
+                num_chars=acc._num_chars, num_kept=n_kept, num_ious=n_iou, num_order=P + c10 + n_kept)
 
 
 # ------------------------------------------------------------------------------------------------------------ proposal recall

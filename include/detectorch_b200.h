@@ -285,7 +285,26 @@ int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_fact
  *                                 annotation order) at its first IoU; NULL keeps them in the workspace
  * dt_coco_det_check: bad [num_dets] uint8, 1 where a segm detection's string (det_i / det_chars as for dt_coco_eval) decodes to
  *   counts that do not sum to h * w.  rleIou never ends on such a mask, so dt_coco_eval must not be given one.
+ * dt_coco_results_append / _count / _write: detect() batches kept on the device as records (utils.coco_eval.DeviceResults) and
+ *   flattened into dt_coco_eval's tables.  Record: rec_f [n, 5] float x1, y1, x2, y2, score; rec_i [n, 7] int64 image ordinal (-1 for a
+ *   dead slot), class, rank inside its class in the image, char offset, char count, h, w.
+ *   append: boxes [B, cap, 4], scores [B, cap] float, classes [B, cap], counts [B] int; images [B, 3] int64 ordinal, h, w; str_offs
+ *   [B cap + 1] the batch's string offsets (NULL without masks) placed at char_base; writes B cap records; err int [2] (err[1] set to
+ *   INT_MAX by the caller): err[0] |= 1 and err[1] = min ordinal of an image with a live class outside 1..num_classes-1 or out of order.
+ *   count: cls_k [num_classes] category index of each class (-1: none), ord_i [ordinals] image index; bin_cnt int [K I] zeroed by the
+ *   caller; scan_in [5, K I] int64 gets D, D > 0, min(D, 10), min(D, 100), min(D, 100) G per (category, image) bin, to be scanned
+ *   (inclusive, along the bins) into write's scan; nonfinite (zeroed) |= 1 for a non-finite value in a counted record.
+ *   write: det_key [N] int64, det_f [N, 5], det_i [N, 4], pairs [num_active, 7], cat_kept [K+1], order_off [3, K+1] as dt_coco_eval takes them.
  * All return 0 on bad sizes or a NULL pointer. */
+int dt_coco_results_append(int batch, int cap, int num_classes, const float* boxes, const float* scores, const int* classes, const int* counts,
+                           const int64_t* images, const int64_t* str_offs, int64_t char_base, float* rec_f, int64_t* rec_i, int* err,
+                           dt_stream_t stream);
+int dt_coco_results_count(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k, const int* ord_i,
+                          int num_images, int num_cats, const int64_t* gt_keys, int64_t num_gts, int* bin_cnt, int64_t* scan_in, int* nonfinite,
+                          dt_stream_t stream);
+int dt_coco_results_write(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k, const int* ord_i,
+                          int num_images, int num_cats, const int64_t* scan, const int64_t* gt_keys, int64_t num_gts, int64_t* det_key, double* det_f,
+                          int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off, dt_stream_t stream);
 int dt_coco_det_check(int64_t num_dets, const int64_t* det_i, const char* det_chars, uint8_t* bad, dt_stream_t stream);
 int64_t dt_coco_gt_workspace_bytes(int64_t num_parts, int64_t num_points, int64_t num_upsampled);
 int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t* parts, const double* xy, const uint32_t* ucounts, const char* chars,
