@@ -492,6 +492,8 @@ void plan_buffers(Engine* e) {
     // Fast R-CNN on the FPN body: each image's pre-computed proposals in original-image coordinates, which the ST_COLLECT op scales,
     // deduplicates and maps to levels into rois / roi_levels / roi_counts (Engine.set_proposals).  Last, so no other offset moves.
     if (!f.c4 && !c.use_rpn) { add_buf(e, "fast_props", {B, post, 4}); add_buf(e, "fast_prop_counts", {B}, 1); }
+    // the reference's detection count per image, which exceeds det_counts when ties at the top-max_dets threshold overflow det_cap
+    add_buf(e, "det_total", {B}, 1);
 }
 
 // ---- program -----------------------------------------------------------------------------------
@@ -849,7 +851,7 @@ void setup_detect(Engine* e) {
     D.keep_flag = e->buf<unsigned char>("det_flag"); D.dec_box = e->buf<float4>("det_dec"); D.cls_counts = e->buf<int>("det_cls_counts");
     D.k0 = e->buf<uint32_t>("det_k0"); D.k1 = e->buf<uint32_t>("det_k1"); D.v0 = e->buf<int>("det_v0"); D.v1 = e->buf<int>("det_v1");
     D.out_boxes = e->buf("det_boxes"); D.out_scores = e->buf("det_scores"); D.out_classes = e->buf<int>("det_classes");
-    D.out_roi_idx = e->buf<int>("det_roi_idx"); D.out_counts = e->buf<int>("det_counts");
+    D.out_roi_idx = e->buf<int>("det_roi_idx"); D.out_counts = e->buf<int>("det_counts"); D.out_total = e->buf<int>("det_total");
 }
 
 // mask head (detector.py:99-112): RoIs from the detections, their 14x14 features, the FPN 4-conv tower or the C4 'upshare' head

@@ -708,7 +708,8 @@ struct DetParams {
     float* out_scores;          // [B, out_cap]
     int* out_classes;           // [B, out_cap]
     int* out_roi_idx;           // [B, out_cap]
-    int* out_counts;            // [B]
+    int* out_counts;            // [B] rows written, <= out_cap
+    int* out_total;             // [B] the reference's count: more than out_counts when ties at the limit overflow out_cap
 };
 
 // grid (NC-1, B), 256 threads; one CTA = one (image, foreground class).  R <= 1024.
@@ -781,9 +782,12 @@ static __global__ void __launch_bounds__(256) det_class_kernel(const __grid_cons
 // The kept flags of a class are swept by ONE WARP (ballot + popc over 32 RoIs at a time, no block barriers): class counts -> exclusive
 // class offsets -> ordered writes.  Two such sweeps (gather keys, emit) replace two block-wide scans of the NC*R flags (79 iterations x 3
 // __syncthreads each).  Order and arithmetic are unchanged: class-major, ascending RoI index.
+// The reference keeps every detection scoring >= the max_dets-th largest score, so ties at that score can make more than max_dets,
+// and more than out_cap.  Then every detection scoring above the threshold is written (there are fewer than max_dets <= out_cap of
+// them), the remaining rows take the tied ones in class-major, RoI-ascending order, and out_total holds the reference's count.
 static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_constant__ DetParams P) {
     __shared__ uint32_t hist[32 * 256];
-    __shared__ int cls_cnt[128], cls_off[129];
+    __shared__ int cls_cnt[128], cls_off[129], cls_tie[128];
     __shared__ float s_thresh;
     const int b = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
@@ -804,7 +808,7 @@ static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_con
         return cls_off[P.NC];
     };
     // sweep 1: kept per class
-    if (threadIdx.x < 128) cls_cnt[threadIdx.x] = 0;
+    if (threadIdx.x < 128) { cls_cnt[threadIdx.x] = 0; cls_tie[threadIdx.x] = 0; }
     __syncthreads();
     for (int j = 1 + warp; j < P.NC; j += nwarps) {
         int c = 0;
@@ -843,29 +847,54 @@ static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_con
         }
         __syncthreads();
         thresh = s_thresh;
-        // sweep 2: per class, how many of the kept pass score >= thresh (:162)
+        // sweep 2: per class, how many of the kept pass score >= thresh (:162), and how many of those tie at it
         __syncthreads();
         for (int j = 1 + warp; j < P.NC; j += nwarps) {
-            int c = 0;
+            int c = 0, t = 0;
     #pragma unroll 8
         for (int base = 0; base < P.R; base += 32) {
                 const int ri = base + lane;
-                const bool f = ri < P.R && flag[(size_t)j * P.R + ri] && P.cls[((size_t)b * P.R + ri) * P.NC + j] >= thresh;
-                c += __popc(__ballot_sync(0xffffffffu, f));
+                const bool f = ri < P.R && flag[(size_t)j * P.R + ri];
+                const float sc = f ? P.cls[((size_t)b * P.R + ri) * P.NC + j] : 0.f;
+                c += __popc(__ballot_sync(0xffffffffu, f && sc >= thresh));
+                t += __popc(__ballot_sync(0xffffffffu, f && sc == thresh));
             }
-            if (lane == 0) cls_cnt[j] = c;
+            if (lane == 0) { cls_cnt[j] = c; cls_tie[j] = t; }
         }
     }
-    const int nout = scan_classes();
+    int nout = scan_classes();
+    const int total = nout;
+    const bool cut_ties = nout > P.out_cap && thresh > -INFINITY;
+    if (cut_ties) {
+        // the ties overflow out_cap: all above-threshold detections, then cls_tie[j] becomes the number of class j's ties written
+        if (threadIdx.x == 0) {
+            int room = P.out_cap;
+            for (int j = 1; j < P.NC; ++j) room -= cls_cnt[j] - cls_tie[j];
+            for (int j = 1; j < P.NC; ++j) {
+                const int t = min(cls_tie[j], room);
+                room -= t;
+                cls_cnt[j] += t - cls_tie[j];
+                cls_tie[j] = t;
+            }
+        }
+        nout = scan_classes();
+    }
     // emit in class-major / RoI-ascending order
     for (int j = 1 + warp; j < P.NC; j += nwarps) {
-        int o = cls_off[j];
+        int o = cls_off[j], ties = 0;
+        const int tie_room = cls_tie[j];
 #pragma unroll 8
         for (int base = 0; base < P.R; base += 32) {
             const int ri = base + lane;
             bool f = ri < P.R && flag[(size_t)j * P.R + ri];
             float sc = 0.f;
             if (f) { sc = P.cls[((size_t)b * P.R + ri) * P.NC + j]; f = sc >= thresh; }
+            if (cut_ties) {
+                const bool tie = f && sc == thresh;
+                const unsigned mt = __ballot_sync(0xffffffffu, tie);
+                if (tie) f = ties + __popc(mt & lt) < tie_room;
+                ties += __popc(mt);
+            }
             const unsigned m = __ballot_sync(0xffffffffu, f);
             const int pos = o + __popc(m & lt);
             if (f && pos < P.out_cap) {
@@ -886,7 +915,7 @@ static __global__ void __launch_bounds__(1024) det_limit_kernel(const __grid_con
         P.out_classes[(size_t)b * P.out_cap + i] = 0;
         P.out_roi_idx[(size_t)b * P.out_cap + i] = -1;
     }
-    if (threadIdx.x == 0) P.out_counts[b] = min(nout, P.out_cap);
+    if (threadIdx.x == 0) { P.out_counts[b] = min(nout, P.out_cap); P.out_total[b] = total; }
 }
 
 // detections -> mask RoIs: boxes_final * scaling_factor, FPN level (eval_mask_FPN.ipynb cell 10; multilevel_rois.py:19-39).

@@ -117,14 +117,22 @@ def roi_align_backward_ref(top_diff, rois, features_shape, pooled_h, pooled_w, s
 
 
 # ----------------------------------------------------------------------------- NMS
-def nms(dets, thresh):
+def nms(dets, thresh, order="numpy"):
     """dets [N,5] fp32 (x1,y1,x2,y2,score) -> ascending original indices kept (int64).
-    boxes.py:332-336: empty input returns []."""
+    boxes.py:332-336: empty input returns [].
+    order: the visiting order of tied scores.  "numpy" is the reference's own (pyx:45, numpy's unstable argsort reversed, which
+    may differ between hosts and numpy builds); "stable" is (score desc, index asc), the order the device kernels document."""
     dets = np.ascontiguousarray(np.asarray(dets, dtype=np.float32))
     n = dets.shape[0]
     if n == 0:
         return np.zeros((0,), np.int64)
-    order = np.ascontiguousarray(dets[:, 4].argsort()[::-1].astype(np.int64))   # pyx:45
+    if order == "numpy":
+        order = dets[:, 4].argsort()[::-1]                                       # pyx:45
+    elif order == "stable":
+        order = np.argsort(-dets[:, 4], kind="stable")
+    else:
+        raise ValueError("nms: order must be 'numpy' or 'stable'")
+    order = np.ascontiguousarray(order.astype(np.int64))
     keep = np.empty((n,), np.int64)
     k = lib().oracle_nms(_fp(dets), _fp(order), ctypes.c_int64(n), ctypes.c_float(thresh), _fp(keep))
     return keep[:k].copy()
@@ -305,15 +313,18 @@ def clip_tiled_boxes(boxes, im_shape):
     return boxes
 
 
-def box_results_with_nms_and_limit(scores, boxes, num_classes=81, score_thresh=0.05, overlap_thresh=0.5,
-                                   max_detections_per_img=100):
-    """result_utils.py:96-168 (hard-NMS branch; soft-NMS / voting are off by default)."""
+def _nms_and_limit(scores, boxes, num_classes, score_thresh, overlap_thresh, max_detections_per_img, tie_order):
+    """result_utils.py:96-168 keeping track of the rows: (cls_boxes, cls_inds) with cls_inds[j] the RoI index of each row of
+    cls_boxes[j], and the image threshold of the limit (None when it did not cut)."""
     cls_boxes = [[] for _ in range(num_classes)]
+    cls_inds = [np.zeros((0,), np.int64) for _ in range(num_classes)]
     for j in range(1, num_classes):
         inds = np.where(scores[:, j] > score_thresh)[0]
         dets_j = np.hstack((boxes[inds, j * 4:(j + 1) * 4], scores[inds, j][:, None])).astype(np.float32, copy=False)
-        keep = nms(dets_j, overlap_thresh)
+        keep = nms(dets_j, overlap_thresh, order=tie_order)
         cls_boxes[j] = dets_j[keep, :]
+        cls_inds[j] = inds[keep]
+    image_thresh = None
     if max_detections_per_img > 0:
         image_scores = np.hstack([cls_boxes[j][:, -1] for j in range(1, num_classes)])
         if len(image_scores) > max_detections_per_img:
@@ -321,8 +332,56 @@ def box_results_with_nms_and_limit(scores, boxes, num_classes=81, score_thresh=0
             for j in range(1, num_classes):
                 k = np.where(cls_boxes[j][:, -1] >= image_thresh)[0]
                 cls_boxes[j] = cls_boxes[j][k, :]
+                cls_inds[j] = cls_inds[j][k]
+    return cls_boxes, cls_inds, image_thresh
+
+
+def box_results_with_nms_and_limit(scores, boxes, num_classes=81, score_thresh=0.05, overlap_thresh=0.5,
+                                   max_detections_per_img=100, tie_order="numpy"):
+    """result_utils.py:96-168 (hard-NMS branch; soft-NMS / voting are off by default).  tie_order: the NMS visiting order of tied
+    scores (nms's `order`); the limit itself does not depend on it."""
+    cls_boxes = _nms_and_limit(scores, boxes, num_classes, score_thresh, overlap_thresh, max_detections_per_img, tie_order)[0]
     im_results = np.vstack([cls_boxes[j] for j in range(1, num_classes)])
     return im_results[:, -1], im_results[:, :-1], cls_boxes
+
+
+def detection_tail(case, b, tie_order="numpy", max_dets=100):
+    """postprocess_output + box_results_with_nms_and_limit on image b of a teacher-forced detection case (the fields of
+    tests/detect_tail_cases.Case: rois [B,R,5] at network scale, roi_counts [B], cls_prob [B*R,NC], bbox_pred [B*R,4NC], scale [B],
+    orig_hw [B,2]).  Returns (classes, roi_idx, scores, boxes, image_thresh) in the reference's class-major, RoI-ascending order."""
+    R, NC = case.rois.shape[1], case.cls_prob.shape[1]
+    n = int(case.roi_counts[b])
+    rois = case.rois[b, :n, 1:5].astype(np.float32)
+    boxes = (rois / np.float32(case.scale[b])).astype(np.float32)                 # rois.div(scaling_factor) in fp32
+    deltas = case.bbox_pred[b * R:b * R + n].astype(np.float32)
+    im = np.asarray(case.orig_hw[b], np.float32)
+    pred = clip_tiled_boxes(bbox_transform(boxes, deltas, (10.0, 10.0, 5.0, 5.0)), im)
+    sc = case.cls_prob[b * R:b * R + n].astype(np.float32)
+    cls_boxes, cls_inds, thresh = _nms_and_limit(sc, pred, NC, 0.05, 0.5, max_dets, tie_order)
+    cls = np.concatenate([np.full(len(cls_inds[j]), j, np.int64) for j in range(1, NC)])
+    dets = np.vstack([np.asarray(cls_boxes[j], np.float32).reshape(-1, 5) for j in range(1, NC)])
+    return cls, np.concatenate(cls_inds[1:]), dets[:, 4], dets[:, :4], thresh
+
+
+def expected_device(case, det_cap, max_dets=100, tie_order="stable"):
+    """What the device detection tail writes for each image of `case` with det_cap output rows: the reference's detections with
+    stable tie order (detection_tail(..., "stable")) and, when more than det_cap of them tie through the limit, the surplus
+    removed from the end of those tied at the image threshold (class-major, RoI-ascending order).  Every detection scoring above
+    the threshold is kept: there are fewer than max_dets <= det_cap of them.  Per image (classes, roi_idx, scores, boxes, total)
+    with total the reference's own count."""
+    out = []
+    for b in range(case.rois.shape[0]):
+        cls, idx, sc, bx, thresh = detection_tail(case, b, tie_order, max_dets)
+        total = len(sc)
+        if total > det_cap:
+            assert thresh is not None, "more detections than det_cap without the limit"
+            tied = np.flatnonzero(sc == thresh)
+            drop = tied[len(tied) - (total - det_cap):]
+            assert len(drop) == total - det_cap, "the surplus is not all tied at the image threshold"
+            keep = np.setdiff1d(np.arange(total), drop)
+            cls, idx, sc, bx = cls[keep], idx[keep], sc[keep], bx[keep]
+        out.append((cls, idx, sc, bx, total))
+    return out
 
 
 def postprocess_output(rois, scaling_factor, im_size, class_scores, bbox_deltas, bbox_reg_weights=(10.0, 10.0, 5.0, 5.0)):
