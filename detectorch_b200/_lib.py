@@ -34,6 +34,8 @@ SIGNATURES = {
     "dt_segm_batch_strings_bytes": (c_int64, [c_int, c_int, c_int]),
     "dt_segm_rle_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_segm_rle_batch_append": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int,
+                                         c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_segm_paste": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                               c_void_p, c_void_p]),
     "dt_roi_align_backward_det_workspace_bytes": (c_int64, [c_int64, c_int64]),

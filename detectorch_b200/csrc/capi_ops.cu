@@ -563,6 +563,54 @@ extern "C" int dt_segm_rle_batch(const float* masks, const int* classes, int num
                            (cudaStream_t)stream);
 }
 
+// dt_segm_rle_batch without a host-known size or a host read: bounded tables, flags, and the strings appended to an arena at a device
+// cursor.  Only stream operations are issued, so the call can be captured into a CUDA graph.
+static_assert(kSegmMaxSide == DT_SEGM_APPEND_MAX_SIDE, "the header states the table bound of segm_rle_bounded_kernel");
+extern "C" int dt_segm_rle_batch_append(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes,
+                                        const int* num_dets_dev, const int* im_sizes, int batch, int cap, float thresh_binarize, int runs_cap,
+                                        uint8_t* arena, int64_t arena_capacity, int64_t* cursor, int64_t* str_offsets, int* flags,
+                                        void* workspace, dt_stream_t stream) {
+    if (batch < 0 || cap < 0 || arena_capacity < 0) { fprintf(stderr, "dt_segm_rle_batch_append: bad sizes\n"); return 0; }
+    if (batch == 0 || cap == 0) return 1;
+    if (!masks || !boxes || !num_dets_dev || !im_sizes || !cursor || !str_offsets || !flags || !workspace || (arena_capacity > 0 && !arena)) {
+        fprintf(stderr, "dt_segm_rle_batch_append: null argument\n");
+        return 0;
+    }
+    const size_t smem = segm_smem_bytes(mask_size, kSegmMaxSide, kSegmMaxSide);
+    if (mask_size < 1 || smem > 200 * 1024 || (classes && num_mask_classes < 1) || runs_cap < 2 || batch > 65535 ||
+        (int64_t)batch * cap >= (1ll << 31)) {
+        fprintf(stderr, "dt_segm_rle_batch_append: unsupported size (mask %d, %d classes, runs_cap %d, %d x %d slots)\n", mask_size,
+                num_mask_classes, runs_cap, batch, cap);
+        return 0;
+    }
+    static bool smem_set = false;
+    if (!smem_set) {
+        DT_CHECK_CUDA(cudaFuncSetAttribute(segm_rle_bounded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        smem_set = true;
+    }
+    const int64_t D = (int64_t)batch * cap;
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
+    uint8_t* staging = ws + D * runs_cap * 4;
+    int* str_len = reinterpret_cast<int*>(staging + ((D * runs_cap * kSegmCharsPerRun + 15) / 16 * 16));
+    uint8_t* scratch = ws + segm_ws_bytes(D, runs_cap);
+    uint32_t* counts = reinterpret_cast<uint32_t*>(scratch);
+    int* num_counts = reinterpret_cast<int*>(scratch + D * runs_cap * 4);
+    cudaStream_t st = (cudaStream_t)stream;
+    DT_CHECK_CUDA(cudaMemsetAsync(flags, 0, 3 * sizeof(int), st));
+    segm_rle_bounded_kernel<<<dim3(cap, batch), 256, smem, st>>>(masks, classes, classes ? num_mask_classes : 1, mask_size, boxes, num_dets_dev,
+                                                                 im_sizes, thresh_binarize, positions, counts, num_counts, runs_cap, staging,
+                                                                 str_len, runs_cap * kSegmCharsPerRun, flags);
+    DT_CHECK_CUDA(cudaGetLastError());
+    long long* offsets = reinterpret_cast<long long*>(str_offsets);
+    segm_arena_offsets_kernel<<<1, 1024, 0, st>>>(str_len, (int)D, reinterpret_cast<long long*>(cursor), arena_capacity, flags, offsets);
+    DT_CHECK_CUDA(cudaGetLastError());
+    segm_arena_compact_kernel<<<(unsigned)((D + 7) / 8), 256, 0, st>>>(staging, str_len, (int)D, runs_cap * kSegmCharsPerRun, offsets, flags,
+                                                                      arena);
+    DT_CHECK_CUDA(cudaGetLastError());
+    return 1;
+}
+
 extern "C" int dt_segm_paste(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,
                              const int* expanded_boxes, const int* num_dets_dev, int max_dets, int im_h, int im_w, float thresh_binarize,
                              uint8_t* out, dt_stream_t stream) {

@@ -129,20 +129,21 @@ __device__ __forceinline__ T block_scan_value(T v, T* scratch, T* total) {
 
 struct SegmRowCoef { int s; float w0, w1; int pad; };
 
+// Image side the tables of segm_rle_bounded_kernel are sized for (dt_segm_rle_batch_append; include/detectorch_b200.h).
+constexpr int kSegmMaxSide = 8192;
+
 // Grid (cap, B): block (d, b) is detection slot d of image b, i.e. slot s = b * cap + d of the flat per-slot arrays.
 // masks: [B*cap, K, M, M] (class-specific: K classes, cls[s] selects) or [B*cap, M, M] (K == 1 / cls == NULL)
 // im_sizes: int32 [B, 2] (im_h, im_w) of each image's canvas, or NULL (every image is max_h x max_w).  The shared row / column tables
 // are sized for max_h x max_w; an image whose size is not within [1, max] produces empty results.
 // num_dets_dev: int32 [B] live slots per image (NULL: all); slots at or past the count produce empty results
 // outputs per slot s: counts[s*runs_cap ..] (uint32 run lengths), num_counts[s], strings (cap str_cap per slot), str_len[s]
-static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
-                                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
-                                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
-                                                              int max_h, int max_w, float thresh,
-                                                              uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
-                                                              int* __restrict__ num_counts, int runs_cap,
-                                                              uint8_t* __restrict__ strings, int* __restrict__ str_len, int str_cap,
-                                                              int* __restrict__ overflow) {
+__device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
+                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
+                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes, int max_h, int max_w,
+                                              float thresh, uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
+                                              int* __restrict__ num_counts, int runs_cap, uint8_t* __restrict__ strings,
+                                              int* __restrict__ str_len, int str_cap, int* __restrict__ overflow) {
     extern __shared__ __align__(16) uint8_t segm_smem[];
     const int b = blockIdx.y, det = blockIdx.x;
     const size_t d = (size_t)b * gridDim.x + det;
@@ -281,6 +282,36 @@ static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __res
     if (threadIdx.x == 0) { num_counts[d] = m; str_len[d] = total_chars; }
 }
 
+static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
+                                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
+                                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
+                                                              int max_h, int max_w, float thresh,
+                                                              uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
+                                                              int* __restrict__ num_counts, int runs_cap,
+                                                              uint8_t* __restrict__ strings, int* __restrict__ str_len, int str_cap,
+                                                              int* __restrict__ overflow) {
+    segm_rle_slot(masks, cls, K, M, ref_boxes, exp_boxes, num_dets_dev, im_sizes, max_h, max_w, thresh, positions, counts, num_counts, runs_cap,
+                  strings, str_len, str_cap, overflow);
+}
+
+// segm_rle_kernel with tables for kSegmMaxSide x kSegmMaxSide whatever the batch holds, so that one launch (one captured graph node)
+// serves any im_sizes table.  flags[0] gets the overflow (atomicMax of the runs a slot needed); an image whose size is outside
+// [1, kSegmMaxSide] sets flags[1] (its slots are still emptied, and the batch is not committed by segm_arena_offsets_kernel).
+static __global__ void __launch_bounds__(256) segm_rle_bounded_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K,
+                                                                      int M, const float* __restrict__ boxes,
+                                                                      const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
+                                                                      float thresh, uint32_t* __restrict__ positions,
+                                                                      uint32_t* __restrict__ counts, int* __restrict__ num_counts,
+                                                                      int runs_cap, uint8_t* __restrict__ strings, int* __restrict__ str_len,
+                                                                      int str_cap, int* __restrict__ flags) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        const int h = im_sizes[2 * blockIdx.y], w = im_sizes[2 * blockIdx.y + 1];
+        if (h < 1 || w < 1 || h > kSegmMaxSide || w > kSegmMaxSide) atomicOr(flags + 1, 1);
+    }
+    segm_rle_slot(masks, cls, K, M, boxes, nullptr, num_dets_dev, im_sizes, kSegmMaxSide, kSegmMaxSide, thresh, positions, counts, num_counts,
+                  runs_cap, strings, str_len, str_cap, flags);
+}
+
 // offsets[0..D] = exclusive scan of str_len[0..D) (offsets[D] = total), one block: each thread sums a contiguous chunk, a block scan
 // of the chunk sums gives each chunk's start
 static __global__ void __launch_bounds__(1024) segm_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ offsets) {
@@ -302,6 +333,42 @@ static __global__ void __launch_bounds__(256) segm_compact_kernel(const uint8_t*
     if (d >= D) return;
     const int n = str_len[d];
     uint8_t* dst = packed + offsets[d];
+    const uint8_t* src = strings + (size_t)d * str_cap;
+    for (int i = lane; i < n; i += 32) dst[i] = src[i];
+}
+
+// segm_offsets_kernel for a batch appended to a char arena at a device-side cursor: offsets[s] = *cursor + the scan (offsets[D] =
+// *cursor + total).  The batch is committed, *cursor advanced by the total, only if no slot overflowed (flags[0]), every image was
+// within the tables (flags[1]) and cursor + total <= capacity; a batch that does not fit sets flags[2] and leaves the cursor.
+static __global__ void __launch_bounds__(1024) segm_arena_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ cursor,
+                                                                         long long capacity, int* __restrict__ flags,
+                                                                         long long* __restrict__ offsets) {
+    __shared__ long long scratch[33];
+    const long long base = *cursor;                 // read by every thread before the scan's barriers, written after them
+    const int chunk = (D + blockDim.x - 1) / blockDim.x;
+    const int lo = min((int)threadIdx.x * chunk, D), hi = min(lo + chunk, D);
+    long long sum = 0;
+    for (int i = lo; i < hi; ++i) sum += str_len[i];
+    long long total;
+    long long run = base + block_scan_value(sum, scratch, &total);
+    for (int i = lo; i < hi; ++i) { offsets[i] = run; run += str_len[i]; }
+    if (threadIdx.x == 0) {
+        offsets[D] = base + total;
+        if (flags[0] == 0 && flags[1] == 0) {
+            if (base + total <= capacity) *cursor = base + total;
+            else flags[2] = 1;
+        }
+    }
+}
+
+// segm_compact_kernel into the arena, for a committed batch only (no flag of segm_arena_offsets_kernel raised)
+static __global__ void __launch_bounds__(256) segm_arena_compact_kernel(const uint8_t* __restrict__ strings, const int* __restrict__ str_len,
+                                                                        int D, int str_cap, const long long* __restrict__ offsets,
+                                                                        const int* __restrict__ flags, uint8_t* __restrict__ arena) {
+    const int d = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (d >= D || flags[0] || flags[1] || flags[2]) return;
+    const int n = str_len[d];
+    uint8_t* dst = arena + offsets[d];
     const uint8_t* src = strings + (size_t)d * str_cap;
     for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }

@@ -247,6 +247,46 @@ def segm_rle_batch_device(masks, classes, boxes, num_dets, im_sizes, thresh=0.5,
         runs_cap = max(2 * runs_cap, need + 1)     # a detection needed more runs than provisioned: grow and redo
 
 
+SEGM_APPEND_MAX_SIDE = 8192     # DT_SEGM_APPEND_MAX_SIDE: the largest image side segm_rle_batch_append encodes
+
+
+def segm_rle_batch_append(masks, classes, boxes, num_dets, im_sizes, arena, cursor, thresh=0.5, runs_cap=4096):
+    """segm_rle_batch's strings appended to a device char arena, without reading anything back (capturable in a CUDA graph).
+    masks, classes, boxes, num_dets: as for segm_rle_batch; im_sizes int32 [B,2] on the device; arena uint8 [capacity] (or None for
+    capacity 0); cursor int64 [1] on the device, the arena's used length.  -> (offsets int64 [B*cap+1] into the arena, flags int32 [3]),
+    both on the device: flags [0] the runs a slot needed beyond runs_cap, [1] an image size outside [1, SEGM_APPEND_MAX_SIDE], [2] the
+    strings did not fit (cursor + offsets[-1] - offsets[0] > capacity).  With a flag raised, the arena and the cursor are untouched."""
+    _need_cuda(masks, classes, boxes, num_dets, im_sizes, arena, cursor)
+    if masks.dim() not in (4, 5) or boxes.dim() != 3 or boxes.size(2) != 4:
+        raise ValueError("segm_rle_batch_append: masks must be [B,cap,M,M] or [B,cap,K,M,M] and boxes [B,cap,4]")
+    B, cap, M = masks.size(0), masks.size(1), masks.size(-1)
+    if tuple(boxes.shape[:2]) != (B, cap) or masks.size(-2) != M:
+        raise ValueError("segm_rle_batch_append: masks %s and boxes %s disagree" % (tuple(masks.shape), tuple(boxes.shape)))
+    if (masks.dim() == 5) != (classes is not None) or (classes is not None and tuple(classes.shape) != (B, cap)):
+        raise ValueError("segm_rle_batch_append: [B,cap,K,M,M] masks need classes [B,cap]; [B,cap,M,M] masks take none")
+    if tuple(im_sizes.shape) != (B, 2) or im_sizes.dtype != torch.int32 or cursor.dtype != torch.int64 or cursor.numel() != 1:
+        raise ValueError("segm_rle_batch_append: im_sizes must be int32 [%d, 2] and cursor int64 [1]" % B)
+    if arena is not None and (arena.dtype != torch.uint8 or arena.dim() != 1 or not arena.is_contiguous()):
+        raise ValueError("segm_rle_batch_append: the arena must be a contiguous uint8 vector")
+    K = masks.size(2) if masks.dim() == 5 else 1
+    dev = masks.device
+    masks, boxes, im_sizes = masks.contiguous().float(), boxes.contiguous().float(), im_sizes.contiguous()
+    if classes is not None:
+        classes = classes.contiguous().to(torch.int32)
+    nd = torch.full((B,), cap, dtype=torch.int32, device=dev) if num_dets is None else num_dets.contiguous().to(torch.int32)
+    offs = torch.empty((B * cap + 1,), dtype=torch.int64, device=dev)
+    flags = torch.zeros((3,), dtype=torch.int32, device=dev)
+    if B * cap == 0:
+        offs.copy_(cursor.reshape(1))
+        return offs, flags
+    L = _lib.lib()
+    ws = torch.empty((L.dt_segm_batch_workspace_bytes(B, cap, runs_cap),), dtype=torch.uint8, device=dev)
+    _lib.check(L.dt_segm_rle_batch_append(_p(masks), _p(classes), K, M, _p(boxes), _p(nd), _p(im_sizes), B, cap, float(thresh), int(runs_cap),
+                                          _p(arena), 0 if arena is None else arena.numel(), _p(cursor), _p(offs), _p(flags), _p(ws), _stream()),
+               "dt_segm_rle_batch_append")
+    return offs, flags
+
+
 def segm_rle_batch(masks, classes, boxes, num_dets, im_sizes, thresh=0.5, runs_cap=4096):
     """Mask paste + COCO RLE of a batch of images on the device (lib/utils/result_utils.py:170-228 for every image at once).
     masks [B,cap,M,M] (the selected class, detect()'s 'masks') or [B,cap,K,M,M] with classes int32 [B,cap] selecting the plane;

@@ -10,6 +10,7 @@ file that lib/utils/json_dataset_evaluator.py would write; no file is written.
 The host only checks and flattens the annotations and results into arrays (csrc/coco_eval.cuh documents their layout); everything
 numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before the evaluation is
 launched (segm results' run sums are checked by a small kernel first)."""
+import collections
 import json
 import math
 
@@ -601,6 +602,15 @@ def _pinned_upload(a, dev):
     return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
 
 
+class _Pending:
+    """One masked add (or its redo) whose outcome the host has not read yet: the batch's own copies of its inputs, the records it
+    wrote, and the status the device copies to pinned memory, [runs needed, size flag, arena full, cursor after, chars needed]."""
+
+    def __init__(self, inputs, n0, num_classes):
+        self.inputs, self.n0, self.num_classes = inputs, n0, num_classes
+        self.runs_cap = self.capacity = self.status = self.event = None
+
+
 class DeviceResults:
     """detect() outputs accumulated on the device, for evaluate(gt, acc, 'bbox' | 'segm') without bringing any detection to the host:
 
@@ -611,14 +621,21 @@ class DeviceResults:
         E = evaluate(gt, acc, 'segm')
 
     The evaluation equals evaluate(gt, per_image_results, ...) where image i holds what batch_results returned for it (images never
-    added have no detections).  add() only enqueues work on the current stream: detect()'s buffers may be overwritten by the next call
-    straight away.  Without masks it does not synchronise the host; with masks it pastes and encodes them as batch_results does (one
-    synchronisation) and keeps the strings in a device char buffer.  Each add keeps B * cap records of 76 bytes (+ the strings).
-    evaluate() takes K * I bins (K categories, I images of the ground truth) of 84 bytes each: an int32 counter and 5 int64 values with
-    their scans, 34 MB for 80 x 5000.  Device-side problems (classes not grouped or out of range, non-finite values) are raised by
-    evaluate().  The category ids given to evaluate() must be distinct, so that each (category, image) bin holds one class's slots."""
+    added have no detections).  add() only enqueues work on the current stream and does not synchronise the host: detect()'s buffers
+    may be overwritten by the next call straight away.  With masks it pastes and encodes them as batch_results does, appending the
+    strings to a device char arena at a device-side cursor (ops.segm_rle_batch_append).  Whether a batch's run lengths or strings
+    overflowed is learnt later: each masked batch keeps a copy of its inputs (masks, boxes, scores, classes, counts, sizes: 2.5 MB for
+    8 x 100 slots of 28 x 28) in a ring of _RING batches until its status, copied to pinned memory, has arrived.  A later add() reads
+    the statuses that have (event query, no wait); an overflowed batch is redone with the grown buffer and its records rewritten, in
+    stream order.  Only an add() that finds the ring full waits, for its oldest batch; evaluate() waits for all of them.
+    Each add keeps B * cap records of 76 bytes (+ the strings).  evaluate() takes K * I bins (K categories, I images of the ground truth)
+    of 84 bytes each: an int32 counter and 5 int64 values with their scans, 34 MB for 80 x 5000.  Device-side problems (classes not
+    grouped or out of range, non-finite values) are raised by evaluate().  The category ids given to evaluate() must be distinct, so
+    that each (category, image) bin holds one class's slots."""
     _MIN_RECORDS = 1 << 12          # initial capacities; both buffers then grow geometrically
     _MIN_CHARS = 1 << 20
+    _RING = 4                       # masked batches whose status may be outstanding before add() waits for the oldest
+    _RUNS_CAP = 4096                # initial run-length capacity per slot; grows when a slot needs more
 
     def __init__(self, device=None):
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
@@ -628,17 +645,27 @@ class DeviceResults:
         self.image_ids = []                 # json id of each image ordinal, in the order added
         self._ordinal = {}
         self._where = []                    # per ordinal: (position in its detect() batch, num_classes of its add)
-        self._num_records = self._num_chars = 0
+        self._num_records = 0
+        self._chars_used = 0                # the arena cursor as of the last status read
         self._num_classes = 1
         self._all_masks = True
         self._rec_f = self._rec_i = self._chars = None
+        self._runs_cap = self._RUNS_CAP
+        self._ring = collections.deque()
         with torch.cuda.device(self.device):
             self._err = _pinned_upload(np.array([0, _INT32_MAX], np.int32), self.device)
+            self._cursor = torch.zeros((1,), dtype=torch.int64, device=self.device)
 
     def __len__(self):
         return len(self.image_ids)
 
-    def _reserve(self, records, chars):
+    @property
+    def _num_chars(self):
+        """Bytes of the char arena in use: exact, as it waits for every outstanding masked batch."""
+        self._drain()
+        return self._chars_used
+
+    def _reserve(self, records):
         dev, n = self.device, self._num_records
         if self._rec_f is None or records > self._rec_f.shape[0]:
             cap = max(records, 2 * (0 if self._rec_f is None else self._rec_f.shape[0]), self._MIN_RECORDS)
@@ -647,17 +674,64 @@ class DeviceResults:
             if n:
                 f[:n].copy_(self._rec_f[:n]); i[:n].copy_(self._rec_i[:n])
             self._rec_f, self._rec_i = f, i
-        if chars and (self._chars is None or chars > self._chars.shape[0]):
-            cap = max(chars, 2 * (0 if self._chars is None else self._chars.shape[0]), self._MIN_CHARS)
-            c = torch.empty((cap,), dtype=torch.uint8, device=dev)
-            if self._num_chars:
-                c[:self._num_chars].copy_(self._chars[:self._num_chars])
-            self._chars = c
+
+    def _launch(self, p):
+        """Paste + RLE of a retained batch appended at the device cursor, its records (re)written with the arena offsets, and its
+        status sent to pinned memory; nothing is waited for."""
+        masks, boxes, scores, classes, counts, sizes, img_d = p.inputs
+        B, cap = int(boxes.size(0)), int(boxes.size(1))
+        L = _lib.lib()
+        from .. import ops
+        p.runs_cap, p.capacity = self._runs_cap, self._chars.shape[0]
+        offs, flags = ops.segm_rle_batch_append(masks, None, boxes, counts, sizes, self._chars, self._cursor, runs_cap=p.runs_cap)
+        _lib.check(L.dt_coco_results_append(B, cap, p.num_classes, _p(boxes), _p(scores), _p(classes), _p(counts), _p(img_d), _p(offs), 0,
+                                            _p(self._rec_f[p.n0:]), _p(self._rec_i[p.n0:]), _p(self._err), _stream(self.device)),
+                   "dt_coco_results_append")
+        status = torch.cat([flags.to(torch.int64), self._cursor, offs[-1:] - offs[:1]])
+        p.status = torch.empty((5,), dtype=torch.int64, pin_memory=True)
+        p.status.copy_(status, non_blocking=True)
+        p.event = torch.cuda.Event()
+        p.event.record()
+        self._ring.append(p)
+
+    def _settle(self, p):
+        """A masked batch whose status has arrived: done if no flag is raised, else the overflowed capacity grows and the batch is
+        redone (in stream order, after everything enqueued so far)."""
+        runs, size, full, cursor, need = p.status.tolist()
+        self._chars_used = cursor
+        if not (runs or size or full):
+            return
+        if size:
+            raise RuntimeError("DeviceResults: an image size beyond the mask encoder's tables reached the device")
+        with torch.cuda.device(self.device):
+            if runs:
+                self._runs_cap = max(self._runs_cap, 2 * p.runs_cap, runs + 1)
+            if full and self._chars.shape[0] == p.capacity:
+                # the batches enqueued since wrote below the old capacity, so the redo finds the cursor there at most; a batch that
+                # failed before an earlier growth is redone first, and grows the arena only if it fails again
+                old = self._chars.shape[0]
+                c = torch.empty((max(2 * old, old + need, self._MIN_CHARS),), dtype=torch.uint8, device=self.device)
+                c[:old].copy_(self._chars)
+                self._chars = c
+            self._launch(p)
+
+    def _poll(self):
+        """Settles the masked batches whose status has arrived, oldest first, without waiting."""
+        while self._ring and self._ring[0].event.query():
+            self._settle(self._ring.popleft())
+
+    def _drain(self, keep=0):
+        """Waits for the oldest masked batches until at most `keep` are outstanding (redoing any that overflowed)."""
+        while len(self._ring) > keep:
+            p = self._ring.popleft()
+            p.event.synchronize()
+            self._settle(p)
 
     def add(self, out, image_ids, original_sizes=None, num_classes=81):
         """Append one detect() output (boxes [B,cap,4], scores, classes, counts and optionally masks [B,cap,M,M]) for the images
         image_ids (one json id each, never added before).  original_sizes [B,2] (host): each image's RLE canvas, int() of each value as
-        in batch_results; required with masks.  num_classes: the model's, classes must lie in 1..num_classes-1."""
+        in batch_results; required with masks, and at most ops.SEGM_APPEND_MAX_SIDE on either side.  num_classes: the model's, classes
+        must lie in 1..num_classes-1."""
         from .. import ops
         if not isinstance(out, dict) or any(k not in out for k in ('boxes', 'scores', 'classes', 'counts')):
             raise ValueError("add: expected detect()'s output dict with 'boxes', 'scores', 'classes' and 'counts'")
@@ -688,32 +762,35 @@ class DeviceResults:
         if masks is not None and original_sizes is None:
             raise ValueError("add: masks need original_sizes, each image's (height, width) RLE canvas")
         sizes = ops.segm_image_sizes(original_sizes, B) if original_sizes is not None else np.zeros((B, 2), np.int64)
+        if masks is not None and B and sizes.max() > ops.SEGM_APPEND_MAX_SIDE:
+            raise ValueError("add: an image of %d x %d is beyond the %d x %d the masks are encoded for" %
+                             (tuple(sizes[int(np.argmax(sizes.max(1)))]) + (ops.SEGM_APPEND_MAX_SIDE,) * 2))
         o0, n0 = len(self.image_ids), self._num_records
         L = _lib.lib()
         with torch.cuda.device(self.device):
-            offs_d, nch = None, 0
-            if masks is not None:
-                strings, host = ops.segm_rle_batch_device(masks, None, boxes, counts, sizes)
-                nch = int(host[0][-1])
-                self._reserve(n0 + B * cap, self._num_chars + nch)
-                if nch:
-                    self._chars[self._num_chars:self._num_chars + nch].copy_(strings[:nch])
-                offs_d = _pinned_upload(host[0].astype(np.int64), self.device)
-            else:
-                self._reserve(n0 + B * cap, 0)
+            self._poll()
+            self._reserve(n0 + B * cap)
             table = np.concatenate([np.arange(o0, o0 + B, dtype=np.int64)[:, None], sizes.astype(np.int64)], 1)
             img_d = _pinned_upload(table, self.device)
-            bx, sc = boxes.contiguous().float(), scores.contiguous().float()
-            cl, ct = classes.contiguous().to(torch.int32), counts.contiguous().to(torch.int32)
-            _lib.check(L.dt_coco_results_append(B, cap, num_classes, _p(bx), _p(sc), _p(cl), _p(ct), _p(img_d), _p(offs_d), self._num_chars,
-                                                _p(self._rec_f[n0:]), _p(self._rec_i[n0:]), _p(self._err), _stream(self.device)),
-                       "dt_coco_results_append")
+            if masks is not None:
+                self._drain(keep=self._RING - 1)
+                if self._chars is None:
+                    self._chars = torch.empty((max(self._MIN_CHARS, 1),), dtype=torch.uint8, device=self.device)
+                own = lambda t, dt: t.to(dtype=dt, memory_format=torch.contiguous_format, copy=True)
+                p = _Pending((own(masks, torch.float32), own(boxes, torch.float32), own(scores, torch.float32), own(classes, torch.int32),
+                              own(counts, torch.int32), img_d[:, 1:].to(torch.int32).contiguous(), img_d), n0, num_classes)
+                self._launch(p)
+            else:
+                bx, sc = boxes.contiguous().float(), scores.contiguous().float()
+                cl, ct = classes.contiguous().to(torch.int32), counts.contiguous().to(torch.int32)
+                _lib.check(L.dt_coco_results_append(B, cap, num_classes, _p(bx), _p(sc), _p(cl), _p(ct), _p(img_d), _p(None), 0,
+                                                    _p(self._rec_f[n0:]), _p(self._rec_i[n0:]), _p(self._err), _stream(self.device)),
+                           "dt_coco_results_append")
         for b, v in enumerate(ids):
             self._ordinal[v] = o0 + b
             self._where.append((b, num_classes))
         self.image_ids += ids
         self._num_records += B * cap
-        self._num_chars += nch
         self._num_classes = max(self._num_classes, num_classes)
         self._all_masks = self._all_masks and masks is not None
 
@@ -740,6 +817,7 @@ def _flatten_device(gt, acc, iou_type, category_ids):
         cls_k[j] = cat_index[category_ids[j - 1]]
     I, K = gt.num_images, gt.num_cats
     nb, n, dev = I * K, acc._num_records, gt.device
+    acc._drain()                        # every masked batch settled (and redone if it overflowed) before its records are read
     L = _lib.lib()
     rec_f, rec_i = (acc._rec_f, acc._rec_i) if n else (None, None)
     with torch.cuda.device(dev):

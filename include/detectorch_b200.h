@@ -134,6 +134,28 @@ int dt_segm_rle_batch(const float* masks, const int* classes, int num_mask_class
                       const int* im_sizes, int batch, int cap, int max_im_h, int max_im_w, float thresh_binarize, int runs_cap,
                       uint8_t* strings, int64_t* str_offsets, int* overflow, void* workspace, dt_stream_t stream);
 
+/* dt_segm_rle_batch for a caller that must not wait for the device (utils.coco_eval.DeviceResults.add, a captured CUDA graph): the
+ * same strings, byte for byte, appended to a caller-owned char arena at a device-side cursor, with every outcome left in device flags.
+ * The call issues stream operations only (no host read, no allocation), so it can be captured and replayed with new table contents.
+ *   masks, classes, num_mask_classes, boxes, num_dets_dev, thresh_binarize, runs_cap, workspace: as for dt_segm_rle_batch (the workspace
+ *                  is dt_segm_batch_workspace_bytes(batch, cap, runs_cap))
+ *   im_sizes       int32 [batch, 2]: (im_h, im_w) of each image's RLE canvas, read on the device only.  The shared-memory tables are
+ *                  sized for images of up to DT_SEGM_APPEND_MAX_SIDE x DT_SEGM_APPEND_MAX_SIDE, which with the 200 KB shared-memory
+ *                  limit allows masks of up to 98 x 98
+ *   arena          arena_capacity bytes; cursor int64 [1]: its used length.  The batch's B*cap strings go to arena[*cursor ..], slot
+ *                  s = b * cap + d after slot s - 1, and *cursor advances by their total; str_offsets [batch*cap+1] int64 are arena
+ *                  offsets (str_offsets[s + 1] - str_offsets[s] is slot s's length)
+ *   flags          int32 [3], zeroed by the call: [0] 0, or the most runs a slot needed when runs_cap (or its string staging) was too
+ *                  small; [1] 1 if an image's size is outside [1, DT_SEGM_APPEND_MAX_SIDE]; [2] 1 if the strings did not fit: cursor +
+ *                  total > arena_capacity (then str_offsets[batch*cap] - str_offsets[0] is the total needed).
+ *                  With any flag raised nothing is written to the arena and the cursor is left as it was: grow, then redo the batch.
+ * Returns 0 for a mask size beyond the table limit, batch > 65535, runs_cap < 2 or a NULL pointer. */
+#define DT_SEGM_APPEND_MAX_SIDE 8192
+int dt_segm_rle_batch_append(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes,
+                             const int* num_dets_dev, const int* im_sizes, int batch, int cap, float thresh_binarize, int runs_cap,
+                             uint8_t* arena, int64_t arena_capacity, int64_t* cursor, int64_t* str_offsets, int* flags, void* workspace,
+                             dt_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Image pre-processing (the step right before the path, SURVEY.md 8f rank 3).
  * Replaces: lib/utils/blob.py:57-87 prep_im_for_blob (float32, minus pixel_means, cv2.resize(fx=fy=im_scale, INTER_LINEAR)) fused
