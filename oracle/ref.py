@@ -190,10 +190,12 @@ def _decode_torch(boxes, deltas, weights=(1.0, 1.0, 1.0, 1.0)):
 
 def generate_proposals_level(rpn_cls_prob, rpn_bbox_pred, im_h, im_w, scaling_factor, spatial_scale,
                              anchor_sizes, aspect_ratios=(0.5, 1, 2), pre_nms_top_n=6000, post_nms_top_n=1000,
-                             nms_thresh=0.7, min_size=0, return_stages=False):
+                             nms_thresh=0.7, min_size=0, return_stages=False, tie_order="numpy"):
     """One image, one level.  rpn_cls_prob [1,A,H,W], rpn_bbox_pred [1,4A,H,W] (torch CPU fp32).
     generate_proposals.py:31-122.  Returns (proposals [n,4], scores [n,1]) torch fp32;
-    with return_stages also a dict of the integer stages (order, filter keep, nms keep)."""
+    with return_stages also a dict of the integer stages (order, filter keep, nms keep).
+    tie_order: the order of equal scores in the top-k and in the NMS.  "numpy" is the reference's own (argpartition / argsort,
+    unspecified among ties); "stable" is (score desc, anchor index asc), the order the device documents."""
     anchors = generate_anchors(stride=1. / spatial_scale, sizes=anchor_sizes, aspect_ratios=aspect_ratios)
     A = anchors.shape[0]
     H, W = rpn_cls_prob.shape[2], rpn_cls_prob.shape[3]
@@ -202,7 +204,13 @@ def generate_proposals_level(rpn_cls_prob, rpn_bbox_pred, im_h, im_w, scaling_fa
     deltas = rpn_bbox_pred.squeeze(0).permute(1, 2, 0).contiguous().view(-1, 4)    # :64
     scores = rpn_cls_prob.squeeze(0).permute(1, 2, 0).contiguous().view(-1, 1)     # :72
     s_np = scores.numpy()
-    if pre_nms_top_n <= 0 or pre_nms_top_n >= len(s_np):
+    if tie_order == "stable":
+        order = np.argsort(-s_np.squeeze(1), kind="stable")
+        if 0 < pre_nms_top_n < len(s_np):
+            order = order[:pre_nms_top_n]
+    elif tie_order != "numpy":
+        raise ValueError("generate_proposals_level: tie_order must be 'numpy' or 'stable'")
+    elif pre_nms_top_n <= 0 or pre_nms_top_n >= len(s_np):
         order = np.argsort(-s_np.squeeze())                                        # :78
     else:
         inds = np.argpartition(-s_np.squeeze(), pre_nms_top_n)[:pre_nms_top_n]      # :82-84
@@ -228,7 +236,7 @@ def generate_proposals_level(rpn_cls_prob, rpn_bbox_pred, im_h, im_w, scaling_fa
     p_np, s_np = p_np[fkeep, :], s_np[fkeep]
     nkeep = None
     if nms_thresh > 0:
-        nkeep = nms(np.hstack((p_np, s_np)), nms_thresh)                           # :115
+        nkeep = nms(np.hstack((p_np, s_np)), nms_thresh, order=tie_order)          # :115
         if post_nms_top_n > 0:
             nkeep = nkeep[:post_nms_top_n]
         props, scores = props[nkeep, :], scores[nkeep, :]
@@ -249,12 +257,14 @@ def map_rois_to_fpn_levels(rois, k_min, k_max, s0=224, lvl0=4):
     return np.clip(lv, k_min, k_max)
 
 
-def collect_and_distribute(roi_list, score_list, lvl_min=2, lvl_max=5, post_nms_top_n=1000):
+def collect_and_distribute(roi_list, score_list, lvl_min=2, lvl_max=5, post_nms_top_n=1000, stable=False):
     """collect...py:84-128.  roi_list: per-level torch [n_l,4]; score_list: [n_l,1].
-    Returns (per-level roi tensors, idx_restore int64 numpy, collected rois [n,4], lvls)."""
+    Returns (per-level roi tensors, idx_restore int64 numpy, collected rois [n,4], lvls).
+    stable: equal scores keep their concatenated (level, rank) order, as the device sorts them; the reference's torch.sort leaves
+    that order unspecified."""
     rois = torch.cat(tuple(roi_list), 0)
-    scores = torch.cat(tuple(score_list), 0).squeeze()
-    _, inds = torch.sort(-scores)                                                  # :102
+    scores = torch.cat(tuple(score_list), 0).reshape(-1)
+    _, inds = torch.sort(-scores, stable=stable)                                   # :102
     rois = rois[inds[:post_nms_top_n], :]
     lvls = map_rois_to_fpn_levels(rois.numpy(), lvl_min, lvl_max)
     order = np.empty((0,))
