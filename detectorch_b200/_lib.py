@@ -59,6 +59,9 @@ SIGNATURES = {
     "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                              c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "dt_coco_eval_imgs": (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p]),
     "dt_coco_results_append": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
     "dt_coco_results_count": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,

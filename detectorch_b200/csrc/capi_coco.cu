@@ -65,6 +65,28 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
     return 1;
 }
 
+extern "C" int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* union_keys, int num_active, const int64_t* pairs, int64_t num_dets,
+                                 const double* det_f, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
+                                 const int64_t* gt_keys, const double* gt_f, const int64_t* gt_i, const double* params, const double* ious,
+                                 const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos, uint8_t* gt_ig,
+                                 dt_stream_t stream) {
+    if ((iou_type != 0 && iou_type != 1) || num_union < 0 || num_active < 0 || num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 ||
+        num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || num_active > num_union) {
+        fprintf(stderr, "dt_coco_eval_imgs: bad sizes\n");
+        return 0;
+    }
+    if (num_union == 0) return 1;
+    if (!union_keys || !params || (num_gts > 0 && (!gt_keys || !gt_f || !gt_i || !gt_dt || !gt_pos || !gt_ig)) ||
+        (num_active > 0 && (!pairs || !det_f || !ious || !workspace || !slot_det || !dt_gt || !dt_ig))) {
+        fprintf(stderr, "dt_coco_eval_imgs: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(coco_eval_imgs_launch(iou_type, num_union, union_keys, num_active, pairs, num_dets, num_chars, kept, num_ious, num_gts, num_order,
+                                        gt_keys, det_f, gt_f, gt_i, params, ious, workspace, slot_det, dt_gt, dt_ig, gt_dt, gt_pos, gt_ig,
+                                        (cudaStream_t)stream));
+    return 1;
+}
+
 extern "C" int dt_coco_results_append(int batch, int cap, int num_classes, const float* boxes, const float* scores, const int* classes,
                                       const int* counts, const int64_t* images, const int64_t* str_offs, int64_t char_base, float* rec_f,
                                       int64_t* rec_i, int* err, dt_stream_t stream) {

@@ -696,4 +696,110 @@ inline cudaError_t coco_results_write_launch(int64_t n, const float* rec_f, cons
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------ per-image records (evalImgs)
+// COCOeval.evaluate() keeps one record per (category, area range, image) whose pair has detections or gts: which gt each detection
+// matched at each threshold, which detection each gt matched last, and which of them were ignored.  After dt_coco_eval, from its
+// workspace (kept slots, segm areas) and the IoU matrices it kept (never recomputed):
+//
+//   coco_eval_imgs_kernel   one CTA per pair of a union table (the sorted pair indices of the pairs with detections and of those with
+//                           gts): per gt and area range its place in the stable ignore-last order; then one thread per (area range,
+//                           threshold) repeats coco_pair_kernel's matching, keeping the indices it matched.
+//
+// Outputs, with state c = area range * 10 + threshold as in state[]:
+//   slot_det [kept]        detection index of each kept slot (for the host's mapping to detection ids and scores)
+//   dt_gt [kept][40]       index in its pair (annotation order) of the gt the kept detection matched, -1 for none
+//   dt_ig [kept][40]       evaluateImg's dtIgnore
+//   gt_dt [gts][40]        rank in its pair of the last kept detection that matched the gt (a crowd gt matches several), -1 for none
+//   gt_pos [gts][4]        the gt's position in the area range's ignore-last order;  gt_ig [gts][4] its ignore flag
+struct CocoEvalImgsArgs {
+    int segm;
+    int64_t n_active, n_gt;
+    const int64_t* ukeys; const int64_t* pairs; const int64_t* gt_keys;
+    const double* det_f; const double* det_area; const int* kept_det;
+    const double* gt_f; const int64_t* gt_i; const double* par; const double* iou;
+    int* slot_det; int* dt_gt; uint8_t* dt_ig; int* gt_dt; int* gt_pos; uint8_t* gt_ig;
+};
+
+__global__ void coco_eval_imgs_kernel(CocoEvalImgsArgs p) {
+    const int64_t key = p.ukeys[blockIdx.x];
+    const int64_t g0 = coco_lower_bound(p.gt_keys, p.n_gt, key, false), G = coco_lower_bound(p.gt_keys, p.n_gt, key, true) - g0;
+    int64_t lo = 0, hi = p.n_active;                 // the pair's row among the pairs with detections, if it has any
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (p.pairs[mid * kCocoPairCols] < key) lo = mid + 1; else hi = mid;
+    }
+    const int64_t* T = lo < p.n_active && p.pairs[lo * kCocoPairCols] == key ? p.pairs + lo * kCocoPairCols : nullptr;
+    const int64_t D = T ? T[2] : 0, k0 = T ? T[5] : 0, i0 = T ? T[6] : 0;
+    const int64_t Dk = D < kCocoKeep ? D : kCocoKeep;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    for (int64_t e = tid; e < G * kCocoStates; e += nt) p.gt_dt[g0 * kCocoStates + e] = -1;
+    for (int64_t r = tid; r < Dk; r += nt) p.slot_det[k0 + r] = p.kept_det[k0 + r];
+    // gtind = np.argsort(_ignore, kind='mergesort'): the kept gts in annotation order, then the ignored ones
+    for (int ar = tid; ar < kCocoAreas; ar += nt) {
+        const double* rng = p.par + kCocoParAreas + 2 * ar;
+        int64_t n_keep = 0;
+        for (int64_t g = 0; g < G; g++) n_keep += !(p.gt_i[(g0 + g) * kCocoGtI + 4] != 0 || coco_out(p.gt_f[(g0 + g) * kCocoGtF + 4], rng));
+        int64_t a = 0, b = n_keep;
+        for (int64_t g = 0; g < G; g++) {
+            const bool ig = p.gt_i[(g0 + g) * kCocoGtI + 4] != 0 || coco_out(p.gt_f[(g0 + g) * kCocoGtF + 4], rng);
+            p.gt_pos[(g0 + g) * kCocoAreas + ar] = (int)(ig ? b++ : a++);
+            p.gt_ig[(g0 + g) * kCocoAreas + ar] = ig;
+        }
+    }
+    __syncthreads();
+    // coco_pair_kernel's matching, step for step; a gt is taken when gt_dt holds a rank (the last one for a crowd gt)
+    for (int c = tid; c < kCocoStates; c += nt) {
+        const int ar = c / kCocoThrs, t = c % kCocoThrs;
+        const double* rng = p.par + kCocoParAreas + 2 * ar;
+        int* gm = p.gt_dt + g0 * kCocoStates + c;    // gm[g * kCocoStates]
+        for (int64_t dr = 0; dr < Dk; dr++) {
+            double best = p.par[kCocoParThrs + t];
+            int64_t m = -1;
+            bool m_ig = false;
+            for (int pass = 0; pass < 2; pass++) {
+                for (int64_t g = 0; g < G; g++) {
+                    const int64_t* GI = p.gt_i + (g0 + g) * kCocoGtI;
+                    const bool ig = GI[4] != 0 || coco_out(p.gt_f[(g0 + g) * kCocoGtF + 4], rng);
+                    if ((int)ig != pass) continue;
+                    if (gm[g * kCocoStates] >= 0 && !GI[4]) continue;
+                    if (m > -1 && !m_ig && ig) goto matched;
+                    const double o = p.iou[i0 + dr * G + g];
+                    if (o < best) continue;
+                    best = o; m = g; m_ig = ig;
+                }
+            }
+        matched:
+            bool hit = false, dig = false;
+            if (m > -1) {
+                dig = m_ig;
+                hit = p.gt_i[(g0 + m) * kCocoGtI + 5] != 0;
+                gm[m * kCocoStates] = (int)dr;
+            }
+            const int64_t d = p.kept_det[k0 + dr];
+            const double area = p.segm ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
+            if (!hit && coco_out(area, rng)) dig = true;
+            p.dt_gt[(k0 + dr) * kCocoStates + c] = (int)m;
+            p.dt_ig[(k0 + dr) * kCocoStates + c] = dig;
+        }
+    }
+}
+
+// workspace: the one dt_coco_eval has just filled, of the same sizes; ious: the IoU matrices it kept
+inline cudaError_t coco_eval_imgs_launch(int segm, int n_union, const int64_t* ukeys, int n_active, const int64_t* pairs, int64_t n_det,
+                                         int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt, int64_t n_order, const int64_t* gt_keys,
+                                         const double* det_f, const double* gt_f, const int64_t* gt_i, const double* par, const double* ious,
+                                         const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos,
+                                         uint8_t* gt_ig, cudaStream_t st) {
+    const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order);
+    const uint8_t* ws = reinterpret_cast<const uint8_t*>(workspace);
+    CocoEvalImgsArgs p;
+    p.segm = segm; p.n_active = n_active; p.n_gt = n_gt;
+    p.ukeys = ukeys; p.pairs = pairs; p.gt_keys = gt_keys;
+    p.det_f = det_f; p.det_area = reinterpret_cast<const double*>(ws + L.det_area); p.kept_det = reinterpret_cast<const int*>(ws + L.kept_det);
+    p.gt_f = gt_f; p.gt_i = gt_i; p.par = par; p.iou = ious;
+    p.slot_det = slot_det; p.dt_gt = dt_gt; p.dt_ig = dt_ig; p.gt_dt = gt_dt; p.gt_pos = gt_pos; p.gt_ig = gt_ig;
+    if (n_union > 0) coco_eval_imgs_kernel<<<n_union, 64, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
 }  // namespace dt

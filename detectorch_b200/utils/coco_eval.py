@@ -6,6 +6,11 @@ file that lib/utils/json_dataset_evaluator.py would write; no file is written.
     E = evaluate(gt, detector.detect_images(ims), "segm")  # or evaluate(gt, all_boxes, "bbox") / evaluate(gt, all_boxes, "segm", all_segms)
     E.stats, E.eval["precision"]                          # summarize()'s 12 numbers, [T, R, K, A, M]
     acc = DeviceResults(); acc.add(detector.detect(...), image_ids, original_sizes=orig); evaluate(gt, acc, "segm")   # no host copy
+    E = evaluate(gt, results, "bbox", keep_eval_imgs=True)  # + COCOeval's per-image records:
+    E.eval_imgs["dtMatches"], E.evalImgs[n]               # as flat columns, or as COCOeval's list of dicts (built when first read)
+
+keep_eval_imgs=True runs one more kernel after the evaluation, on the IoUs it kept; the records' detection ids are the ones loadRes
+gives the rows of the results file (1 + the row's index), their GT ids the annotation ids.
 
 The host only checks and flattens the annotations and results into arrays (csrc/coco_eval.cuh documents their layout); everything
 numeric runs in the CUDA kernels of coco_eval.cuh.  Malformed annotations or results raise ValueError before the evaluation is
@@ -368,13 +373,24 @@ class Params:
 
 
 class CocoEvalResult:
-    """What a COCOeval object holds after evaluate() + accumulate() (+ summarize() for .stats): .params, .eval, .stats."""
+    """What a COCOeval object holds after evaluate() + accumulate() (+ summarize() for .stats): .params, .eval, .stats; with
+    evaluate(..., keep_eval_imgs=True) also .evalImgs, built from the columns .eval_imgs when first read."""
+    eval_imgs = None
 
     def __init__(self, params, precision, recall, scores):
         self.params = params
         T, R, K, A, M = precision.shape
         self.eval = {'params': params, 'counts': [T, R, K, A, M], 'precision': precision, 'recall': recall, 'scores': scores}
         self.stats = self._stats(verbose=False)
+        self._eval_imgs_list = None
+
+    @property
+    def evalImgs(self):
+        if self.eval_imgs is None:
+            raise AttributeError("evalImgs: evaluate(..., keep_eval_imgs=True) keeps the per-image records")
+        if self._eval_imgs_list is None:
+            self._eval_imgs_list = _eval_imgs_list(self.params, self.eval_imgs)
+        return self._eval_imgs_list
 
     def summarize(self):
         self.stats = self._stats(verbose=True)
@@ -438,9 +454,10 @@ def _per_class(gt, results, all_segms, iou_type):
     return results, all_segms
 
 
-def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids):
+def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids, with_ids=False):
     """_write_coco_{bbox,segms}_results_file + COCO.loadRes, as arrays: one row per result in the file's order (class-major, images in
-    sorted-id order), bbox = xyxy_to_xywh of the float64 boxes (+1 width), score = the float64 of the stored value."""
+    sorted-id order), bbox = xyxy_to_xywh of the float64 boxes (+1 width), score = the float64 of the stored value.  Rows come back
+    sorted by key (category index, image index); with_ids adds each row's loadRes id (1 + its index in the file) as a fifth value."""
     I = gt.num_images
     cat_index = {v: n for n, v in enumerate(gt.cat_ids)}
     segm = iou_type == 'segm'
@@ -502,15 +519,19 @@ def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids):
         det_i[:, 1] = lens
         det_i[:, 2:4] = sizes
     order = np.argsort(key, kind='stable')
+    if with_ids:
+        return key[order], det_f[order], det_i[order], chars, order + 1
     return key[order], det_f[order], det_i[order], chars
 
 
-def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False):
+def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False, keep_eval_imgs=False):
     """COCOeval(gt, loadRes(results file), iou_type).evaluate() + accumulate() on the device -> CocoEvalResult.
     results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), the notebooks' all_boxes
     [class][image] (with all_segms [class][image] for 'segm'), or a DeviceResults (flattened on the device, on gt's device).  category_ids: json id of contiguous class j (1-based) at j - 1;
     default: the dataset's category order, as JsonDataset builds its classes.  keep_ious: also return COCOeval's .ious, {(image id,
-    category id): [min(D, 100), G] array} for the pairs with detections and GTs."""
+    category id): [min(D, 100), G] array} for the pairs with detections and GTs.  keep_eval_imgs: also return COCOeval's per-image
+    records, as .eval_imgs (columns, see _eval_imgs_columns) and .evalImgs (the list of dicts, built from the columns when first read);
+    detection ids are the ones loadRes gives the results file's rows, 1 + the row's index."""
     if iou_type not in ('bbox', 'segm'):
         raise ValueError("iou_type must be 'bbox' or 'segm'")
     if not isinstance(gt, CocoGroundTruth):
@@ -523,18 +544,23 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
     if isinstance(results, DeviceResults):
         if all_segms is not None:
             raise ValueError("a DeviceResults carries its masks; all_segms is for all_boxes input")
-        f = _flatten_device(gt, results, iou_type, category_ids)
+        f = _flatten_device(gt, results, iou_type, category_ids, keep_eval_imgs)
+        imgs = (f['union'], f['det_ids']) if keep_eval_imgs else None
         return _evaluate_tables(gt, iou_type, None, f['pairs'], f['cat_kept'], f['order_off'], f['det_f'], f['det_i'], f['chars'],
-                                f['num_chars'], f['num_kept'], f['num_ious'], f['num_order'], keep_ious)
+                                f['num_chars'], f['num_kept'], f['num_ious'], f['num_order'], keep_ious, imgs)
     boxes, segms = _per_class(gt, results, all_segms, iou_type)
-    key, det_f, det_i, chars = _flatten_results(gt, boxes, segms, iou_type, category_ids)
+    key, det_f, det_i, chars, det_ids = _flatten_results(gt, boxes, segms, iou_type, category_ids, with_ids=True)
     pairs, cat_kept, order_off = _pair_tables(gt, key)
     kept, gn = np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
     n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(order_off[-1, -1])
     dev = gt.device
     up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, cat_kept, order_off, det_f, det_i)]
     ch = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
-    return _evaluate_tables(gt, iou_type, pairs, *up, ch, len(chars), n_kept, n_iou, n_order, keep_ious)
+    imgs = None
+    if keep_eval_imgs:
+        # the pairs COCOeval keeps a record of: those with detections and those with gts
+        imgs = tuple(torch.from_numpy(x).to(dev) for x in (np.union1d(pairs[:, 0], gt.keys).astype(np.int64), det_ids.astype(np.int64)))
+    return _evaluate_tables(gt, iou_type, pairs, *up, ch, len(chars), n_kept, n_iou, n_order, keep_ious, imgs)
 
 
 def _pair_tables(gt, key):
@@ -560,8 +586,10 @@ def _pair_tables(gt, key):
     return pairs, cat_kept, order_off
 
 
-def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_f_d, det_i_d, ch, num_chars, n_kept, n_iou, n_order, keep_ious):
-    """dt_coco_eval on the flattened results, already on gt's device (pairs: their host copy, or None to read it back for keep_ious)."""
+def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_f_d, det_i_d, ch, num_chars, n_kept, n_iou, n_order, keep_ious,
+                     imgs=None):
+    """dt_coco_eval on the flattened results, already on gt's device (pairs: their host copy, or None to read it back for keep_ious).
+    imgs: (union keys [Q], detection ids [N]) on the device to also run dt_coco_eval_imgs, None to leave it out."""
     I, K, N = gt.num_images, gt.num_cats, int(det_f_d.shape[0])
     dev = gt.device
     T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
@@ -577,20 +605,107 @@ def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_
         nb = torch.nonzero(bad).flatten()[:1].cpu().numpy()
         if len(nb):
             raise ValueError("results: RLE counts of result %d (in (category, image) order) do not sum to h * w" % nb[0])
-    ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious else None
+    # the records read the IoU matrices dt_coco_eval keeps, rather than computing them again
+    ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious or imgs is not None else None
     ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, num_chars, n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
     _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, int(pairs_d.shape[0]), _p(pairs_d), _p(cat_gt_d), _p(cat_kept_d),
                               _p(order_off_d), N, _p(det_f_d), _p(det_i_d), _p(ch), num_chars, n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f),
                               _p(gt.gt_i), _p(gt.gt_counts), _p(par_d), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
+    if imgs is not None:
+        ukeys_d, det_ids_d = imgs
+        Q, G = int(ukeys_d.shape[0]), gt.num_gts
+        slot_det = torch.empty((max(n_kept, 1),), dtype=torch.int32, device=dev)
+        dt_gt = torch.empty((max(n_kept, 1), A * T), dtype=torch.int32, device=dev)
+        dt_ig = torch.empty((max(n_kept, 1), A * T), dtype=torch.uint8, device=dev)
+        gt_dt = torch.empty((max(G, 1), A * T), dtype=torch.int32, device=dev)
+        gt_pos = torch.empty((max(G, 1), A), dtype=torch.int32, device=dev)
+        gt_ig = torch.empty((max(G, 1), A), dtype=torch.uint8, device=dev)
+        _lib.check(L.dt_coco_eval_imgs(1 if iou_type == 'segm' else 0, Q, _p(ukeys_d), int(pairs_d.shape[0]), _p(pairs_d), N, _p(det_f_d),
+                                       num_chars, n_kept, n_iou, G, n_order, _p(gt.keys_d), _p(gt.gt_f), _p(gt.gt_i), _p(par_d), _p(ious), _p(ws),
+                                       _p(slot_det), _p(dt_gt), _p(dt_ig), _p(gt_dt), _p(gt_pos), _p(gt_ig), _stream(dev)), "dt_coco_eval_imgs")
+        # each kept slot's detection id and score, gathered on the device
+        sd = slot_det[:n_kept].long()
+        slot_id, slot_score = det_ids_d[sd], det_f_d[sd, 0]
+        dev_out = dict(ukeys=ukeys_d, slot_id=slot_id, slot_score=slot_score, dt_gt=dt_gt[:n_kept], dt_ig=dt_ig[:n_kept], gt_dt=gt_dt[:G],
+                       gt_pos=gt_pos[:G], gt_ig=gt_ig[:G])
     E = CocoEvalResult(Params(gt, iou_type), prec.cpu().numpy(), rec.cpu().numpy(), scr.cpu().numpy())
+    if (keep_ious or imgs is not None) and pairs is None:
+        pairs = pairs_d.cpu().numpy()
+    if imgs is not None:
+        E.eval_imgs = _eval_imgs_columns(gt, pairs, {k: v.cpu().numpy() for k, v in dev_out.items()})
     if keep_ious:
-        if pairs is None:
-            pairs = pairs_d.cpu().numpy()
         pk, kept, gn = pairs[:, 0], np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
         iv = ious.cpu().numpy()
         E.ious = {(gt.img_ids[k % I], gt.cat_ids[k // I]): iv[o:o + d * g].reshape(d, g)
                   for k, d, g, o in zip(pk, kept, gn, pairs[:, 6]) if g > 0}
     return E
+
+
+def _eval_imgs_columns(gt, pairs, o):
+    """dt_coco_eval_imgs' outputs (host copies, with each kept slot's detection id and score) -> COCOeval.evalImgs as flat columns.
+    The records are evalImgs' non-None entries in its order (category, area range, image), one per area range of each pair with
+    detections or gts; record r owns detection rows dt_off[r]:dt_off[r + 1] (score order, cut to 100) and gt rows gt_off[r]:gt_off[r + 1]
+    (the area range's ignore-last order):
+        index [R]                         the record's position in evalImgs (K * 4 * I entries)
+        image_id, category_id, area [R]   its json ids and area range index
+        dt_off, gt_off [R + 1]
+        dtIds [n_dt] int64, dtScores [n_dt] float64, dtMatches [10, n_dt] float64 (matched gt's id, 0 for none), dtIgnore [10, n_dt] bool
+        gtIds [n_gt] int64, gtIgnore [n_gt] int64, gtMatches [10, n_gt] float64 (id of the last detection that matched, 0 for none)"""
+    I, A, T = gt.num_images, len(AREA_RNG), len(IOU_THRS)
+    uk = o['ukeys']
+    Q, P, n_kept = len(uk), len(pairs), len(o['slot_id'])
+    pi = np.minimum(np.searchsorted(pairs[:, 0], uk), max(P - 1, 0))
+    has = pairs[pi, 0] == uk if P else np.zeros(Q, bool)
+    Dk = np.where(has, np.minimum(pairs[pi, 2], MAX_DETS[-1]), 0) if P else np.zeros(Q, np.int64)
+    k0 = np.where(has, pairs[pi, 5], 0) if P else np.zeros(Q, np.int64)
+    g0 = np.searchsorted(gt.keys, uk, 'left')
+    Gq = np.searchsorted(gt.keys, uk, 'right') - g0
+    # records (q, a) in evalImgs order
+    pos = ((uk // max(I, 1))[:, None] * A + np.arange(A)) * I + (uk % max(I, 1))[:, None]
+    order = np.argsort(pos, axis=None)
+    rq, ra = order // A, order % A
+    R = len(order)
+    off = lambda c: np.concatenate([[0], np.cumsum(c)]).astype(np.int64)
+    dt_off, gt_off = off(Dk[rq]), off(Gq[rq])
+    ann = np.concatenate([np.asarray(gt.ann_ids, np.int64), [0]])          # index num_gts: "no gt"
+    sid = np.concatenate([o['slot_id'].astype(np.int64), [0]])               # index n_kept: "no detection"
+    # detection rows: the record's kept slots, in rank order
+    rec = np.repeat(np.arange(R), Dk[rq])
+    slot = k0[rq][rec] + np.arange(len(rec)) - dt_off[rec]
+    a_dt = ra[rec]
+    m = o['dt_gt'].reshape(-1, A, T)[slot, a_dt]
+    dt_matches = ann[np.where(m >= 0, g0[rq][rec][:, None] + m, len(ann) - 1)].astype(np.float64).T.copy()
+    dt_ignore = o['dt_ig'].reshape(-1, A, T)[slot, a_dt].astype(bool).T.copy()
+    # gt rows: each gt of each area range at its place in that range's order
+    Gt = len(gt.keys)
+    rec_of = np.empty(Q * A, np.int64)
+    rec_of[order] = np.arange(R)
+    qg = np.searchsorted(uk, gt.keys)
+    dest = (gt_off[rec_of[qg[:, None] * A + np.arange(A)]] + o['gt_pos']).reshape(-1)
+    src_g, src_a = np.empty(Gt * A, np.int64), np.empty(Gt * A, np.int64)
+    src_g[dest], src_a[dest] = np.repeat(np.arange(Gt), A), np.tile(np.arange(A), Gt)
+    r = o['gt_dt'].reshape(-1, A, T)[src_g, src_a]
+    gt_matches = sid[np.where(r >= 0, k0[qg][src_g][:, None] + r, n_kept)].astype(np.float64).T.copy()
+    return dict(index=pos.reshape(-1)[order], image_id=np.asarray(gt.img_ids, np.int64)[uk[rq] % max(I, 1)],
+                category_id=np.asarray(gt.cat_ids, np.int64)[uk[rq] // max(I, 1)], area=ra, dt_off=dt_off, gt_off=gt_off,
+                dtIds=o['slot_id'].astype(np.int64)[slot], dtScores=o['slot_score'][slot], dtMatches=dt_matches, dtIgnore=dt_ignore,
+                gtIds=ann[src_g], gtIgnore=o['gt_ig'][src_g, src_a].astype(np.int64), gtMatches=gt_matches)
+
+
+def _eval_imgs_list(params, c):
+    """The columns of _eval_imgs_columns -> COCOeval.evalImgs, a list of K * 4 * I dicts or None.  The arrays of a record are views of
+    the columns."""
+    out = [None] * (len(params.catIds) * len(params.areaRng) * len(params.imgIds))
+    dt_off, gt_off = c['dt_off'].tolist(), c['gt_off'].tolist()
+    dt_ids, dt_scores, gt_ids = c['dtIds'].tolist(), c['dtScores'].tolist(), c['gtIds'].tolist()
+    dm, di, gm, gi = c['dtMatches'], c['dtIgnore'], c['gtMatches'], c['gtIgnore']
+    max_det = params.maxDets[-1]
+    for r, (n, img, cat, a) in enumerate(zip(c['index'].tolist(), c['image_id'].tolist(), c['category_id'].tolist(), c['area'].tolist())):
+        d0, d1, g0, g1 = dt_off[r], dt_off[r + 1], gt_off[r], gt_off[r + 1]
+        out[n] = {'image_id': img, 'category_id': cat, 'aRng': params.areaRng[a], 'maxDet': max_det, 'dtIds': dt_ids[d0:d1],
+                  'gtIds': gt_ids[g0:g1], 'dtMatches': dm[:, d0:d1], 'gtMatches': gm[:, g0:g1], 'dtScores': dt_scores[d0:d1],
+                  'gtIgnore': gi[g0:g1] if g1 > g0 else np.array([]), 'dtIgnore': di[:, d0:d1]}   # COCOeval's np.array([]) of no gts
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------ device-resident results
@@ -795,10 +910,55 @@ class DeviceResults:
         self._all_masks = self._all_masks and masks is not None
 
 
-def _flatten_device(gt, acc, iou_type, category_ids):
+def _flatten_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
     """_flatten_results + _pair_tables for a DeviceResults, on the device: -> dict of device tensors key [N], det_f [N, 5], det_i [N, 4]
     (char offsets into acc's buffer `chars`), pairs [P, 7], cat_kept [K + 1], order_off [3, K + 1], and the sizes dt_coco_eval takes.
-    Host checks raise ValueError before anything is launched; the device's error flags come back with the sizes, in one copy."""
+    Host checks raise ValueError before anything is launched; the device's error flags come back with the sizes, in one copy.
+    keep_eval_imgs adds det_ids [N] (loadRes ids, as with_ids of _flatten_results) and union [Q], the sorted keys of the pairs with
+    detections or gts."""
+    b = _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs)
+    I, K, nb, dev = gt.num_images, gt.num_cats, gt.num_images * gt.num_cats, gt.device
+    n, nc, rec_f, rec_i, cls_d, ord_d, scan = b['n'], b['nc'], b['rec_f'], b['rec_i'], b['cls_d'], b['ord_d'], b['scan']
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        tail = b['tail'].cpu().numpy()
+        if tail[5]:
+            bo, ncls = acc._where[int(tail[6])]
+            raise RuntimeError("batch_results: the detections of image %d are not grouped by class in 1..%d" % (bo, ncls - 1))
+        if tail[7]:
+            raise ValueError("non-finite box or score in the results")
+        N, P, c10, n_kept, n_iou = (int(v) for v in tail[:5])
+        key = torch.empty((max(N, 1),), dtype=torch.int64, device=dev)
+        det_f = torch.empty((max(N, 1), 5), dtype=torch.float64, device=dev)
+        det_i = torch.empty((max(N, 1), 4), dtype=torch.int64, device=dev)
+        pairs = torch.empty((max(P, 1), 7), dtype=torch.int64, device=dev)
+        cat_kept = torch.empty((K + 1,), dtype=torch.int64, device=dev)
+        order_off = torch.empty((3, K + 1), dtype=torch.int64, device=dev)
+        _lib.check(L.dt_coco_results_write(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(scan), _p(gt.keys_d), gt.num_gts, _p(key),
+                                           _p(det_f), _p(det_i), _p(pairs), _p(cat_kept), _p(order_off), _stream(dev)), "dt_coco_results_write")
+        extra = {}
+        if keep_eval_imgs:
+            # row n of key k is file row file_start[k] + (n - first row of k); the union's keys are compacted by their scan
+            Q = int(tail[8])
+            if nb:
+                k = key[:N]
+                first = scan[0] - b['vals'][0]
+                extra['det_ids'] = torch.arange(N, device=dev) - first[k] + b['file_start'][k] + 1
+                dst = torch.where(b['has'], b['union_scan'] - 1, nb)
+                union = torch.empty((nb + 1,), dtype=torch.int64, device=dev)         # slot nb takes the bins left out
+                extra['union'] = union.scatter_(0, dst, torch.arange(nb, device=dev))[:Q]
+            else:
+                extra['det_ids'] = extra['union'] = torch.zeros((0,), dtype=torch.int64, device=dev)
+    chars = acc._chars if acc._chars is not None else torch.zeros((1,), dtype=torch.uint8, device=dev)
+    return dict(key=key[:N], det_f=det_f[:N], det_i=det_i[:N], pairs=pairs[:P], cat_kept=cat_kept, order_off=order_off, chars=chars,
+                num_chars=acc._num_chars, num_kept=n_kept, num_ious=n_iou, num_order=P + c10 + n_kept, **extra)
+
+
+def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
+    """_flatten_device up to its one read-back, without a host synchronisation: the host checks, the counting pass and the bin scans;
+    -> dict of the tables the write pass takes and `tail`, the device vector of sizes and flags to read back.  keep_eval_imgs adds
+    each bin's first row in the results file (file_start: class-major, images in sorted-id order, the scan of the bins' counts in
+    that order), the bins that have detections or gts (has) and their inclusive scan, whose total ends `tail`."""
     if acc.device != gt.device:
         raise ValueError("the results are on %s, the ground truth on %s" % (acc.device, gt.device))
     if iou_type == 'segm' and not acc._all_masks:
@@ -820,8 +980,9 @@ def _flatten_device(gt, acc, iou_type, category_ids):
     acc._drain()                        # every masked batch settled (and redone if it overflowed) before its records are read
     L = _lib.lib()
     rec_f, rec_i = (acc._rec_f, acc._rec_i) if n else (None, None)
+    out = dict(n=n, nc=nc, rec_f=rec_f, rec_i=rec_i)
     with torch.cuda.device(dev):
-        cls_d, ord_d = torch.from_numpy(cls_k).to(dev), torch.from_numpy(ord_i).to(dev)
+        cls_d, ord_d = _pinned_upload(cls_k, dev), _pinned_upload(ord_i, dev)
         nonfinite = torch.zeros((1,), dtype=torch.int32, device=dev)
         cnt = torch.zeros((nb,), dtype=torch.int32, device=dev) if nb else None
         vals = torch.empty((5, nb), dtype=torch.int64, device=dev) if nb else None
@@ -829,24 +990,24 @@ def _flatten_device(gt, acc, iou_type, category_ids):
                                            _p(nonfinite), _stream(dev)), "dt_coco_results_count")
         scan = torch.cumsum(vals, 1) if nb else None
         totals = scan[:, -1] if nb else torch.zeros((5,), dtype=torch.int64, device=dev)
-        tail = torch.cat([totals, acc._err.to(torch.int64), nonfinite.to(torch.int64)]).cpu().numpy()
-        if tail[5]:
-            b, ncls = acc._where[int(tail[6])]
-            raise RuntimeError("batch_results: the detections of image %d are not grouped by class in 1..%d" % (b, ncls - 1))
-        if tail[7]:
-            raise ValueError("non-finite box or score in the results")
-        N, P, c10, n_kept, n_iou = (int(v) for v in tail[:5])
-        key = torch.empty((max(N, 1),), dtype=torch.int64, device=dev)
-        det_f = torch.empty((max(N, 1), 5), dtype=torch.float64, device=dev)
-        det_i = torch.empty((max(N, 1), 4), dtype=torch.int64, device=dev)
-        pairs = torch.empty((max(P, 1), 7), dtype=torch.int64, device=dev)
-        cat_kept = torch.empty((K + 1,), dtype=torch.int64, device=dev)
-        order_off = torch.empty((3, K + 1), dtype=torch.int64, device=dev)
-        _lib.check(L.dt_coco_results_write(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(scan), _p(gt.keys_d), gt.num_gts, _p(key),
-                                           _p(det_f), _p(det_i), _p(pairs), _p(cat_kept), _p(order_off), _stream(dev)), "dt_coco_results_write")
-    chars = acc._chars if acc._chars is not None else torch.zeros((1,), dtype=torch.uint8, device=dev)
-    return dict(key=key[:N], det_f=det_f[:N], det_i=det_i[:N], pairs=pairs[:P], cat_kept=cat_kept, order_off=order_off, chars=chars,
-                num_chars=acc._num_chars, num_kept=n_kept, num_ious=n_iou, num_order=P + c10 + n_kept)
+        parts = [totals, acc._err.to(torch.int64), nonfinite.to(torch.int64)]
+        if keep_eval_imgs and nb:
+            # the results file's order of the bins: class j = 1, 2, .. (its category's bins, images in sorted-id order)
+            cats = cls_k[1:][cls_k[1:] >= 0].astype(np.int64)
+            cats_d = _pinned_upload(cats, dev)
+            counts = vals[0].view(K, I).index_select(0, cats_d)
+            in_file = torch.cumsum(counts.reshape(-1), 0).view(len(cats), I) - counts
+            file_start = torch.zeros((K, I), dtype=torch.int64, device=dev).index_copy_(0, cats_d, in_file)
+            has = cnt > 0
+            if gt.num_gts:
+                has.index_fill_(0, gt.keys_d, True)
+            union_scan = torch.cumsum(has, 0)
+            out.update(vals=vals, file_start=file_start.view(-1), has=has, union_scan=union_scan)
+            parts.append(union_scan[-1:])
+        elif keep_eval_imgs:
+            parts.append(torch.zeros((1,), dtype=torch.int64, device=dev))
+        out.update(cls_d=cls_d, ord_d=ord_d, scan=scan, tail=torch.cat(parts))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------ proposal recall

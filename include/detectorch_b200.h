@@ -337,6 +337,17 @@ int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, con
                  int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order, const double* gt_f, const int64_t* gt_i,
                  const uint32_t* gt_counts, const double* params, double* precision, double* recall, double* scores, double* ious, void* workspace,
                  dt_stream_t stream);
+/* dt_coco_eval_imgs: COCOeval's per-image records (evalImgs) of the evaluation dt_coco_eval has just enqueued, from its workspace and
+ * IoU matrices (every size argument and table as given to it; ious must not be NULL there).  union_keys [num_union] int64: the sorted
+ * pair indices of the pairs with detections or gts; gt_keys [num_gts] each gt's pair index (sorted).  Outputs, state c = area * 10 +
+ * threshold:  slot_det [kept] int: detection index of each kept slot;  dt_gt [kept, 40] int: index in its pair of the gt a kept detection
+ * matched, -1 none;  dt_ig [kept, 40] uint8: dtIgnore;  gt_dt [num_gts, 40] int: rank in its pair of the last kept detection that matched
+ * the gt, -1 none;  gt_pos [num_gts, 4] int: position in the area's ignore-last gt order;  gt_ig [num_gts, 4] uint8: gtIgnore. */
+int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* union_keys, int num_active, const int64_t* pairs, int64_t num_dets,
+                      const double* det_f, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
+                      const int64_t* gt_keys, const double* gt_f, const int64_t* gt_i, const double* params, const double* ious,
+                      const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos, uint8_t* gt_ig,
+                      dt_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Proposal recall (Detectron's evaluate_box_proposals), bit for bit.  One CTA per (image, combination); every combination of
