@@ -635,9 +635,15 @@ extern "C" int dt_prep_image(const uint8_t* image_hwc, int height, int width, co
         fprintf(stderr, "dt_prep_image: bad argument\n");
         return 0;
     }
-    const double inv_scale = 1.0 / im_scale;
-    // cv::resize: INTER_LINEAR becomes the area-fast kernel when both scale factors are exactly 2
-    const int area2 = (fabs(inv_scale - 2.0) < 2.220446049250313e-16 && out_height * 2 <= height && out_width * 2 <= width) ? 1 : 0;
+    // cv::resize copies the image when dsize == ssize whatever the factor; the linear kernel at scale 1 is that copy
+    const double inv_scale = (out_height == height && out_width == width) ? 1.0 : 1.0 / im_scale;
+    // cv::resize: INTER_LINEAR becomes the area-fast kernel when both scale factors are exactly 2, whatever the image size (the
+    // kernel handles the partial cells of odd sides)
+    const int area2 = fabs(inv_scale - 2.0) < 2.220446049250313e-16 ? 1 : 0;
+    if (area2 && (out_height > (height + 1) / 2 || out_width > (width + 1) / 2)) {
+        fprintf(stderr, "dt_prep_image: a %dx%d output is more than half of the %dx%d image\n", out_height, out_width, height, width);
+        return 0;
+    }
     dim3 grid((blob_width + 255) / 256, blob_height);
     prep_image_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(image_hwc, height, width, pixel_means[0], pixel_means[1], pixel_means[2], inv_scale,
                                                              out_height, out_width, area2, blob_chw, blob_height, blob_width);

@@ -417,7 +417,9 @@ static __global__ void __launch_bounds__(256) segm_paste_kernel(const float* __r
 // lib/utils/blob.py:57-87 prep_im_for_blob (uint8 BGR HWC -> float32, minus the per-channel mean, cv2.resize(fx = fy = im_scale,
 // INTER_LINEAR)) fused with blob.py:27-55 im_list_to_blob (zero-pad to blob_h x blob_w, HWC -> CHW).  The resize is OpenCV's own
 // float kernel: coefficients from scale = 1 / im_scale (the fx/fy form of cv::resize), horizontal then vertical pass with separately
-// rounded products; im_scale == 0.5 takes OpenCV's area-fast path (2x2 box, ((a+b)+c)+d times 0.25f for 3 channels).
+// rounded products; im_scale == 0.5 takes OpenCV's area-fast path (2x2 box, ((a+b)+c)+d times 0.25f for 3 channels).  On an odd side
+// whose half rounds up (cvRound(n / 2) = (n + 1) / 2) the last column / row / corner cell is partial: OpenCV sums its in-range pixels
+// row-major from 0 and divides by their count.
 static __global__ void __launch_bounds__(256) prep_image_kernel(const uint8_t* __restrict__ im, int h, int w, double m0, double m1, double m2,
                                                                 double inv_scale, int out_h, int out_w, int area2,
                                                                 float* __restrict__ blob, int blob_h, int blob_w) {
@@ -430,10 +432,18 @@ static __global__ void __launch_bounds__(256) prep_image_kernel(const uint8_t* _
     const double mean[3] = {m0, m1, m2};
     auto px = [&](int r, int cidx, int c) -> float { return (float)((double)im[((size_t)r * w + cidx) * 3 + c] - mean[c]); };
     if (area2) {
+        const int nr = min(h - 2 * y, 2), nc = min(w - 2 * x, 2);
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            const float a = px(2 * y, 2 * x, c), b = px(2 * y, 2 * x + 1, c), cc = px(2 * y + 1, 2 * x, c), d = px(2 * y + 1, 2 * x + 1, c);
-            o[c * plane] = __fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(a, b), cc), d), 0.25f);
+            if (nr == 2 && nc == 2) {
+                const float a = px(2 * y, 2 * x, c), b = px(2 * y, 2 * x + 1, c), cc = px(2 * y + 1, 2 * x, c), d = px(2 * y + 1, 2 * x + 1, c);
+                o[c * plane] = __fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(a, b), cc), d), 0.25f);
+            } else {
+                float s = 0.f;
+                for (int r = 0; r < nr; ++r)
+                    for (int q = 0; q < nc; ++q) s = __fadd_rn(s, px(2 * y + r, 2 * x + q, c));
+                o[c * plane] = __fdiv_rn(s, (float)(nr * nc));
+            }
         }
         return;
     }

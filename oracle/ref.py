@@ -564,15 +564,30 @@ def segm_results(cls_boxes, masks, ref_boxes, im_h, im_w, num_classes=81, M=14, 
 # ------------------------------------------------------------------------------------------------ image pre-processing (8f rank 3)
 def resize_linear_f32_scale(src, fx):
     """cv2.resize(src float32 HxWxC, None, None, fx=fx, fy=fx, INTER_LINEAR): dsize = cvRound(size * fx), coefficients from
-    scale = 1/fx (not src/dst); fx == 0.5 is routed by OpenCV to its area-fast kernel (for C == 3: ((a+b)+c)+d times 0.25f)."""
+    scale = 1/fx (not src/dst); fx == 0.5 is routed by OpenCV to its area-fast kernel whatever the size: a full 2x2 cell is
+    ((a+b)+c)+d times 0.25f (for C == 3), and the partial cells of an odd side whose half rounds up (the last column, row or
+    corner) are the sum of their in-range pixels, row-major from 0, divided by their count."""
     f32 = np.float32
     src = np.ascontiguousarray(src, dtype=f32)
     sh, sw = src.shape[:2]
     w, h = int(np.rint(sw * fx)), int(np.rint(sh * fx))
     scale = 1.0 / fx
+    if (h, w) == (sh, sw):
+        return src.copy()                                                # cv::resize copies when dsize == ssize, whatever fx
     if abs(scale - 2.0) < np.finfo(np.float64).eps:
-        a, b, c, d = src[0:2 * h:2, 0:2 * w:2], src[0:2 * h:2, 1:2 * w:2], src[1:2 * h:2, 0:2 * w:2], src[1:2 * h:2, 1:2 * w:2]
-        return ((((a + b).astype(f32) + c).astype(f32) + d).astype(f32) * f32(.25)).astype(f32)
+        hf, wf = min(h, sh // 2), min(w, sw // 2)                        # full cells
+        out = np.empty((h, w) + src.shape[2:], f32)
+        a, b, c, d = src[0:2 * hf:2, 0:2 * wf:2], src[0:2 * hf:2, 1:2 * wf:2], src[1:2 * hf:2, 0:2 * wf:2], src[1:2 * hf:2, 1:2 * wf:2]
+        out[:hf, :wf] = ((((a + b).astype(f32) + c).astype(f32) + d).astype(f32) * f32(.25)).astype(f32)
+        for y in range(h):
+            for x in range(wf if y < hf else 0, w):
+                s = np.zeros(src.shape[2:], f32)
+                rows, cols = range(2 * y, min(2 * y + 2, sh)), range(2 * x, min(2 * x + 2, sw))
+                for r in rows:
+                    for q in cols:
+                        s = (s + src[r, q]).astype(f32)
+                out[y, x] = (s / f32(len(rows) * len(cols))).astype(f32)
+        return out
 
     def axis(dst):
         f = ((np.arange(dst, dtype=np.float64) + 0.5) * scale - 0.5).astype(f32)
