@@ -55,7 +55,7 @@ SIGNATURES = {
     "dt_coco_gt_build": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
     "dt_coco_det_check": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "dt_coco_eval_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int64]),
+    "dt_coco_eval_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int]),
     "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                              c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
@@ -64,10 +64,10 @@ SIGNATURES = {
                                   c_void_p, c_void_p]),
     "dt_coco_results_append": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
-    "dt_coco_results_count": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
-                                      c_void_p, c_void_p]),
-    "dt_coco_results_write": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p,
-                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_coco_results_count": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p,
+                                      c_void_p, c_void_p, c_void_p]),
+    "dt_coco_results_write": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                      c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_proposal_recall_smem_bytes": (c_int64, [c_int, c_int64]),
     "dt_proposal_recall": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64,
                                    c_void_p, c_void_p, c_void_p]),

@@ -37,9 +37,11 @@ extern "C" int dt_coco_det_check(int64_t num_dets, const int64_t* det_i, const c
 }
 
 extern "C" int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts,
-                                                int64_t num_order) {
-    if (num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 || num_gts < 0 || num_order < 0) return 0;
-    return (int64_t)coco_eval_ws(num_dets, num_chars, kept, num_ious, num_gts, num_order).total;
+                                                int64_t num_order, int num_cats) {
+    if (num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 || num_gts < 0 || num_order < 0 || num_cats < 0 ||
+        kCocoMaxDets * kept >= (1ll << 31))
+        return 0;
+    return (int64_t)coco_eval_ws(num_dets, num_chars, kept, num_ious, num_gts, num_order, num_cats).total_with_rank;
 }
 
 extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, const int64_t* pairs, const int64_t* cat_gt,
@@ -48,7 +50,8 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
                             const double* gt_f, const int64_t* gt_i, const uint32_t* gt_counts, const double* params, double* precision,
                             double* recall, double* scores, double* ious, void* workspace, dt_stream_t stream) {
     if ((iou_type != 0 && iou_type != 1) || num_images < 0 || num_cats < 0 || num_active < 0 || num_dets < 0 || num_chars < 0 || kept < 0 ||
-        num_ious < 0 || num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || (int64_t)num_cats * 120 >= (1ll << 31)) {
+        num_ious < 0 || num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || (int64_t)num_cats * 120 >= (1ll << 31) ||
+        kCocoMaxDets * kept >= (1ll << 31)) {
         fprintf(stderr, "dt_coco_eval: bad sizes\n");
         return 0;
     }
@@ -102,9 +105,10 @@ extern "C" int dt_coco_results_append(int batch, int cap, int num_classes, const
 }
 
 extern "C" int dt_coco_results_count(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k,
-                                     const int* ord_i, int num_images, int num_cats, const int64_t* gt_keys, int64_t num_gts, int* bin_cnt,
-                                     int64_t* scan_in, int* nonfinite, dt_stream_t stream) {
-    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0) {
+                                     const int* ord_i, int num_images, int num_cats, int cats_per_pair, const int64_t* gt_keys, int64_t num_gts,
+                                     int* bin_cnt, int64_t* scan_in, int* nonfinite, dt_stream_t stream) {
+    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0 || cats_per_pair < 1 ||
+        (cats_per_pair > 1 && num_cats != 1)) {
         fprintf(stderr, "dt_coco_results_count: bad sizes\n");
         return 0;
     }
@@ -113,27 +117,28 @@ extern "C" int dt_coco_results_count(int64_t num_records, const float* rec_f, co
         fprintf(stderr, "dt_coco_results_count: null argument\n");
         return 0;
     }
-    DT_CHECK_CUDA(coco_results_count_launch(num_records, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, gt_keys, num_gts, bin_cnt,
-                                            scan_in, nonfinite, (cudaStream_t)stream));
+    DT_CHECK_CUDA(coco_results_count_launch(num_records, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, cats_per_pair, gt_keys,
+                                            num_gts, bin_cnt, scan_in, nonfinite, (cudaStream_t)stream));
     return 1;
 }
 
 extern "C" int dt_coco_results_write(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k,
-                                     const int* ord_i, int num_images, int num_cats, const int64_t* scan, const int64_t* gt_keys, int64_t num_gts,
-                                     int64_t* det_key, double* det_f, int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off,
-                                     dt_stream_t stream) {
-    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0) {
+                                     const int* ord_i, int num_images, int num_cats, int cats_per_pair, const int* bin_cnt, const int64_t* scan,
+                                     const int64_t* gt_keys, int64_t num_gts, int64_t* det_key, double* det_f, int64_t* det_i, int64_t* pairs,
+                                     int64_t* cat_kept, int64_t* order_off, dt_stream_t stream) {
+    if (num_records < 0 || num_classes < 1 || num_images < 0 || num_cats < 0 || num_gts < 0 || cats_per_pair < 1 ||
+        (cats_per_pair > 1 && num_cats != 1)) {
         fprintf(stderr, "dt_coco_results_write: bad sizes\n");
         return 0;
     }
     const bool bins = (int64_t)num_images * num_cats > 0;
     if ((num_records > 0 && (!rec_f || !rec_i || !cls_k || !ord_i || (bins && (!det_key || !det_f || !det_i)))) || !cat_kept || !order_off ||
-        (bins && (!scan || (num_gts > 0 && !gt_keys)))) {
+        (bins && (!scan || !bin_cnt || (num_gts > 0 && !gt_keys)))) {
         fprintf(stderr, "dt_coco_results_write: null argument\n");
         return 0;
     }
-    DT_CHECK_CUDA(coco_results_write_launch(bins ? num_records : 0, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, scan, gt_keys,
-                                            num_gts, det_key, det_f, det_i, pairs, cat_kept, order_off, (cudaStream_t)stream));
+    DT_CHECK_CUDA(coco_results_write_launch(bins ? num_records : 0, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, cats_per_pair,
+                                            bin_cnt, scan, gt_keys, num_gts, det_key, det_f, det_i, pairs, cat_kept, order_off, (cudaStream_t)stream));
     return 1;
 }
 

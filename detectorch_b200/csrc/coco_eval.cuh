@@ -1,4 +1,4 @@
-// detectorch_b200 -- COCO box and mask evaluation on the device: pycocotools' COCOeval (iouType 'bbox' / 'segm', default Params)
+// detectorch_b200 -- COCO box and mask evaluation on the device: pycocotools' COCOeval (iouType 'bbox' / 'segm', default thresholds)
 // restated kernel by kernel so that precision, recall and scores come out bit for bit as COCOeval.evaluate() + accumulate() give them.
 //
 //   coco_gt_kernel        one CTA per annotation: polygon -> RLE (maskApi rleFrPoly: x5 upsampling, edge walk, y-boundary points,
@@ -8,8 +8,9 @@
 //   coco_pair_kernel      one CTA per (category, image) pair with detections: stable score sort cut to 100 (computeIoU), the IoU
 //                         matrix (bbIou / rleIou, double), then one thread per (area range, IoU threshold) runs evaluateImg's greedy
 //                         matching and writes a 2-bit state (matched, ignored) per detection.
-//   coco_rank_kernel      one thread per kept detection: its position in accumulate()'s stable sort by -score of the category's
-//                         detections concatenated in image order, for each maxDets cut.
+//   coco_rank_*           accumulate()'s stable sort by -score of each category's kept detections, concatenated in image order:
+//                         a stable segmented sort (CUB) of descending score keys per category, then one scan of the maxDets cut
+//                         flags places each detection in the list of every cut it survives.
 //   coco_accum_kernel     one thread per (category, area, maxDets, threshold): cumulative tp / fp, recall, the right-to-left
 //                         precision envelope and searchsorted(rc, recThrs, 'left'), in float64 as numpy computes them.
 //
@@ -18,6 +19,8 @@
 // range in image order, which is the concatenation accumulate() sorts.
 #pragma once
 #include <cstdint>
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 #include <cuda_runtime.h>
 
 namespace dt {
@@ -385,28 +388,43 @@ __global__ void coco_pair_kernel(CocoEvalArgs p) {
     }
 }
 
-// accumulate(): position of each kept detection in the stable -score sort of its category, per maxDets cut.
-// order_off [3][K + 1]: start of category k's list for cut m; cat_kept [K + 1]: the category's kept slots
-__global__ void coco_rank_kernel(int64_t kept, int K, const int64_t* __restrict__ cat_kept, const int64_t* __restrict__ order_off,
-                                 const int* __restrict__ kept_rank, const double* __restrict__ kept_score, int* __restrict__ order) {
+// accumulate(): each kept detection's position in the stable -score sort of its category, per maxDets cut (order_off [3][K + 1]: start
+// of category k's list for cut m; cat_kept [K + 1]: the category's kept slots).  The key sorts ascending as -score does (-0.0 and 0.0
+// equal, as numpy compares them) and the slot index is the value, so a stable sort of each category's slots keeps the concatenation
+// order among equal scores.
+__global__ void coco_rank_keys_kernel(int64_t kept, const double* __restrict__ kept_score, uint64_t* __restrict__ keys, int* __restrict__ vals) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= kept) return;
-    int lo = 0, hi = K - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (cat_kept[mid] <= e) lo = mid; else hi = mid - 1; }
-    const int k = lo;
     const double s = kept_score[e];
-    const int r = kept_rank[e];
-    int64_t pos[kCocoMaxDets] = {0, 0, 0};
-    const int cut[kCocoMaxDets] = {1, 10, 100};
-    for (int64_t j = cat_kept[k]; j < cat_kept[k + 1]; j++) {
-        const double sj = kept_score[j];
-        if ((sj > s) || (sj == s && j < e)) {
-            const int rj = kept_rank[j];
-            pos[0] += rj < cut[0]; pos[1] += rj < cut[1]; pos[2] += rj < cut[2];
-        }
-    }
-    for (int m = 0; m < kCocoMaxDets; m++)
-        if (r < cut[m]) order[order_off[m * (K + 1) + k] + pos[m]] = (int)e;
+    const uint64_t u = s == 0.0 ? 0ull : (uint64_t)__double_as_longlong(s);
+    const uint64_t asc = (u >> 63) ? ~u : (u | (1ull << 63));
+    keys[e] = ~asc;
+    vals[e] = (int)e;
+}
+
+// flags[m * kept + i] = 1 when the i-th slot of the sorted order is inside maxDets cut m.  Their exclusive scan over the three cuts in a
+// row is each surviving slot's index in order[] (cut-major, then category, then sort order: order_off's layout).
+__global__ void coco_rank_flags_kernel(int64_t kept, const int* __restrict__ sorted, const int* __restrict__ kept_rank, int* __restrict__ flags) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= kept) return;
+    const int r = kept_rank[sorted[i]];
+    flags[i] = r < 1; flags[kept + i] = r < 10; flags[2 * kept + i] = r < kCocoKeep;
+}
+
+__global__ void coco_rank_scatter_kernel(int64_t kept, const int* __restrict__ sorted, const int* __restrict__ flags,
+                                         const int* __restrict__ pos, int* __restrict__ order) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= kCocoMaxDets * kept) return;
+    if (flags[i]) order[pos[i]] = sorted[i % kept];
+}
+
+// bytes of CUB temporary storage for the sort of `kept` slots in K categories and the scan of 3 kept flags
+inline size_t coco_rank_temp_bytes(int64_t kept, int K) {
+    size_t sort_b = 0, scan_b = 0;
+    cub::DeviceSegmentedSort::StableSortPairs(nullptr, sort_b, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int*)nullptr, (int*)nullptr,
+                                              (int)kept, K, (const int64_t*)nullptr, (const int64_t*)nullptr);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const int*)nullptr, (int*)nullptr, (int64_t)kCocoMaxDets * kept);
+    return sort_b > scan_b ? sort_b : scan_b;
 }
 
 // one thread per (category, area range, maxDets, threshold).  precision / scores [T, R, K, A, M], recall [T, K, A, M]
@@ -459,10 +477,12 @@ __global__ void coco_accum_kernel(int K, const int64_t* __restrict__ cat_gt, con
 }
 
 // workspace of dt_coco_eval, 256-byte aligned pieces
+// (the rank sort's pieces come last, so the earlier offsets do not depend on the number of categories)
 struct CocoEvalWs {
     size_t det_cnts, det_m, det_area, det_rbox, kept_det, kept_rank, kept_score, state, iou, gtm, order, total;
+    size_t rank_keys, rank_keys_out, rank_vals, rank_sorted, rank_flags, rank_pos, rank_temp, rank_temp_bytes, total_with_rank;
 };
-inline CocoEvalWs coco_eval_ws(int64_t n_det, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt, int64_t n_order) {
+inline CocoEvalWs coco_eval_ws(int64_t n_det, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt, int64_t n_order, int K = 0) {
     CocoEvalWs w;
     size_t o = 0;
     auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) / 256 * 256; return at; };
@@ -478,6 +498,15 @@ inline CocoEvalWs coco_eval_ws(int64_t n_det, int64_t n_chars, int64_t kept, int
     w.gtm = take((size_t)kCocoStates * n_gt);
     w.order = take(4 * (size_t)n_order);
     w.total = o;
+    w.rank_keys = take(8 * (size_t)kept);
+    w.rank_keys_out = take(8 * (size_t)kept);
+    w.rank_vals = take(4 * (size_t)kept);
+    w.rank_sorted = take(4 * (size_t)kept);
+    w.rank_flags = take(4 * (size_t)kCocoMaxDets * kept);
+    w.rank_pos = take(4 * (size_t)kCocoMaxDets * kept);
+    w.rank_temp_bytes = kept > 0 && K > 0 ? coco_rank_temp_bytes(kept, K) : 0;
+    w.rank_temp = take(w.rank_temp_bytes);
+    w.total_with_rank = o;
     return w;
 }
 
@@ -488,12 +517,34 @@ inline cudaError_t coco_gt_launch(int n_ann, const int64_t* ann, const int64_t* 
     return cudaGetLastError();
 }
 
+// accumulate()'s lists for the three maxDets cuts (order[], laid out by order_off) from the kept slots of dt_coco_eval's workspace
+inline cudaError_t coco_rank_launch(int64_t kept, int K, const int64_t* cat_kept, const int* kept_rank, const double* kept_score, int* order,
+                                    uint8_t* ws, const CocoEvalWs& L, cudaStream_t st) {
+    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + L.rank_keys);
+    uint64_t* keys_out = reinterpret_cast<uint64_t*>(ws + L.rank_keys_out);
+    int* vals = reinterpret_cast<int*>(ws + L.rank_vals);
+    int* sorted = reinterpret_cast<int*>(ws + L.rank_sorted);
+    int* flags = reinterpret_cast<int*>(ws + L.rank_flags);
+    int* pos = reinterpret_cast<int*>(ws + L.rank_pos);
+    size_t temp = L.rank_temp_bytes;
+    coco_rank_keys_kernel<<<(unsigned)((kept + 255) / 256), 256, 0, st>>>(kept, kept_score, keys, vals);
+    cudaError_t e = cub::DeviceSegmentedSort::StableSortPairs(ws + L.rank_temp, temp, keys, keys_out, vals, sorted, (int)kept, K, cat_kept,
+                                                              cat_kept + 1, st);
+    if (e != cudaSuccess) return e;
+    coco_rank_flags_kernel<<<(unsigned)((kept + 255) / 256), 256, 0, st>>>(kept, sorted, kept_rank, flags);
+    temp = L.rank_temp_bytes;
+    e = cub::DeviceScan::ExclusiveSum(ws + L.rank_temp, temp, flags, pos, (int64_t)kCocoMaxDets * kept, st);
+    if (e != cudaSuccess) return e;
+    coco_rank_scatter_kernel<<<(unsigned)((kCocoMaxDets * kept + 255) / 256), 256, 0, st>>>(kept, sorted, flags, pos, order);
+    return cudaGetLastError();
+}
+
 inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_active, const int64_t* pairs, const int64_t* cat_gt,
                                     const int64_t* cat_kept, const int64_t* order_off, int64_t n_det, const double* det_f,
                                     const int64_t* det_i, const char* det_chars, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt,
                                     int64_t n_order, const double* gt_f, const int64_t* gt_i, const uint32_t* gt_cnts, const double* par,
                                     double* precision, double* recall, double* scores, double* ious, void* workspace, cudaStream_t st) {
-    const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order);
+    const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order, K);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     CocoEvalArgs p;
     p.segm = segm; p.num_images = num_images; p.pairs = pairs;
@@ -512,7 +563,8 @@ inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_activ
         coco_pair_kernel<<<n_active, 128, 0, st>>>(p);
     }
     if (kept > 0) {
-        coco_rank_kernel<<<(unsigned)((kept + 255) / 256), 256, 0, st>>>(kept, K, cat_kept, order_off, p.kept_rank, p.kept_score, order);
+        cudaError_t e = coco_rank_launch(kept, K, cat_kept, p.kept_rank, p.kept_score, order, ws, L, st);
+        if (e != cudaSuccess) return e;
     }
     const int cells = K * kCocoAreas * kCocoMaxDets * kCocoThrs;
     if (cells > 0) {
@@ -536,6 +588,12 @@ inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_activ
 //                                cat_kept and order_off from the scans at the category's first bin.
 // Each (category, image) bin is filled by one class of one image (category ids are distinct), so no two groups share a bin and the
 // only atomics are the integer error flags.
+//
+// Subsets and class-agnostic evaluation (COCOeval's imgIds, catIds, useCats) only change the maps: cls_k takes a class to its category
+// slot or -1, ord_i an image ordinal to its image index or -1 (records mapped to -1 take no part).  With `per` category slots per pair
+// (useCats = 0: the evaluated categories, in COCOeval's concatenation order; otherwise 1) the records are counted in per * P fine bins,
+// fine bin = image * per + slot (per > 1) or slot * I + image (per = 1), and pair p holds fine bins p * per .. p * per + per - 1 in a row,
+// so its detections come in concatenation order.
 // record: f32 [x1, y1, x2, y2, score]; i64 [image ordinal (-1: dead slot), class, rank in class, char offset, char count, h, w]
 constexpr int kCocoRecF = 5, kCocoRecI = 7;
 // the bin scans, int64 [5][K I] inclusive: D, D > 0 (= min(D, 1)), min(D, 10), min(D, 100), min(D, 100) G
@@ -594,27 +652,32 @@ __device__ __forceinline__ int coco_rec_cat(const int64_t* R, int num_cls, const
     return cls_k[c];
 }
 
+__device__ __forceinline__ int64_t coco_fine_bin(int k, int i, int I, int per) {
+    return per > 1 ? (int64_t)i * per + k : (int64_t)k * I + i;
+}
+
 __global__ void coco_results_count_kernel(int64_t n, const float* __restrict__ rec_f, const int64_t* __restrict__ rec_i, int num_cls,
-                                          const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, int* __restrict__ bin_cnt,
+                                          const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, int per, int* __restrict__ bin_cnt,
                                           int* __restrict__ nonfinite) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     const int64_t* R = rec_i + r * kCocoRecI;
     const int k = coco_rec_cat(R, num_cls, cls_k);
-    if (k < 0) return;
+    if (k < 0 || ord_i[R[0]] < 0) return;
     const float* F = rec_f + r * kCocoRecF;
     bool fin = true;
     for (int j = 0; j < kCocoRecF; j++) fin = fin && isfinite(F[j]);
     if (!fin) atomicOr(nonfinite, 1);
     const bool last = r + 1 == n || R[kCocoRecI] != R[0] || R[kCocoRecI + 1] != R[1];
-    if (last) bin_cnt[(int64_t)k * I + ord_i[R[0]]] = (int)R[2] + 1;
+    if (last) bin_cnt[coco_fine_bin(k, ord_i[R[0]], I, per)] = (int)R[2] + 1;
 }
 
-__global__ void coco_results_bins_kernel(int64_t nb, const int* __restrict__ bin_cnt, const int64_t* __restrict__ gt_keys, int64_t G,
+__global__ void coco_results_bins_kernel(int64_t nb, int per, const int* __restrict__ bin_cnt, const int64_t* __restrict__ gt_keys, int64_t G,
                                          int64_t* __restrict__ vals) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
-    const int64_t D = bin_cnt[b];
+    int64_t D = 0;
+    for (int c = 0; c < per; c++) D += bin_cnt[b * per + c];
     int64_t gn = 0;
     if (D > 0) gn = coco_lower_bound(gt_keys, G, b, true) - coco_lower_bound(gt_keys, G, b, false);
     const int64_t kept = D < kCocoKeep ? D : kCocoKeep;
@@ -626,16 +689,19 @@ __global__ void coco_results_bins_kernel(int64_t nb, const int* __restrict__ bin
 }
 
 // det_f: (score, x1, y1, x2 - x1 + 1, y2 - y1 + 1), each term the double of the stored float, as the host's float64 arithmetic
+// det_key: each row's fine bin (its pair when per = 1)
 __global__ void coco_results_scatter_kernel(int64_t n, const float* __restrict__ rec_f, const int64_t* __restrict__ rec_i, int num_cls,
-                                            const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, const int64_t* __restrict__ scan,
-                                            int64_t* __restrict__ det_key, double* __restrict__ det_f, int64_t* __restrict__ det_i) {
+                                            const int* __restrict__ cls_k, const int* __restrict__ ord_i, int I, int per,
+                                            const int* __restrict__ bin_cnt, const int64_t* __restrict__ scan, int64_t* __restrict__ det_key,
+                                            double* __restrict__ det_f, int64_t* __restrict__ det_i) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     const int64_t* R = rec_i + r * kCocoRecI;
     const int k = coco_rec_cat(R, num_cls, cls_k);
-    if (k < 0) return;
-    const int64_t key = (int64_t)k * I + ord_i[R[0]];
-    const int64_t pos = (key > 0 ? scan[key - 1] : 0) + R[2];
+    if (k < 0 || ord_i[R[0]] < 0) return;
+    const int64_t key = coco_fine_bin(k, ord_i[R[0]], I, per), b = key / per;
+    int64_t pos = (b > 0 ? scan[b - 1] : 0) + R[2];
+    for (int64_t f = b * per; f < key; f++) pos += bin_cnt[f];
     const float* F = rec_f + r * kCocoRecF;
     const double x1 = F[0], y1 = F[1], x2 = F[2], y2 = F[3];
     double* D = det_f + pos * kCocoDetF;
@@ -679,19 +745,21 @@ inline cudaError_t coco_results_append_launch(int B, int cap, int num_classes, c
 }
 
 inline cudaError_t coco_results_count_launch(int64_t n, const float* rec_f, const int64_t* rec_i, int num_cls, const int* cls_k, const int* ord_i,
-                                             int I, int K, const int64_t* gt_keys, int64_t G, int* bin_cnt, int64_t* vals, int* nonfinite,
+                                             int I, int K, int per, const int64_t* gt_keys, int64_t G, int* bin_cnt, int64_t* vals, int* nonfinite,
                                              cudaStream_t st) {
     const int64_t nb = (int64_t)K * I;
-    if (n > 0) coco_results_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, bin_cnt, nonfinite);
-    if (nb > 0) coco_results_bins_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(nb, bin_cnt, gt_keys, G, vals);
+    if (n > 0) coco_results_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, per, bin_cnt, nonfinite);
+    if (nb > 0) coco_results_bins_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(nb, per, bin_cnt, gt_keys, G, vals);
     return cudaGetLastError();
 }
 
 inline cudaError_t coco_results_write_launch(int64_t n, const float* rec_f, const int64_t* rec_i, int num_cls, const int* cls_k, const int* ord_i,
-                                             int I, int K, const int64_t* scan, const int64_t* gt_keys, int64_t G, int64_t* det_key, double* det_f,
-                                             int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off, cudaStream_t st) {
+                                             int I, int K, int per, const int* bin_cnt, const int64_t* scan, const int64_t* gt_keys, int64_t G,
+                                             int64_t* det_key, double* det_f, int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off,
+                                             cudaStream_t st) {
     const int64_t nb = (int64_t)K * I, nt = nb > K + 1 ? nb : K + 1;
-    if (n > 0) coco_results_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, scan, det_key, det_f, det_i);
+    if (n > 0) coco_results_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, rec_f, rec_i, num_cls, cls_k, ord_i, I, per, bin_cnt, scan,
+                                                                                      det_key, det_f, det_i);
     coco_results_pairs_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(K, I, scan, gt_keys, G, pairs, cat_kept, order_off);
     return cudaGetLastError();
 }

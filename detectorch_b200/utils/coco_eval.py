@@ -1,11 +1,12 @@
-"""COCO box and mask evaluation on the device: pycocotools' COCOeval ('bbox' / 'segm', default Params) without its per-(image,
-category) Python loops.  Precision, recall and scores are bit-identical to COCOeval.evaluate() + accumulate() run on the results
+"""COCO box and mask evaluation on the device: pycocotools' COCOeval ('bbox' / 'segm'; its default thresholds, area ranges and maxDets,
+any imgIds / catIds / useCats) without its per-(image, category) Python loops.  Precision, recall and scores are bit-identical to COCOeval.evaluate() + accumulate() run on the results
 file that lib/utils/json_dataset_evaluator.py would write; no file is written.
 
     gt = CocoGroundTruth("instances_minival2014.json")   # or the annotation dict; GT masks are built once, on the device
     E = evaluate(gt, detector.detect_images(ims), "segm")  # or evaluate(gt, all_boxes, "bbox") / evaluate(gt, all_boxes, "segm", all_segms)
     E.stats, E.eval["precision"]                          # summarize()'s 12 numbers, [T, R, K, A, M]
     acc = DeviceResults(); acc.add(detector.detect(...), image_ids, original_sizes=orig); evaluate(gt, acc, "segm")   # no host copy
+    p = Params(gt, "bbox"); p.imgIds = ids[:500]; p.useCats = 0; E = evaluate(gt, results, "bbox", params=p)   # subsets, class-agnostic
     E = evaluate(gt, results, "bbox", keep_eval_imgs=True)  # + COCOeval's per-image records:
     E.eval_imgs["dtMatches"], E.evalImgs[n]               # as flat columns, or as COCOeval's list of dicts (built when first read)
 
@@ -363,13 +364,113 @@ class CocoGroundTruth:
 
 
 class Params:
-    """The parts of COCOeval's Params that evaluation results refer to."""
+    """COCOeval's Params for 'bbox' / 'segm', with gt's images and categories.  evaluate(..., params=) takes one edited as on a COCOeval
+    object: imgIds (a subset of the images), catIds (a subset of the categories) and useCats (0: class-agnostic matching).  iouThrs,
+    recThrs, maxDets, areaRng and areaRngLbl must keep their defaults."""
 
     def __init__(self, gt, iou_type):
         self.imgIds, self.catIds = list(gt.img_ids), list(gt.cat_ids)
         self.iouThrs, self.recThrs = IOU_THRS.copy(), REC_THRS.copy()
         self.maxDets, self.areaRng, self.areaRngLbl = list(MAX_DETS), [list(a) for a in AREA_RNG], list(AREA_LBL)
         self.useCats, self.iouType = 1, iou_type
+
+
+def _id_list(v, what, known):
+    if isinstance(v, (str, bytes)) or not hasattr(v, '__len__'):
+        raise ValueError("params.%s must be a list of ids" % what)
+    ids = [_int(x, "params.%s entry" % what) for x in v]
+    if not ids:
+        raise ValueError("params.%s is empty" % what)
+    bad = [x for x in ids if x not in known]
+    if bad:
+        raise ValueError("params.%s: %d is not in the ground truth" % (what, bad[0]))
+    return ids
+
+
+def _same(a, b):
+    try:
+        a = np.asarray(a, np.float64)
+    except (TypeError, ValueError):
+        return False
+    return a.shape == np.shape(b) and np.array_equal(a, b)
+
+
+def _normalised_params(gt, params, iou_type):
+    """Checks params on the host and returns a copy normalised as COCOeval.evaluate() normalises it: imgIds unique and sorted, catIds
+    too when useCats is 1 (with useCats 0 their order is the order in which each image's categories are concatenated), maxDets sorted."""
+    if not isinstance(params, Params):
+        raise ValueError("params must be a coco_eval.Params")
+    if params.iouType != iou_type:
+        raise ValueError("params.iouType is %r, the evaluation is %r" % (params.iouType, iou_type))
+    if not _same(params.iouThrs, IOU_THRS):
+        raise ValueError("params.iouThrs: only COCOeval's default IoU thresholds are supported")
+    if not _same(params.recThrs, REC_THRS):
+        raise ValueError("params.recThrs: only COCOeval's default recall thresholds are supported")
+    if not (isinstance(params.maxDets, (list, tuple)) and _same(sorted(params.maxDets), MAX_DETS)):
+        raise ValueError("params.maxDets: only COCOeval's default [1, 10, 100] is supported")
+    if not _same(params.areaRng, AREA_RNG) or list(params.areaRngLbl) != AREA_LBL:
+        raise ValueError("params.areaRng / areaRngLbl: only COCOeval's default area ranges are supported")
+    if isinstance(params.useCats, float) or params.useCats not in (0, 1):
+        raise ValueError("params.useCats must be 0 or 1, got %r" % (params.useCats,))
+    p = Params(gt, iou_type)
+    p.useCats = int(params.useCats)
+    p.imgIds = [int(v) for v in np.unique(_id_list(params.imgIds, 'imgIds', gt.image_hw))]
+    cats = _id_list(params.catIds, 'catIds', set(gt.cat_ids))
+    if p.useCats:
+        cats = [int(v) for v in np.unique(cats)]
+    elif len(set(cats)) != len(cats):
+        raise ValueError("params.catIds: a category is repeated (with useCats 0 its ground truth would count twice)")
+    p.catIds = cats
+    return p
+
+
+def _is_default(gt, p):
+    return p.useCats == 1 and p.imgIds == list(gt.img_ids) and p.catIds == list(gt.cat_ids)
+
+
+class _GtView:
+    """The ground truth re-indexed for a Params: the evaluated images and categories (one category, -1, when useCats is 0), pair keys
+    over them, and the gt rows of those pairs gathered on the device (the masks stay where CocoGroundTruth built them).  It has the
+    attributes of CocoGroundTruth that the evaluation reads.  per: category slots per pair (with useCats 0 the evaluated categories, in
+    the order COCOeval concatenates them per image; else 1); cat_slot / img_slot: each category / image index of gt to its slot / index
+    here, -1 when it takes no part."""
+
+    def __init__(self, gt, p):
+        self.device, self.has_masks, self.gt_counts = gt.device, gt.has_masks, gt.gt_counts
+        self.img_ids = list(p.imgIds)
+        self.cat_ids = list(p.catIds) if p.useCats else [-1]
+        self.num_images, self.num_cats = len(self.img_ids), len(self.cat_ids)
+        self.per = 1 if p.useCats else len(p.catIds)
+        cat_index = {v: n for n, v in enumerate(gt.cat_ids)}
+        img_index = {v: n for n, v in enumerate(gt.img_ids)}
+        self.cat_slot = np.full(gt.num_cats, -1, np.int64)
+        self.cat_slot[[cat_index[c] for c in p.catIds]] = np.arange(len(p.catIds))
+        self.img_slot = np.full(gt.num_images, -1, np.int64)
+        self.img_slot[[img_index[i] for i in p.imgIds]] = np.arange(self.num_images)
+        self.I0 = gt.num_images
+        rows, fine = self.select(gt.keys)
+        self.rows = rows
+        self.keys = fine // self.per
+        self.num_gts = len(rows)
+        self.ann_ids = [gt.ann_ids[r] for r in rows]
+        self.cat_gt = np.searchsorted(self.keys // max(self.num_images, 1), np.arange(self.num_cats + 1)).astype(np.int64)
+        rows_d = torch.from_numpy(rows).to(gt.device)
+        self.gt_f, self.gt_i = gt.gt_f.index_select(0, rows_d), gt.gt_i.index_select(0, rows_d)
+        self.keys_d = torch.from_numpy(self.keys).to(gt.device)
+
+    def fine_key(self, k, i):
+        """(category slot, image index) -> fine bin (csrc/coco_eval.cuh): pairs in a row, each pair's slots in concatenation order."""
+        return i * self.per + k if self.per > 1 else k * self.num_images + i
+
+    def select(self, key):
+        """Rows keyed as gt keys them (category index * images + image index, sorted; rows of a key in their order) -> the rows that take
+        part, in this view's order (stable), and their fine bins."""
+        I0 = max(self.I0, 1)
+        k, i = self.cat_slot[key // I0], self.img_slot[key % I0]
+        rows = np.flatnonzero((k >= 0) & (i >= 0))
+        fine = self.fine_key(k[rows], i[rows])
+        o = np.argsort(fine, kind='stable')
+        return rows[o], fine[o]
 
 
 class CocoEvalResult:
@@ -524,14 +625,19 @@ def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids, with_ids=
     return key[order], det_f[order], det_i[order], chars
 
 
-def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False, keep_eval_imgs=False):
+def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False, keep_eval_imgs=False, params=None):
     """COCOeval(gt, loadRes(results file), iou_type).evaluate() + accumulate() on the device -> CocoEvalResult.
     results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), the notebooks' all_boxes
     [class][image] (with all_segms [class][image] for 'segm'), or a DeviceResults (flattened on the device, on gt's device).  category_ids: json id of contiguous class j (1-based) at j - 1;
     default: the dataset's category order, as JsonDataset builds its classes.  keep_ious: also return COCOeval's .ious, {(image id,
     category id): [min(D, 100), G] array} for the pairs with detections and GTs.  keep_eval_imgs: also return COCOeval's per-image
     records, as .eval_imgs (columns, see _eval_imgs_columns) and .evalImgs (the list of dicts, built from the columns when first read);
-    detection ids are the ones loadRes gives the results file's rows, 1 + the row's index."""
+    detection ids are the ones loadRes gives the results file's rows, 1 + the row's index.
+    params: a Params (Params(gt, iou_type), then edited) whose imgIds, catIds and useCats are evaluated as COCOeval evaluates them:
+    only the listed images' and categories' gts and detections take part (detections on other images are left out), and with useCats 0
+    each image's detections and gts of all listed categories are matched together (one category, -1, as accumulate() makes it).  The
+    other fields must keep their defaults.  Bad params raise ValueError before anything is launched; the result's .params is the
+    one used, normalised as COCOeval.evaluate() normalises it.  None: the defaults."""
     if iou_type not in ('bbox', 'segm'):
         raise ValueError("iou_type must be 'bbox' or 'segm'")
     if not isinstance(gt, CocoGroundTruth):
@@ -541,16 +647,22 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
     category_ids = list(gt.category_ids if category_ids is None else category_ids)
     if any(c not in set(gt.cat_ids) for c in category_ids):
         raise ValueError("category_ids names a category the ground truth does not have")
+    p = Params(gt, iou_type) if params is None else _normalised_params(gt, params, iou_type)
+    view = None if _is_default(gt, p) else _GtView(gt, p)
+    ev = gt if view is None else view
     if isinstance(results, DeviceResults):
         if all_segms is not None:
             raise ValueError("a DeviceResults carries its masks; all_segms is for all_boxes input")
-        f = _flatten_device(gt, results, iou_type, category_ids, keep_eval_imgs)
+        f = _flatten_device(gt, results, iou_type, category_ids, keep_eval_imgs, view)
         imgs = (f['union'], f['det_ids']) if keep_eval_imgs else None
-        return _evaluate_tables(gt, iou_type, None, f['pairs'], f['cat_kept'], f['order_off'], f['det_f'], f['det_i'], f['chars'],
-                                f['num_chars'], f['num_kept'], f['num_ious'], f['num_order'], keep_ious, imgs)
+        return _evaluate_tables(ev, iou_type, None, f['pairs'], f['cat_kept'], f['order_off'], f['det_f'], f['det_i'], f['chars'],
+                                f['num_chars'], f['num_kept'], f['num_ious'], f['num_order'], keep_ious, imgs, p)
     boxes, segms = _per_class(gt, results, all_segms, iou_type)
     key, det_f, det_i, chars, det_ids = _flatten_results(gt, boxes, segms, iou_type, category_ids, with_ids=True)
-    pairs, cat_kept, order_off = _pair_tables(gt, key)
+    if view is not None:
+        rows, fine = view.select(key)
+        key, det_f, det_i, det_ids = fine // view.per, det_f[rows], det_i[rows], det_ids[rows]
+    pairs, cat_kept, order_off = _pair_tables(ev, key)
     kept, gn = np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
     n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(order_off[-1, -1])
     dev = gt.device
@@ -559,8 +671,8 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
     imgs = None
     if keep_eval_imgs:
         # the pairs COCOeval keeps a record of: those with detections and those with gts
-        imgs = tuple(torch.from_numpy(x).to(dev) for x in (np.union1d(pairs[:, 0], gt.keys).astype(np.int64), det_ids.astype(np.int64)))
-    return _evaluate_tables(gt, iou_type, pairs, *up, ch, len(chars), n_kept, n_iou, n_order, keep_ious, imgs)
+        imgs = tuple(torch.from_numpy(x).to(dev) for x in (np.union1d(pairs[:, 0], ev.keys).astype(np.int64), det_ids.astype(np.int64)))
+    return _evaluate_tables(ev, iou_type, pairs, *up, ch, len(chars), n_kept, n_iou, n_order, keep_ious, imgs, p)
 
 
 def _pair_tables(gt, key):
@@ -587,9 +699,10 @@ def _pair_tables(gt, key):
 
 
 def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_f_d, det_i_d, ch, num_chars, n_kept, n_iou, n_order, keep_ious,
-                     imgs=None):
+                     imgs, params):
     """dt_coco_eval on the flattened results, already on gt's device (pairs: their host copy, or None to read it back for keep_ious).
-    imgs: (union keys [Q], detection ids [N]) on the device to also run dt_coco_eval_imgs, None to leave it out."""
+    gt: the CocoGroundTruth, or its _GtView for params.  imgs: (union keys [Q], detection ids [N]) on the device to also run
+    dt_coco_eval_imgs, None to leave it out."""
     I, K, N = gt.num_images, gt.num_cats, int(det_f_d.shape[0])
     dev = gt.device
     T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
@@ -607,7 +720,10 @@ def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_
             raise ValueError("results: RLE counts of result %d (in (category, image) order) do not sum to h * w" % nb[0])
     # the records read the IoU matrices dt_coco_eval keeps, rather than computing them again
     ious = torch.empty((max(n_iou, 1),), dtype=torch.float64, device=dev) if keep_ious or imgs is not None else None
-    ws = torch.empty((max(L.dt_coco_eval_workspace_bytes(N, num_chars, n_kept, n_iou, gt.num_gts, n_order), 1),), dtype=torch.uint8, device=dev)
+    ws_bytes = L.dt_coco_eval_workspace_bytes(N, num_chars, n_kept, n_iou, gt.num_gts, n_order, K)
+    if ws_bytes <= 0 and N:
+        raise ValueError("evaluate: %d kept detections are more than the evaluation can rank" % n_kept)
+    ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
     _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, int(pairs_d.shape[0]), _p(pairs_d), _p(cat_gt_d), _p(cat_kept_d),
                               _p(order_off_d), N, _p(det_f_d), _p(det_i_d), _p(ch), num_chars, n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f),
                               _p(gt.gt_i), _p(gt.gt_counts), _p(par_d), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
@@ -628,7 +744,7 @@ def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_
         slot_id, slot_score = det_ids_d[sd], det_f_d[sd, 0]
         dev_out = dict(ukeys=ukeys_d, slot_id=slot_id, slot_score=slot_score, dt_gt=dt_gt[:n_kept], dt_ig=dt_ig[:n_kept], gt_dt=gt_dt[:G],
                        gt_pos=gt_pos[:G], gt_ig=gt_ig[:G])
-    E = CocoEvalResult(Params(gt, iou_type), prec.cpu().numpy(), rec.cpu().numpy(), scr.cpu().numpy())
+    E = CocoEvalResult(params, prec.cpu().numpy(), rec.cpu().numpy(), scr.cpu().numpy())
     if (keep_ious or imgs is not None) and pairs is None:
         pairs = pairs_d.cpu().numpy()
     if imgs is not None:
@@ -695,7 +811,7 @@ def _eval_imgs_columns(gt, pairs, o):
 def _eval_imgs_list(params, c):
     """The columns of _eval_imgs_columns -> COCOeval.evalImgs, a list of K * 4 * I dicts or None.  The arrays of a record are views of
     the columns."""
-    out = [None] * (len(params.catIds) * len(params.areaRng) * len(params.imgIds))
+    out = [None] * ((len(params.catIds) if params.useCats else 1) * len(params.areaRng) * len(params.imgIds))
     dt_off, gt_off = c['dt_off'].tolist(), c['gt_off'].tolist()
     dt_ids, dt_scores, gt_ids = c['dtIds'].tolist(), c['dtScores'].tolist(), c['gtIds'].tolist()
     dm, di, gm, gi = c['dtMatches'], c['dtIgnore'], c['gtMatches'], c['gtIgnore']
@@ -910,14 +1026,16 @@ class DeviceResults:
         self._all_masks = self._all_masks and masks is not None
 
 
-def _flatten_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
+def _flatten_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False, view=None):
     """_flatten_results + _pair_tables for a DeviceResults, on the device: -> dict of device tensors key [N], det_f [N, 5], det_i [N, 4]
     (char offsets into acc's buffer `chars`), pairs [P, 7], cat_kept [K + 1], order_off [3, K + 1], and the sizes dt_coco_eval takes.
     Host checks raise ValueError before anything is launched; the device's error flags come back with the sizes, in one copy.
     keep_eval_imgs adds det_ids [N] (loadRes ids, as with_ids of _flatten_results) and union [Q], the sorted keys of the pairs with
-    detections or gts."""
-    b = _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs)
-    I, K, nb, dev = gt.num_images, gt.num_cats, gt.num_images * gt.num_cats, gt.device
+    detections or gts.  view: the _GtView of a Params (None: the default), whose images, categories and pairs the tables are over."""
+    b = _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs, view)
+    ev = gt if view is None else view
+    per = 1 if view is None else view.per
+    I, K, nb, dev = ev.num_images, ev.num_cats, ev.num_images * ev.num_cats, gt.device
     n, nc, rec_f, rec_i, cls_d, ord_d, scan = b['n'], b['nc'], b['rec_f'], b['rec_i'], b['cls_d'], b['ord_d'], b['scan']
     L = _lib.lib()
     with torch.cuda.device(dev):
@@ -934,15 +1052,20 @@ def _flatten_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
         pairs = torch.empty((max(P, 1), 7), dtype=torch.int64, device=dev)
         cat_kept = torch.empty((K + 1,), dtype=torch.int64, device=dev)
         order_off = torch.empty((3, K + 1), dtype=torch.int64, device=dev)
-        _lib.check(L.dt_coco_results_write(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(scan), _p(gt.keys_d), gt.num_gts, _p(key),
-                                           _p(det_f), _p(det_i), _p(pairs), _p(cat_kept), _p(order_off), _stream(dev)), "dt_coco_results_write")
+        _lib.check(L.dt_coco_results_write(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, per, _p(b['cnt']), _p(scan), _p(ev.keys_d),
+                                           ev.num_gts, _p(key), _p(det_f), _p(det_i), _p(pairs), _p(cat_kept), _p(order_off), _stream(dev)),
+                   "dt_coco_results_write")
         extra = {}
         if keep_eval_imgs:
             # row n of key k is file row file_start[k] + (n - first row of k); the union's keys are compacted by their scan
             Q = int(tail[8])
             if nb:
                 k = key[:N]
-                first = scan[0] - b['vals'][0]
+                if view is None:
+                    first = scan[0] - b['vals'][0]
+                else:                           # rows are in fine bin order; key holds each row's fine bin
+                    cnt = b['cnt'].to(torch.int64)
+                    first = torch.cumsum(cnt, 0) - cnt
                 extra['det_ids'] = torch.arange(N, device=dev) - first[k] + b['file_start'][k] + 1
                 dst = torch.where(b['has'], b['union_scan'] - 1, nb)
                 union = torch.empty((nb + 1,), dtype=torch.int64, device=dev)         # slot nb takes the bins left out
@@ -954,11 +1077,12 @@ def _flatten_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
                 num_chars=acc._num_chars, num_kept=n_kept, num_ious=n_iou, num_order=P + c10 + n_kept, **extra)
 
 
-def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
+def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False, view=None):
     """_flatten_device up to its one read-back, without a host synchronisation: the host checks, the counting pass and the bin scans;
     -> dict of the tables the write pass takes and `tail`, the device vector of sizes and flags to read back.  keep_eval_imgs adds
     each bin's first row in the results file (file_start: class-major, images in sorted-id order, the scan of the bins' counts in
-    that order), the bins that have detections or gts (has) and their inclusive scan, whose total ends `tail`."""
+    that order), the bins that have detections or gts (has) and their inclusive scan, whose total ends `tail`.  With a view, the bins
+    are its fine bins (cnt), the scans over its pairs, and file_start is per fine bin, counted over every record of the results file."""
     if acc.device != gt.device:
         raise ValueError("the results are on %s, the ground truth on %s" % (acc.device, gt.device))
     if iou_type == 'segm' and not acc._all_masks:
@@ -975,7 +1099,11 @@ def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
     cls_k = np.full(nc, -1, np.int32)
     for j in range(1, min(len(category_ids) + 1, nc)):        # classes past category_ids are dropped, as the host loop's break drops them
         cls_k[j] = cat_index[category_ids[j - 1]]
-    I, K = gt.num_images, gt.num_cats
+    ev, per = (gt, 1) if view is None else (view, view.per)
+    if view is not None:                # the maps of the view: category slot of each class, image index of each ordinal (-1: left out)
+        cls_v = np.where(cls_k >= 0, view.cat_slot[np.maximum(cls_k, 0)], -1).astype(np.int32)
+        ord_v = view.img_slot[ord_i].astype(np.int32) if acc.image_ids else ord_i
+    I, K = ev.num_images, ev.num_cats
     nb, n, dev = I * K, acc._num_records, gt.device
     acc._drain()                        # every masked batch settled (and redone if it overflowed) before its records are read
     L = _lib.lib()
@@ -984,29 +1112,47 @@ def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False):
     with torch.cuda.device(dev):
         cls_d, ord_d = _pinned_upload(cls_k, dev), _pinned_upload(ord_i, dev)
         nonfinite = torch.zeros((1,), dtype=torch.int32, device=dev)
-        cnt = torch.zeros((nb,), dtype=torch.int32, device=dev) if nb else None
+        if view is not None:
+            full = (cls_d, ord_d)
+            cls_d, ord_d = _pinned_upload(cls_v, dev), _pinned_upload(ord_v, dev)
+        cnt = torch.zeros((nb * per,), dtype=torch.int32, device=dev) if nb else None
         vals = torch.empty((5, nb), dtype=torch.int64, device=dev) if nb else None
-        _lib.check(L.dt_coco_results_count(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, _p(gt.keys_d), gt.num_gts, _p(cnt), _p(vals),
-                                           _p(nonfinite), _stream(dev)), "dt_coco_results_count")
+        _lib.check(L.dt_coco_results_count(n, _p(rec_f), _p(rec_i), nc, _p(cls_d), _p(ord_d), I, K, per, _p(ev.keys_d), ev.num_gts, _p(cnt),
+                                           _p(vals), _p(nonfinite), _stream(dev)), "dt_coco_results_count")
         scan = torch.cumsum(vals, 1) if nb else None
         totals = scan[:, -1] if nb else torch.zeros((5,), dtype=torch.int64, device=dev)
         parts = [totals, acc._err.to(torch.int64), nonfinite.to(torch.int64)]
         if keep_eval_imgs and nb:
             # the results file's order of the bins: class j = 1, 2, .. (its category's bins, images in sorted-id order)
+            K0, I0 = gt.num_cats, gt.num_images
             cats = cls_k[1:][cls_k[1:] >= 0].astype(np.int64)
             cats_d = _pinned_upload(cats, dev)
-            counts = vals[0].view(K, I).index_select(0, cats_d)
-            in_file = torch.cumsum(counts.reshape(-1), 0).view(len(cats), I) - counts
-            file_start = torch.zeros((K, I), dtype=torch.int64, device=dev).index_copy_(0, cats_d, in_file)
-            has = cnt > 0
-            if gt.num_gts:
-                has.index_fill_(0, gt.keys_d, True)
+            if view is None:
+                counts = vals[0].view(K, I).index_select(0, cats_d)
+            else:                   # the file holds every record: its bins are counted over all of gt's images and categories
+                cnt0 = torch.zeros((K0 * I0,), dtype=torch.int32, device=dev)
+                vals0 = torch.empty((5, K0 * I0), dtype=torch.int64, device=dev)
+                _lib.check(L.dt_coco_results_count(n, _p(rec_f), _p(rec_i), nc, _p(full[0]), _p(full[1]), I0, K0, 1, _p(gt.keys_d), gt.num_gts,
+                                                   _p(cnt0), _p(vals0), _p(torch.zeros_like(nonfinite)), _stream(dev)), "dt_coco_results_count")
+                counts = cnt0.to(torch.int64).view(K0, I0).index_select(0, cats_d)
+            in_file = torch.cumsum(counts.reshape(-1), 0).view(len(cats), I0) - counts
+            file_start = torch.zeros((K0, I0), dtype=torch.int64, device=dev).index_copy_(0, cats_d, in_file).view(-1)
+            if view is not None:    # each fine bin's (category, image) of gt
+                ks, ims = np.flatnonzero(view.cat_slot >= 0), np.flatnonzero(view.img_slot >= 0)
+                kk, ii = np.meshgrid(ks, ims, indexing='ij')
+                fine = view.fine_key(view.cat_slot[kk], view.img_slot[ii]).reshape(-1)
+                src = np.empty(nb * per, np.int64)
+                src[fine] = (kk * I0 + ii).reshape(-1)
+                file_start = file_start.index_select(0, _pinned_upload(src, dev))
+            has = vals[1] > 0
+            if ev.num_gts:
+                has.index_fill_(0, ev.keys_d, True)
             union_scan = torch.cumsum(has, 0)
-            out.update(vals=vals, file_start=file_start.view(-1), has=has, union_scan=union_scan)
+            out.update(vals=vals, file_start=file_start, has=has, union_scan=union_scan)
             parts.append(union_scan[-1:])
         elif keep_eval_imgs:
             parts.append(torch.zeros((1,), dtype=torch.int64, device=dev))
-        out.update(cls_d=cls_d, ord_d=ord_d, scan=scan, tail=torch.cat(parts))
+        out.update(cls_d=cls_d, ord_d=ord_d, scan=scan, cnt=cnt, tail=torch.cat(parts))
     return out
 
 

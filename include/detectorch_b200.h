@@ -287,7 +287,7 @@ int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_fact
                       float* ms_out, double* flops_out, int* stage_out, int* block_n_out, int cap);
 
 /* ---------------------------------------------------------------------------------------------
- * COCO box / mask evaluation (pycocotools COCOeval, iouType 'bbox' or 'segm', default Params), bit for bit.
+ * COCO box / mask evaluation (pycocotools COCOeval, iouType 'bbox' or 'segm'; the default thresholds, area ranges and maxDets), bit for bit.
  * Table layouts are the constants at the top of detectorch_b200/csrc/coco_eval.cuh.
  * dt_coco_gt_build: ground-truth masks -> RLE, one CTA per annotation.
  *   anns [num_anns, 6] int64      kind (0 polygon parts, 1 uncompressed counts, 2 compressed string), h, w, first part, parts, output offset
@@ -313,25 +313,30 @@ int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_fact
  *   append: boxes [B, cap, 4], scores [B, cap] float, classes [B, cap], counts [B] int; images [B, 3] int64 ordinal, h, w; str_offs
  *   [B cap + 1] the batch's string offsets (NULL without masks) placed at char_base; writes B cap records; err int [2] (err[1] set to
  *   INT_MAX by the caller): err[0] |= 1 and err[1] = min ordinal of an image with a live class outside 1..num_classes-1 or out of order.
- *   count: cls_k [num_classes] category index of each class (-1: none), ord_i [ordinals] image index; bin_cnt int [K I] zeroed by the
- *   caller; scan_in [5, K I] int64 gets D, D > 0, min(D, 10), min(D, 100), min(D, 100) G per (category, image) bin, to be scanned
- *   (inclusive, along the bins) into write's scan; nonfinite (zeroed) |= 1 for a non-finite value in a counted record.
- *   write: det_key [N] int64, det_f [N, 5], det_i [N, 4], pairs [num_active, 7], cat_kept [K+1], order_off [3, K+1] as dt_coco_eval takes them.
+ *   count: cls_k [num_classes] category slot of each class (-1: none), ord_i [ordinals] image index (-1: none); num_images x num_cats
+ *   pairs of cats_per_pair slots each (1, or num_cats = 1 for a class-agnostic evaluation whose slots are the categories in the order
+ *   their detections are concatenated; coco_eval.cuh has the fine bin layout); bin_cnt int [K I cats_per_pair] zeroed by the caller;
+ *   scan_in [5, K I] int64 gets D, D > 0, min(D, 10), min(D, 100), min(D, 100) G per pair, to be scanned (inclusive, along the pairs)
+ *   into write's scan; gt_keys: the evaluated gts' pair indices (sorted); nonfinite (zeroed) |= 1 for a non-finite value in a counted record.
+ *   write: det_key [N] int64 (each row's fine bin), det_f [N, 5], det_i [N, 4], pairs [num_active, 7], cat_kept [K+1], order_off [3, K+1]
+ *   as dt_coco_eval takes them.
  * All return 0 on bad sizes or a NULL pointer. */
 int dt_coco_results_append(int batch, int cap, int num_classes, const float* boxes, const float* scores, const int* classes, const int* counts,
                            const int64_t* images, const int64_t* str_offs, int64_t char_base, float* rec_f, int64_t* rec_i, int* err,
                            dt_stream_t stream);
 int dt_coco_results_count(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k, const int* ord_i,
-                          int num_images, int num_cats, const int64_t* gt_keys, int64_t num_gts, int* bin_cnt, int64_t* scan_in, int* nonfinite,
-                          dt_stream_t stream);
+                          int num_images, int num_cats, int cats_per_pair, const int64_t* gt_keys, int64_t num_gts, int* bin_cnt, int64_t* scan_in,
+                          int* nonfinite, dt_stream_t stream);
 int dt_coco_results_write(int64_t num_records, const float* rec_f, const int64_t* rec_i, int num_classes, const int* cls_k, const int* ord_i,
-                          int num_images, int num_cats, const int64_t* scan, const int64_t* gt_keys, int64_t num_gts, int64_t* det_key, double* det_f,
-                          int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off, dt_stream_t stream);
+                          int num_images, int num_cats, int cats_per_pair, const int* bin_cnt, const int64_t* scan, const int64_t* gt_keys,
+                          int64_t num_gts, int64_t* det_key, double* det_f, int64_t* det_i, int64_t* pairs, int64_t* cat_kept, int64_t* order_off,
+                          dt_stream_t stream);
 int dt_coco_det_check(int64_t num_dets, const int64_t* det_i, const char* det_chars, uint8_t* bad, dt_stream_t stream);
 int64_t dt_coco_gt_workspace_bytes(int64_t num_parts, int64_t num_points, int64_t num_upsampled);
 int dt_coco_gt_build(int num_anns, const int64_t* anns, const int64_t* parts, const double* xy, const uint32_t* ucounts, const char* chars,
                      void* workspace, uint32_t* out_counts, uint32_t* tmp_counts, int64_t* out_len, double* out_box, dt_stream_t stream);
-int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order);
+int64_t dt_coco_eval_workspace_bytes(int64_t num_dets, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
+                                     int num_cats);
 int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, const int64_t* pairs, const int64_t* cat_gt, const int64_t* cat_kept,
                  const int64_t* order_off, int64_t num_dets, const double* det_f, const int64_t* det_i, const char* det_chars, int64_t num_chars,
                  int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order, const double* gt_f, const int64_t* gt_i,
