@@ -508,10 +508,9 @@ struct ConvOpt {
     int sigmoid_ch = 0;                                     // output channels [0, sigmoid_ch) get a sigmoid (RPN objectness)
     size_t w_off = 0;                                       // float offset of the weight sub-matrix (a deconv quadrant)
     int out_h = 0, out_w = 0, out_step = 0, out_y0 = 0, out_x0 = 0;   // output remap (transposed conv, see ConvSpec)
-    bool precise = false;                                   // 64-wide tiles with 3 rotating main-term accumulators
     int tap0 = 0, ntaps = 0;                                // K-split: only filter taps [tap0, tap0 + ntaps)
     bool zero_shift = false;                                // add no shift (the other half of the K-split adds it)
-    bool planes_in = false, planes_out = false;             // fp16 hi/lo plane hand-over (kind::f16 only)
+    bool planes_in = false, planes_out = false;             // fp16 hi/lo plane hand-over (kind::f16 only, see add_layer)
 };
 
 struct ProgBuilder {
@@ -552,11 +551,11 @@ struct ProgBuilder {
         s.y = y; s.y_pix_stride = ystride;
         const int Ho = conv_out(H, c.k, stride, kpad), Wo = conv_out(W, c.k, stride, kpad);
         // fp16 hi/lo plane hand-over (kind::f16 only): the fp32 buffer of N*H*W*C floats holds the two fp16 planes back to back
-        if (o.planes_in && e->cfg.conv_kind == 0) s.x_lo = reinterpret_cast<const __half*>(x) + (size_t)N * H * W * c.cin;
-        if (o.planes_out && e->cfg.conv_kind == 0) s.y_lo = reinterpret_cast<__half*>(y) + (size_t)N * Ho * Wo * c.cout;
+        if (o.planes_in) s.x_lo = reinterpret_cast<const __half*>(x) + (size_t)N * H * W * c.cin;
+        if (o.planes_out) s.y_lo = reinterpret_cast<__half*>(y) + (size_t)N * Ho * Wo * c.cout;
         s.out_h = o.out_h; s.out_w = o.out_w; s.out_step = o.out_step; s.out_y0 = o.out_y0; s.out_x0 = o.out_x0;
         s.residual = o.res; s.res_pix_stride = c.cout; s.up_src = o.up; s.up_h = o.up_h; s.up_w = o.up_w;
-        s.res_mode = o.res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = o.sigmoid_ch; s.passes = e->cfg.passes; s.precise = o.precise ? 1 : 0;
+        s.res_mode = o.res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = o.sigmoid_ch; s.passes = e->cfg.passes;
         s.im_stride = img_stride;
         op.stage = stage; op.kind = 0; op.fn = -1;
         op.flops = 2.0 * (double)N * Ho * Wo * c.flop_cout * c.flop_cin * (o.ntaps > 0 ? o.ntaps : c.k * c.k);
@@ -586,13 +585,7 @@ cudaError_t fn_stem_pack_planes(Engine* e, cudaStream_t s) {
 }
 cudaError_t fn_maxpool(Engine* e, cudaStream_t s) {
     const long long n = (long long)e->cfg.batch * e->H2 * e->W2 * 16;
-    maxpool3x3s2_nhwc_kernel<false><<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"), nullptr, e->im_info());
-    return cudaGetLastError();
-}
-cudaError_t fn_maxpool_planes(Engine* e, cudaStream_t s) {
-    const long long n = (long long)e->cfg.batch * e->H2 * e->W2 * 16;
-    maxpool3x3s2_nhwc_kernel<true><<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"),
-                                                              e->buf<int>("range_flag"), e->im_info());
+    maxpool3x3s2_nhwc_kernel<<<grid_for(n), 256, 0, s>>>(e->buf("c1"), e->cfg.batch, e->H1, e->W1, 64, e->H2, e->W2, e->buf("pool"), e->im_info());
     return cudaGetLastError();
 }
 
@@ -701,9 +694,10 @@ void gen_anchors(double stride, const double* sizes, int nsizes, float* out) {
     }
 }
 
-// the stem (detector.py:170-172): the fused-window conv over the packed image.  f16: it runs the kind::f16 product (else 3xTF32 from
-// the fp32 weights).
-void add_stem(ProgBuilder& pb, bool f16, int handover) {
+// the stem (detector.py:170-172): the fused-window conv over the packed image.  f16: the packed image arrives as two fp16 planes and
+// the stem runs the kind::f16 product (the stem's converter warps -- 7 k-blocks of fp32 -> fp16 splits per 64-wide tile -- were what
+// bounded it); else 3xTF32 from the fp32 image and weights.
+void add_stem(ProgBuilder& pb, bool f16) {
     Engine* e = pb.e;
     const dt_engine_config& c = e->cfg;
     const int B = c.batch;
@@ -711,32 +705,28 @@ void add_stem(ProgBuilder& pb, bool f16, int handover) {
     Op op;
     op.stage = ST_TRUNK; op.kind = 0; op.fn = -1;
     op.flops = 2.0 * (double)B * e->H1 * e->W1 * sw.flop_cout * sw.flop_cin;
-    bool stem_planes = false, ok;
+    bool ok;
     if (f16) {
         op.matrix = e->matrix_of(sw.w);
         op.scale_src = e->wvec(sw.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = 64;
         e->scale16_used += 64;
-        // plane_handover >= 3: the packed image arrives as two fp16 planes (the stem's converter warps -- 7 k-blocks of fp32 -> fp16
-        // splits per 64-wide tile -- were what bounded it)
-        stem_planes = handover >= 3 && (e->Wp % 2) == 0;
         ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w), e->wlo16(sw.w), op.scale16, e->wvec(sw.shift),
-                             e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"), stem_planes);
+                             e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"));
     } else {
         ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w), e->wlo(sw.w), e->wvec(sw.scale), e->wvec(sw.shift),
                              e->buf("c1"), c.passes, &op.conv);
     }
     if (!ok) { pb.ok = false; fprintf(stderr, "[detectorch_b200] engine: conv_build_stem failed\n"); return; }
-    pb.fn(ST_TRUNK, stem_planes ? fn_stem_pack_planes : fn_stem_pack);
+    pb.fn(ST_TRUNK, f16 ? fn_stem_pack_planes : fn_stem_pack);
     op.conv.p.im_stride = 2;        // c1 is an image-shaped map at stride 2 (masked per image when the table is on)
     e->ops.push_back(op);
 }
 
 // ResNet layer li (detector.py:183; the C4 res5 head: detector.py:136,191,217) over N maps of h x w, into the buffers
 // plan_layer(pre) made: bottlenecks 1x1 -> 3x3 -> 1x1 + identity (downsample in the first block, which has stride 2 unless li == 1).
-// handover: the plane_handover level inside each block (0 = none); x_planes: x arrives as fp16 planes.  Returns the output map and
-// leaves its size in h, w.
-const float* add_layer(ProgBuilder& pb, int stage, const std::string& pre, int li, const float* x, int N, int& h, int& w, int handover,
-                       bool x_planes) {
+// handover: conv1 -> conv2 -> conv3 inside each block hand fp16 planes over (kind::f16 only).  Returns the output map and leaves its
+// size in h, w.
+const float* add_layer(ProgBuilder& pb, int stage, const std::string& pre, int li, const float* x, int N, int& h, int& w, bool handover) {
     Engine* e = pb.e;
     const int planes = 64 << (li - 1);
     for (int b = 0; b < e->cfg.arch_blocks[li - 1]; ++b) {
@@ -746,19 +736,18 @@ const float* add_layer(ProgBuilder& pb, int stage, const std::string& pre, int l
         const int ho = conv_out(h, 1, stride, 0), wo = conv_out(w, 1, stride, 0);
         // conv1 -> conv2 hand-over as fp16 hi/lo planes: the 3x3 conv would otherwise re-convert every input element once per filter tap
         // (the converter warps' fp32->fp16 packs are what bounds the 64/128-wide layers)
-        ConvOpt o1; o1.planes_in = b == 0 && x_planes; o1.planes_out = handover >= 1;
+        ConvOpt o1; o1.planes_out = handover;
         pb.conv(stage, wp + "conv1", x, N, h, w, cin, e->buf(p + ".t1"), planes, 0, stride, true, o1);
-        // conv2 -> conv3 the same way (plane_handover >= 2): conv3 is a 1x1 conv, so this saves one conversion per element, the converter
-        // warps' shared-memory round trip (16 KB read + 16 KB written per k-block) and their issue slots in the epilogue-bound conv3
-        ConvOpt o2; o2.planes_in = handover >= 1; o2.planes_out = handover >= 2;
+        // conv2 -> conv3 the same way: conv3 is a 1x1 conv, so this saves one conversion per element, the converter warps' shared-memory
+        // round trip (16 KB read + 16 KB written per k-block) and their issue slots in the epilogue-bound conv3
+        ConvOpt o2; o2.planes_in = handover; o2.planes_out = handover;
         pb.conv(stage, wp + "conv2", e->buf(p + ".t1"), N, ho, wo, planes, e->buf(p + ".t2"), planes, 1, 1, true, o2);
         const float* idt = x;
         if (b == 0) {
-            ConvOpt od; od.planes_in = x_planes;
-            pb.conv(stage, wp + "downsample.0", x, N, h, w, cin, e->buf(p + ".ds"), planes * 4, 0, stride, false, od);
+            pb.conv(stage, wp + "downsample.0", x, N, h, w, cin, e->buf(p + ".ds"), planes * 4, 0, stride, false);
             idt = e->buf(p + ".ds");
         }
-        ConvOpt o3; o3.res_mode = RES_TILE; o3.res = idt; o3.planes_in = handover >= 2;
+        ConvOpt o3; o3.res_mode = RES_TILE; o3.res = idt; o3.planes_in = handover;
         pb.conv(stage, wp + "conv3", e->buf(p + ".t2"), N, ho, wo, planes, e->buf(p + ".out"), planes * 4, 0, 1, true, o3);
         x = e->buf(p + ".out");
         h = ho; w = wo;
@@ -864,29 +853,21 @@ void add_mask_head(ProgBuilder& pb) {
     pb.fn(ST_MASK_ROIS, fn_mask_rois);
     pb.fn(ST_MASK_ROI_FEAT, fn_mask_roi_feat);
     const float* mx = e->buf("mask_feat");
-    bool precise = false;
     if (f.c4) {
         int h = 14, w = 14;
-        mx = add_layer(pb, ST_MASK_HEAD, "m5", 4, mx, D, h, w, 0, false);
+        mx = add_layer(pb, ST_MASK_HEAD, "m5", 4, mx, D, h, w, false);
     } else {
         // The mask logits carry the tightest parity bar (1e-4 absolute) and sit behind four K = 2304 convolutions, where the tensor
-        // core's truncating fp32 accumulate is the error floor.  precise_mask shortens the chains by SPLITTING K: each 3x3 convolution
-        // runs as two launches over filter taps [0,5) and [5,9); the second adds the first's fp32 result in its epilogue (RES_TILE on the
-        // output buffer itself, round-to-nearest) before the ReLU.  precise_mask = 2 instead runs 64-wide tiles with 3 rotating
-        // main-term accumulators.
-        precise = c.precise_mask == 2;
+        // core's truncating fp32 accumulate is the error floor.  The chains are shortened by SPLITTING K: each 3x3 convolution runs as
+        // two launches over filter taps [0,5) and [5,9); the second adds the first's fp32 result in its epilogue (RES_TILE on the output
+        // buffer itself, round-to-nearest) before the ReLU.
         for (int i = 1; i <= 4; ++i) {
             const std::string wn = "mask_head.conv_head.fcn" + std::to_string(i);
             float* my = e->buf("mask_c" + std::to_string(i));
-            if (c.precise_mask == 1) {
-                ConvOpt lo; lo.ntaps = 5;
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, lo);
-                ConvOpt hi; hi.res_mode = RES_TILE; hi.res = my; hi.tap0 = 5; hi.ntaps = 4; hi.zero_shift = true;
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, hi);
-            } else {
-                ConvOpt o; o.precise = precise;
-                pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, o);
-            }
+            ConvOpt lo; lo.ntaps = 5;
+            pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, lo);
+            ConvOpt hi; hi.res_mode = RES_TILE; hi.res = my; hi.tap0 = 5; hi.ntaps = 4; hi.zero_shift = true;
+            pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, hi);
             mx = my;
         }
     }
@@ -894,7 +875,6 @@ void add_mask_head(ProgBuilder& pb) {
         ConvOpt o;
         o.w_off = (size_t)ij * 256 * f.mask_in;
         o.out_h = o.out_w = M; o.out_step = 2; o.out_y0 = ij / 2; o.out_x0 = ij % 2;
-        o.precise = precise;
         pb.conv(ST_MASK_HEAD, "deconv", mx, D, M / 2, M / 2, f.mask_in, e->buf("mask_up"), 256, 0, 1, true, o);
     }
     pb.conv(ST_MASK_HEAD, "mask_logits", e->buf("mask_up"), D, M, M, 256, e->buf("mask_logits"), e->convs["mask_logits"].cout, 0, 1, false);
@@ -908,18 +888,14 @@ bool build_program(Engine* e) {
     ProgBuilder pb{e};
     // ---- trunk (detector.py:170-183): to layer4 for FPN, to layer3 for C4 (which runs layer4 per RoI).  The C4 family always builds
     // the fused stem from the fp32 weights and hands no fp16 planes over.
-    const int handover = f.c4 ? 0 : c.plane_handover;
-    add_stem(pb, !f.c4 && c.conv_kind == 0, handover);
-    // plane_handover >= 4 (opt-in): the pooled map leaves as fp16 planes too (its two consumers -- conv1 and the downsample conv of the first
-    // bottleneck -- then load their operand tiles directly).  Measured twice, before and after the epilogue rewrite: the consumers gain 7 us
-    // each, the pool kernel loses 16 us -- no net gain, so the default hand-over level stays 3.
-    const bool pool_planes = c.conv_kind == 0 && handover >= 4;
-    pb.fn(ST_TRUNK, pool_planes ? fn_maxpool_planes : fn_maxpool);
+    const bool f16_planes = !f.c4 && c.conv_kind == 0;
+    add_stem(pb, f16_planes);
+    pb.fn(ST_TRUNK, fn_maxpool);
     const float* x = e->buf("pool");
     int h = e->H2, w = e->W2;
     for (int li = 1; li <= (f.c4 ? 3 : 4); ++li) {
         pb.img_stride = 4 << (li - 1);
-        x = add_layer(pb, ST_TRUNK, "l" + std::to_string(li), li, x, B, h, w, handover, li == 1 && pool_planes);
+        x = add_layer(pb, ST_TRUNK, "l" + std::to_string(li), li, x, B, h, w, f16_planes);
     }
     if (!f.c4) add_fpn(pb);
     if (c.use_rpn) add_rpn(pb);
@@ -939,7 +915,7 @@ bool build_program(Engine* e) {
     const int R = B * c.post_nms_top_n;
     if (f.c4) {
         int rh = 14, rw = 14;
-        add_layer(pb, ST_BOX_HEAD, "r5", 4, e->buf("roi_feat"), R, rh, rw, 0, false);
+        add_layer(pb, ST_BOX_HEAD, "r5", 4, e->buf("roi_feat"), R, rh, rw, false);
         pb.fn(ST_BOX_HEAD, fn_avgpool);
     } else {
         pb.conv(ST_BOX_HEAD, "fc6", e->buf("roi_feat"), 1, 1, R, 49 * 256, e->buf("fc6"), 1024, 0, 1, true);

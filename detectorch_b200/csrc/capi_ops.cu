@@ -161,27 +161,24 @@ __global__ void nchw_to_nhwc_tr_kernel(const float* __restrict__ x, int HW, int 
 }  // namespace
 
 namespace {
+constexpr int kSmemMapWarps = 24;       // warps per CTA of the shared-memory-resident map kernel
+constexpr int kRoiTileKB = 28;          // shared-memory output tile of the transpose path: 128 channels x 49 bins
+
 // shared-memory-resident map variant: geometry of the launch, or false if the map slab does not fit
-struct SmemMapPlan { int group, nwarps, num_chunks, num_items; size_t smem; };
+struct SmemMapPlan { int group, num_chunks, num_items; size_t smem; };
 bool smem_map_plan(int batch, int channels, int height, int width, int64_t num_rois, int ph, int pw, SmemMapPlan* pl) {
-    static int mode = -1;
-    if (mode < 0) { const char* e = getenv("DT_ROI_SMEM_MAP"); mode = e ? atoi(e) : 1; }
-    if (!mode) return false;
     if (!((ph == 7 && pw == 7) || (ph == 14 && pw == 14)) || channels % kSlabC) return false;
     const size_t hw = (size_t)height * width;
     if ((size_t)(height - 1) * width > 65535) return false;      // row offsets are packed as uint16
     const size_t map_bytes = ((hw + 7) / 8 * 8) * kSlabC * 4;
-    static int nwarps = 0;
-    if (!nwarps) { const char* e = getenv("DT_ROI_SMEM_WARPS"); nwarps = e ? atoi(e) : 24; if (nwarps < 4) nwarps = 4; if (nwarps > 24) nwarps = 24; }
-    pl->nwarps = nwarps;
     pl->group = 3584 / ((ph + pw) * 32);
-    pl->smem = map_bytes + (size_t)pl->nwarps * pl->group * (ph + pw) * 32;
+    pl->smem = map_bytes + (size_t)kSmemMapWarps * pl->group * (ph + pw) * 32;
     if (pl->smem > 227 * 1024) return false;
     const int slabs = batch * (channels / kSlabC);
     int a = num_sms(), b = slabs;
     while (b) { const int t = a % b; a = b; b = t; }
     int chunks = num_sms() / a;                                        // slabs * chunks is a multiple of the SM count
-    const int64_t per_pass = (int64_t)pl->nwarps * pl->group;       // RoIs one CTA covers per sweep of its warps
+    const int64_t per_pass = (int64_t)kSmemMapWarps * pl->group;       // RoIs one CTA covers per sweep of its warps
     const int64_t max_chunks = (num_rois + per_pass - 1) / per_pass;
     if (chunks > max_chunks) chunks = (int)max_chunks;
     pl->num_chunks = chunks < 1 ? 1 : chunks;
@@ -201,14 +198,11 @@ extern "C" int dt_roi_align_forward_nchw_fast(const float* features, int batch, 
                                               int height, int width, int pooled_height, int pooled_width, float spatial_scale,
                                               int sampling_ratio, float* out, void* workspace, dt_stream_t stream) {
     if (num_rois <= 0) return 1;
-    // channel slab: the largest divisor of C (multiple of 4) whose [CS][ph*pw] fp32 tile fits ~50 KB of shared memory
-    // smaller tiles = more resident CTAs and more L1 left for the gathers; default 28 KB (128 channels x 49 bins)
-    // (tunable: DT_ROI_TILE_KB)
-    static int tile_kb = 0;
-    if (!tile_kb) { const char* e = getenv("DT_ROI_TILE_KB"); tile_kb = e ? atoi(e) : 28; if (tile_kb < 4) tile_kb = 4; if (tile_kb > 100) tile_kb = 100; }
+    // channel slab: the largest divisor of C (multiple of 4) whose [CS][ph*pw] fp32 tile fits kRoiTileKB of shared memory
+    // (smaller tiles = more resident CTAs and more L1 left for the gathers)
     int cs = 0;
     for (int d = channels; d >= 4; --d)
-        if (channels % d == 0 && (d & 3) == 0 && (size_t)d * pooled_height * pooled_width * 4 <= (size_t)tile_kb * 1024 && ((size_t)d * pooled_height * pooled_width * 4) % 16 == 0) { cs = d; break; }
+        if (channels % d == 0 && (d & 3) == 0 && (size_t)d * pooled_height * pooled_width * 4 <= (size_t)kRoiTileKB * 1024 && ((size_t)d * pooled_height * pooled_width * 4) % 16 == 0) { cs = d; break; }
     const size_t tile_bytes = (size_t)cs * pooled_height * pooled_width * 4;
     if (sampling_ratio != 2 || (channels & 3) || pooled_height > kMaxPooled || pooled_width > kMaxPooled || cs == 0) {
         // outside the fast path's envelope: the exact kernel handles every configuration
@@ -235,8 +229,9 @@ extern "C" int dt_roi_align_forward_nchw_fast(const float* features, int batch, 
                                                227 * 1024));                                                                              \
             attr = true;                                                                                                                   \
         }                                                                                                                                  \
-        roi_align_smem_map_kernel<PHW, PHW, BATCHED><<<grid, pl.nwarps * 32, pl.smem, st>>>(features, tab, (long long)num_rois, channels,   \
-                                                                                           HW, pl.num_items, pl.num_chunks, pl.group, out); \
+        roi_align_smem_map_kernel<PHW, PHW, BATCHED><<<grid, kSmemMapWarps * 32, pl.smem, st>>>(features, tab, (long long)num_rois,       \
+                                                                                               channels, HW, pl.num_items, pl.num_chunks,   \
+                                                                                               pl.group, out);                              \
     }
         if (pooled_height == 7 && batch == 1) DT_LAUNCH_SMEM_MAP(7, false)
         else if (pooled_height == 7) DT_LAUNCH_SMEM_MAP(7, true)

@@ -112,11 +112,6 @@ __device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int
                  "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                  : "memory");
 }
-// programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may become resident while its
-// predecessor in the stream still runs; it must not touch the predecessor's results before griddep_wait() returns (= predecessor complete,
-// memory flushed).  griddep_launch_dependents() lets the NEXT kernel in the stream do the same with respect to this one.
-__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 template <int kPending>

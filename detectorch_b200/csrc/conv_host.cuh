@@ -259,18 +259,16 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
 // (2 pixels) delivers, per ky, one 32-float K-block per output pixel straight into the swizzled A tile (last 4 floats
 // hit zero weights).  K = 7 x 32.  H uses elementStride 2.
 inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int W1, const void* w_hi, const void* w_lo, const float* scale,
-                            const float* shift, float* y, int passes, ConvLayer* L, int kind = KIND_TF32X3, int* range_flag = nullptr,
-                            bool x4_planes = false) {
+                            const float* shift, float* y, int passes, ConvLayer* L, int kind = KIND_TF32X3, int* range_flag = nullptr) {
     memset(&L->p, 0, sizeof(ConvParams));
     ConvParams& p = L->p;
     int wbox, hbox, nbox;
     choose_box(W1, H1, B, 256, &wbox, &hbox, &nbox);
     const int bn = 64;
     L->block_n = bn;
-    const uint64_t row = (uint64_t)Wp * 16;
-    if (x4_planes) {
+    if (kind == KIND_F16X3) {
         // x4 holds two fp16 planes [B, Hp, Wp, 4] back to back (hi, lo): same overlapping-stride window, 16 bytes (2 pixels) per step
-        if (kind != KIND_F16X3 || (Wp & 1)) return false;
+        if (Wp & 1) { fprintf(stderr, "[detectorch_b200] conv_build_stem: the fp16 planes need an even padded width (got %d)\n", Wp); return false; }
         const __half* xh = reinterpret_cast<const __half*>(x4);
         const __half* xl = xh + (size_t)B * Hp * Wp * 4;
         const uint64_t rowh = (uint64_t)Wp * 8;
@@ -278,11 +276,11 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
             !make_tmap_4d_f16(&p.tm_a2, xl, 32, W1, Hp, B, 16, rowh, rowh * Hp, 32, wbox, hbox * 2, nbox, 1, 2))
             return false;
         p.a_planes = 1;
-    } else if (!make_tmap_4d(&p.tm_a, x4, 32, W1, Hp, B, 32, row, row * Hp, 32, wbox, hbox * 2, nbox, 1, 2)) return false;
-    if (kind == KIND_F16X3) {
         if (!make_tmap_2d_f16(&p.tm_bhi, w_hi, 224, 64, 224 * 2, 32, bn)) return false;
         if (!make_tmap_2d_f16(&p.tm_blo, w_lo, 224, 64, 224 * 2, 32, bn)) return false;
     } else {
+        const uint64_t row = (uint64_t)Wp * 16;
+        if (!make_tmap_4d(&p.tm_a, x4, 32, W1, Hp, B, 32, row, row * Hp, 32, wbox, hbox * 2, nbox, 1, 2)) return false;
         if (!make_tmap_2d(&p.tm_bhi, w_hi, 224, 64, 224 * 4, 32, bn)) return false;
         if (!make_tmap_2d(&p.tm_blo, w_lo, 224, 64, 224 * 4, 32, bn)) return false;
     }
@@ -303,14 +301,6 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
     return true;
 }
 
-// DT_CONV_PDL=1: conv launches carry the programmatic-stream-serialization attribute (see griddep_wait in common.cuh): the prologue of
-// launch i+1 overlaps the tail of launch i.  Only conv launches take part; every other kernel keeps plain stream order.
-inline bool conv_use_pdl() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("DT_CONV_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
-    return v == 1;
-}
-
 template <int BN, int NM, int KIND, bool MASK>
 inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
     using Cfg = ConvCfg<BN, NM, KIND>;
@@ -319,18 +309,6 @@ inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
         cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         attr_set = true;
-    }
-    if (conv_use_pdl()) {
-        ConvParams prm = L.p;
-        prm.pdl = 1;
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = L.grid; cfg.blockDim = dim3(Cfg::THREADS, 1, 1); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, conv_wgmma_kernel<BN, NM, KIND, MASK>, prm);
     }
     conv_wgmma_kernel<BN, NM, KIND, MASK><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
     return cudaGetLastError();

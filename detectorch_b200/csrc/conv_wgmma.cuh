@@ -74,7 +74,6 @@ struct ConvParams {
     int a_planes;          // KIND_F16X3: the input already is a pair of fp16 planes (hi, lo) written by the producing layer
     int out_planes;        // KIND_F16X3: write the output as a pair of fp16 planes (hi = fp16(y), lo = fp16(y - hi)) instead of fp32
     int* range_flag;       // KIND_F16X3: set to 1 when an activation does not fit fp16 (|x| >= 65504 or NaN); may be null
-    int pdl;               // launched with programmatic stream serialization: release the next launch early, wait for the previous one
     // image-shaped maps of a batch of differently-sized images: output pixels outside image n's extent at im_stride (image_info) are
     // written as exact zeros, so the next 3x3 conv reads what a batch-1 run of that image reads through TMA zero fill.  Null = off.
     const float* im_info;
@@ -174,12 +173,6 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
         fence_mbar_init();
     }
     __syncthreads();
-    if (p.pdl) {
-        // Everything above touched no global data: with PDL it overlaps the tail of the previous launch.  The next launch in the
-        // stream may become resident as soon as every CTA of this grid got here (it then parks in its own griddep_wait).
-        griddep_launch_dependents();
-        griddep_wait();
-    }
 
     // work item -> tile coordinates.  The N-tile varies fastest so that consecutive items re-read the same A tile from L2.
     auto tile_of = [&](int item, int& w0, int& h0, int& n0img, int& n0) {

@@ -77,14 +77,12 @@ static __global__ void stem_pack_nhwc4_planes_kernel(const float* __restrict__ i
     if (bad && range_flag) *range_flag = 1;
 }
 
-// NHWC 3x3 stride-2 pad-1 max pool (torchvision maxpool); PLANES: the result leaves as two fp16 planes (hi, lo) for plane-input convs.
-// im_info (may be null): the window ends at image b's extent (the input is the stride-2 map), and outputs past it are zero.
-template <bool PLANES>
+// NHWC 3x3 stride-2 pad-1 max pool (torchvision maxpool).  im_info (may be null): the window ends at image b's extent (the input is the
+// stride-2 map), and outputs past it are zero.
 static __global__ void maxpool3x3s2_nhwc_kernel(const float* __restrict__ x, int B, int H, int W, int C, int Ho, int Wo, float* __restrict__ y,
-                                                int* __restrict__ range_flag, const float* __restrict__ im_info) {
+                                                const float* __restrict__ im_info) {
     const int C4 = C >> 2;
     const long long total = (long long)B * Ho * Wo * C4;
-    bool bad = false;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int c4 = (int)(i % C4);
         long long m = i / C4;
@@ -104,16 +102,8 @@ static __global__ void maxpool3x3s2_nhwc_kernel(const float* __restrict__ x, int
             }
         }
         if (ho * 2 >= g.h || wo * 2 >= g.w) best = make_float4(0.f, 0.f, 0.f, 0.f);
-        if constexpr (PLANES) {
-            uint2 h, l;
-            split_planes4(best, &h, &l, &bad);
-            reinterpret_cast<uint2*>(y)[i] = h;
-            reinterpret_cast<uint2*>(y)[total + i] = l;       // the low plane follows the high plane (ProgBuilder::conv, planes_in)
-        } else {
-            reinterpret_cast<float4*>(y)[i] = best;
-        }
+        reinterpret_cast<float4*>(y)[i] = best;
     }
-    if (PLANES && bad && range_flag) *range_flag = 1;
 }
 
 // P6 = max_pool2d(P5, kernel 1, stride 2) == stride-2 subsample (detector.py:250).  With per-image sizes no mask is needed: output

@@ -44,8 +44,8 @@ class EngineConfig(ctypes.Structure):
                 ("rpn_min_size", ctypes.c_float), ("num_classes", ctypes.c_int), ("score_thresh", ctypes.c_float),
                 ("det_nms_thresh", ctypes.c_float), ("max_dets", ctypes.c_int), ("det_cap", ctypes.c_int),
                 ("use_mask", ctypes.c_int), ("output_prob", ctypes.c_int), ("emit_full_masks", ctypes.c_int),
-                ("passes", ctypes.c_int), ("precise_mask", ctypes.c_int), ("exact_roialign", ctypes.c_int), ("model_type", ctypes.c_int), ("use_rpn", ctypes.c_int),
-                ("conv_kind", ctypes.c_int), ("plane_handover", ctypes.c_int)]
+                ("passes", ctypes.c_int), ("exact_roialign", ctypes.c_int), ("model_type", ctypes.c_int), ("use_rpn", ctypes.c_int),
+                ("conv_kind", ctypes.c_int)]
 
 
 _DTYPES = {0: torch.float32, 1: torch.int32, 2: torch.uint8}
@@ -139,7 +139,7 @@ def pad_proposals(boxes_list, batch, cap):
 class Engine:
     def __init__(self, arch="resnet50", batch=1, height=800, width=1216, pre_nms_top_n=1000, post_nms_top_n=1000,
                  rpn_nms_thresh=0.7, rpn_min_size=0.0, num_classes=81, score_thresh=0.05, det_nms_thresh=0.5, max_dets=100,
-                 det_cap=100, use_mask=True, output_prob=True, emit_full_masks=False, passes=3, precise_mask=True, exact_roialign=False, model="fpn", use_rpn=True, conv_kind=None, device="cuda:0",
+                 det_cap=100, use_mask=True, output_prob=True, emit_full_masks=False, passes=3, exact_roialign=False, model="fpn", use_rpn=True, conv_kind=None, device="cuda:0",
                  share_weights_with=None):
         if not torch.cuda.is_available():
             raise RuntimeError("detectorch_b200.Engine needs a CUDA device (no CPU fallback)")
@@ -154,7 +154,6 @@ class Engine:
         cfg.num_classes, cfg.score_thresh, cfg.det_nms_thresh = num_classes, score_thresh, det_nms_thresh
         cfg.max_dets, cfg.det_cap = max_dets, det_cap
         cfg.use_mask, cfg.output_prob, cfg.emit_full_masks, cfg.passes = int(use_mask), int(output_prob), int(emit_full_masks), passes
-        cfg.precise_mask = int(precise_mask)          # 1/True = K-split mask convs, 2 = 64-wide tiles with 3 rotating accumulators, 0 = plain
         cfg.exact_roialign = int(exact_roialign)
         cfg.model_type = 1 if model == "c4" else 0
         cfg.use_rpn = int(use_rpn)
@@ -163,7 +162,6 @@ class Engine:
         if conv_kind not in ("f16", "tf32"):
             raise ValueError("conv_kind must be 'f16' or 'tf32'")
         cfg.conv_kind = 0 if conv_kind == "f16" else 1
-        cfg.plane_handover = int(os.environ.get("DT_PLANE_HANDOVER", "3"))     # 0 = fp32 hand-over, 1 = conv1 -> conv2 as fp16 planes, 2 = also conv2 -> conv3, 3 = also image -> stem; 4 = also pool -> first bottleneck (measured: no net gain, opt-in)
         self.cfg = cfg
         self.h = self.L.dt_engine_create(ctypes.byref(cfg))
         if not self.h:
@@ -192,7 +190,7 @@ class Engine:
         """What shapes the packed weight buffer (matrices, fp16 halves, and the per-conv-launch scale vectors, which are laid out in launch
         order): the model and the numerics mode -- not the image size, RoI / detection capacities or thresholds."""
         c = self.cfg
-        return tuple(c.arch_blocks) + (c.num_classes, c.use_mask, c.model_type, c.use_rpn, c.conv_kind, c.precise_mask, c.passes)
+        return tuple(c.arch_blocks) + (c.num_classes, c.use_mask, c.model_type, c.use_rpn, c.conv_kind, c.passes)
 
     def owns(self, ptr):
         return self._ws_lo <= ptr < self._ws_hi

@@ -241,7 +241,7 @@ class detector(torch.nn.Module):
         while len(self._engines) >= max(1, self.max_cached_engines):
             self._engines.popitem(last=False)                       # least recently used
         # what shapes the packed weight buffer (and the per-launch scale vectors in it): the model, not the image size / capacities
-        mk = tuple(sorted((k, str(v)) for k, v in kw.items() if k in ("arch", "num_classes", "use_mask", "model", "use_rpn", "conv_kind", "precise_mask", "passes")))
+        mk = tuple(sorted((k, str(v)) for k, v in kw.items() if k in ("arch", "num_classes", "use_mask", "model", "use_rpn", "conv_kind", "passes")))
         donor = next((e for e, _ in self._engines.values() if getattr(e, "_mirror_model_key", None) == mk), None)
         if donor is not None:
             eng = Engine(share_weights_with=donor, **kw)

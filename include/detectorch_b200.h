@@ -219,8 +219,6 @@ typedef struct dt_engine_config {
     int output_prob;             /* softmax / sigmoid on the outputs (detector.py:147) */
     int emit_full_masks;         /* also materialise masks_full [D,num_classes,28,28] (the public layout) */
     int passes;                  /* 3 = 3xTF32 (fp32-accurate, default), 1 = single-pass TF32 */
-    int precise_mask;            /* mask-head 3x3 convs (K = 2304): 1 = K-split in two launches with an fp32 RN add between them (halves the
-                                    truncating-accumulate error; default), 2 = 128-wide tiles with 3 rotating accumulators, 0 = plain */
     int exact_roialign;          /* 1 = RoIAlign in the reference's exact fp32 operation order (bit-identical to its CPU loop);
                                     0 = separable / FMA fast path (fp32 re-association only, ~1e-7 relative) */
     int model_type;              /* 0 = R-50/101-FPN + RPN (+ '1up4convs' mask head); 1 = R-50/101-C4 (res5 head, 'upshare' mask head) */
@@ -233,11 +231,9 @@ typedef struct dt_engine_config {
                                     `roi_levels` / `roi_counts`.  The host must keep |box * scale / 16| below 8990 (exact hash). */
     int conv_kind;               /* 0 = three-term product on the kind::f16 pipe (fp16 hi/lo halves, default: twice the tf32 issue rate; an
                                     activation >= 65504 raises the int32 buffer "range_flag", which every run that starts at the first stage clears
-                                    before it launches anything), 1 = 3xTF32 (no range limit) */
-    int plane_handover;          /* kind::f16 only: 1 = conv1 of every bottleneck writes its output as two fp16 planes (hi, lo) that conv2 (3x3)
-                                    loads straight into its operand tiles (no per-tap re-conversion); 2 = conv2 -> conv3 as well; 3 = also the
-                                    packed image -> stem (FPN engine); 4 = also the pooled map -> first bottleneck (no net gain measured:
-                                    opt-in); 0 = fp32 hand-over */
+                                    before it launches anything), 1 = 3xTF32 (no range limit).  An FPN engine of kind 0 hands activations
+                                    over as two fp16 planes (hi, lo) from conv1 to conv2 to conv3 of every trunk bottleneck and from the packed
+                                    image to the stem, so the consumer loads its operand tiles without re-converting them */
 } dt_engine_config;
 
 typedef void* dt_engine_t;

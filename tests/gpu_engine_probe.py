@@ -42,7 +42,7 @@ def parity(h=320, w=416, arch="resnet50"):
     eng.load_state_dict(P)
     eng.run(img.to(dev), 1.0)
     torch.cuda.synchronize()
-    print("engine ran (exact_roialign=True, precise_mask=True)", flush=True)
+    print("engine ran (exact_roialign=True)", flush=True)
     for i in range(4):
         cmp("C%d" % (i + 2), nhwc_to_nchw(eng.buffer("C%d" % (i + 2))), S["C"][i])
     for i in range(4):

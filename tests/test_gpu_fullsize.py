@@ -1,7 +1,7 @@
 """GPU parity at the BENCHED configuration and sizes (BASELINE.json configs[1..4]):
 
   * Mask R-CNN R-50-FPN, 3x800x1216, batch 2 of distinct images, exactly the engine bench.py times
-    (conv_kind f16, fast RoIAlign, precise_mask, det_cap 100, no full-mask materialisation) against
+    (conv_kind f16, fast RoIAlign, det_cap 100, no full-mask materialisation) against
     oracle.network.detect_and_mask_fpn per image: activations, RPN outputs, teacher-forced integer
     stages bit-exact, mask logits < 1e-4 absolute, un-forced detections as matched sets;
   * Faster R-CNN R-50-C4 at 800x1216 (the 6000-of-57000 argpartition branch of generate_proposals.py:80-86);
@@ -103,7 +103,7 @@ def fpn_ctx(built):
     P = net.synthetic_params("resnet50")
     imgs = [net.synthetic_image(1, H, W, seed=s) for s in (0, 1)]
     S = [net.detect_and_mask_fpn(im, P) for im in imgs]
-    # exactly bench.py's engine: defaults (conv_kind f16, exact_roialign False, precise_mask, plane hand-over), det_cap 100, no full masks
+    # exactly bench.py's engine: defaults (conv_kind f16, exact_roialign False), det_cap 100, no full masks
     eng = E.Engine(arch="resnet50", batch=2, height=H, width=W, det_cap=100, use_mask=True, emit_full_masks=False)
     assert eng.cfg.conv_kind == 0 and eng.cfg.exact_roialign == 0
     eng.load_state_dict(P)

@@ -1,6 +1,6 @@
 """Batches of differently-sized images on one padded canvas (detect(..., image_sizes, original_sizes), Engine.set_image_info):
 every image's maps, proposals, detections and masks are bit-identical to a batch-1 run of that image at its own size, whatever the
-canvas holds around it (NaN here), on every conv kind / plane hand-over / RoIAlign variant; a captured graph replays for any size mix."""
+canvas holds around it (NaN here), on every conv kind and RoIAlign variant; a captured graph replays for any size mix."""
 import numpy as np
 import pytest
 import torch
@@ -44,10 +44,9 @@ def _mask_model(params):
     return model.cuda()
 
 
-@pytest.mark.parametrize("conv_kind,handover,exact", [("f16", "3", False), ("f16", "3", True), ("f16", "0", False), ("tf32", "3", False)])
-def test_per_image_equality(params, monkeypatch, conv_kind, handover, exact):
+@pytest.mark.parametrize("conv_kind,exact", [("f16", False), ("f16", True), ("tf32", False)])
+def test_per_image_equality(params, conv_kind, exact):
     from detectorch_b200.engine import Engine
-    monkeypatch.setenv("DT_PLANE_HANDOVER", handover)
     dev = torch.device("cuda:0")
     kw = dict(arch="resnet50", det_cap=128, exact_roialign=exact, conv_kind=conv_kind)
     img, crops = _canvas_batch(SIZES)

@@ -36,6 +36,23 @@ def test_ctypes_signatures_cover_operator_api(built):
         assert n in _lib.SIGNATURES
 
 
+def test_engine_config_matches_header_struct():
+    """EngineConfig (ctypes) declares the fields of the header's dt_engine_config in the same order and with the same C types."""
+    from detectorch_b200.engine import EngineConfig
+    src = open(os.path.join(ROOT, "include", "detectorch_b200.h")).read()
+    body = re.search(r"typedef struct dt_engine_config \{(.*?)\} dt_engine_config;", src, flags=re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    ctype = {"int": ctypes.c_int, "float": ctypes.c_float}
+    fields = []
+    for decl in filter(None, (d.strip() for d in body.split(";"))):
+        t, names = decl.split(None, 1)
+        for n in names.split(","):
+            name, length = re.fullmatch(r"\s*(\w+)\s*(?:\[(\d+)\])?\s*", n).groups()
+            fields.append((name, ctype[t] * int(length) if length else ctype[t]))
+    assert [n for n, _ in fields] == [n for n, _ in EngineConfig._fields_]
+    assert [t for _, t in fields] == [t for _, t in EngineConfig._fields_]
+
+
 def test_engine_param_table_matches_reference_names(built):
     from detectorch_b200 import engine
     from oracle import network as net
