@@ -51,6 +51,8 @@ SIGNATURES = {
     "dt_conv2d_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                c_void_p, c_int, c_void_p]),
+    "dt_conv2d_nhwc_two_phase": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                         c_void_p, c_void_p]),
     "dt_coco_gt_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
     "dt_coco_gt_build": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),

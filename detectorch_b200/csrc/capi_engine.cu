@@ -165,11 +165,12 @@ struct Op {
     int kind;            // 0 conv, 1 custom lambda index
     ConvLayer conv;
     int fn;              // index into engine fns for kind==1
-    // kind::f16 convs: scale16 = scale / multiplier(matrix) is (re)derived at finalize time
-    const float* scale_src = nullptr;
-    float* scale16 = nullptr;
-    int scale_n = 0;
-    int matrix = -1;
+    // kind::f16 convs: scale16 = scale / multiplier(matrix) is (re)derived at finalize time, for each weight matrix the launch reads
+    // ([1]: the phase-1 matrix of a RES_STAGED launch)
+    const float* scale_src[2] = {nullptr, nullptr};
+    float* scale16[2] = {nullptr, nullptr};
+    int scale_n[2] = {0, 0};
+    int matrix[2] = {-1, -1};
 };
 
 // one RoIAlign launch: n RoIs (on the level `levels` gives, or all on level 0 when it is null) -> out [n, res, res, ch]
@@ -395,14 +396,13 @@ void add_buf(Engine* e, const std::string& name, std::initializer_list<long long
 
 int conv_out(int x, int k, int s, int p) { return (x + 2 * p - k) / s + 1; }
 
-// the buffers of ResNet layer li (add_layer) over N maps whose output is h x w, named pre + "b<block>.t1" / ".t2" / ".ds" / ".out"
+// the buffers of ResNet layer li (add_layer) over N maps whose output is h x w, named pre + "b<block>.t1" / ".t2" / ".out"
 void plan_layer(Engine* e, const std::string& pre, int li, long long N, int h, int w) {
     const int planes = 64 << (li - 1);
     for (int b = 0; b < e->cfg.arch_blocks[li - 1]; ++b) {
         const std::string p = pre + "b" + std::to_string(b);
         add_buf(e, p + ".t1", {N, h, w, planes});
         add_buf(e, p + ".t2", {N, h, w, planes});
-        if (b == 0) add_buf(e, p + ".ds", {N, h, w, planes * 4});
         add_buf(e, p + ".out", {N, h, w, planes * 4});
     }
 }
@@ -513,54 +513,86 @@ struct ConvOpt {
     bool planes_in = false, planes_out = false;             // fp16 hi/lo plane hand-over (kind::f16 only, see add_layer)
 };
 
+// one convolution of the program: the weights of layer `w` over x [N, H, W] (xstride floats per pixel) into y (ystride floats per pixel)
+struct ConvCall {
+    std::string w;
+    const float* x; int N, H, W, xstride;
+    float* y; int ystride, pad, stride;
+    bool relu;
+    ConvOpt o;
+};
+
 struct ProgBuilder {
     Engine* e;
     bool ok = true;
     int img_stride = 0;     // > 0: the following convs write image-shaped maps at this stride (masked per image when the table is on)
 
-    void conv(int stage, const std::string& wname, const float* x, int N, int H, int W, int xstride, float* y, int ystride, int kpad,
-              int stride, bool relu, const ConvOpt& o = ConvOpt()) {
-        const ConvW& c = e->convs[wname];
-        ConvSpec s;
+    // the ConvSpec of c; its weight matrix / scale vector go to slot `slot` of op, its FLOPs are added to op's
+    bool spec(const ConvCall& k, Op& op, int slot, ConvSpec& s) {
+        const ConvW& c = e->convs[k.w];
+        const ConvOpt& o = k.o;
         memset(&s, 0, sizeof(s));
-        s.x = x; s.N = N; s.H = H; s.W = W; s.Cin = c.cin; s.x_pix_stride = xstride;
-        Op op;
-        s.Cout = c.cout; s.kh = c.k; s.kw = c.k; s.pad = kpad; s.stride = stride;
+        s.x = k.x; s.N = k.N; s.H = k.H; s.W = k.W; s.Cin = c.cin; s.x_pix_stride = k.xstride;
+        s.Cout = c.cout; s.kh = c.k; s.kw = c.k; s.pad = k.pad; s.stride = k.stride;
         s.shift = e->wvec(o.zero_shift ? e->zeros : c.shift);
         s.tap0 = o.tap0; s.ntaps = o.ntaps;
         if (e->cfg.conv_kind == 0) {
             // kind::f16 three-term product: fp16 halves of w * multiplier(matrix); the multiplier is undone through a per-op scale vector
             const size_t n16 = align_up((size_t)c.cout, 64);
-            op.matrix = e->matrix_of(c.w + o.w_off);
-            if (op.matrix < 0 || e->scale16_used + n16 > Engine::kScale16Floats) {
-                ok = false;
-                fprintf(stderr, "[detectorch_b200] engine: scale16 arena / matrix lookup failed for %s\n", wname.c_str());
-                return;
+            op.matrix[slot] = e->matrix_of(c.w + o.w_off);
+            if (op.matrix[slot] < 0 || e->scale16_used + n16 > Engine::kScale16Floats) {
+                fprintf(stderr, "[detectorch_b200] engine: scale16 arena / matrix lookup failed for %s\n", k.w.c_str());
+                return false;
             }
-            op.scale_src = e->wvec(c.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = c.cout;
+            op.scale_src[slot] = e->wvec(c.scale); op.scale16[slot] = e->scale16_arena() + e->scale16_used; op.scale_n[slot] = c.cout;
             e->scale16_used += n16;
             s.kind = KIND_F16X3;
             s.w_hi = e->whi16(c.w + o.w_off); s.w_lo = e->wlo16(c.w + o.w_off);
-            s.scale = op.scale16;
+            s.scale = op.scale16[slot];
             s.range_flag = e->buf<int>("range_flag");
         } else {
             s.kind = KIND_TF32X3;
             s.w_hi = e->wmat(c.w + o.w_off); s.w_lo = e->wlo(c.w + o.w_off);
             s.scale = e->wvec(c.scale);
         }
-        s.y = y; s.y_pix_stride = ystride;
-        const int Ho = conv_out(H, c.k, stride, kpad), Wo = conv_out(W, c.k, stride, kpad);
+        s.y = k.y; s.y_pix_stride = k.ystride;
+        const int Ho = conv_out(k.H, c.k, k.stride, k.pad), Wo = conv_out(k.W, c.k, k.stride, k.pad);
         // fp16 hi/lo plane hand-over (kind::f16 only): the fp32 buffer of N*H*W*C floats holds the two fp16 planes back to back
-        if (o.planes_in) s.x_lo = reinterpret_cast<const __half*>(x) + (size_t)N * H * W * c.cin;
-        if (o.planes_out) s.y_lo = reinterpret_cast<__half*>(y) + (size_t)N * Ho * Wo * c.cout;
+        if (o.planes_in) s.x_lo = reinterpret_cast<const __half*>(k.x) + (size_t)k.N * k.H * k.W * c.cin;
+        if (o.planes_out) s.y_lo = reinterpret_cast<__half*>(k.y) + (size_t)k.N * Ho * Wo * c.cout;
         s.out_h = o.out_h; s.out_w = o.out_w; s.out_step = o.out_step; s.out_y0 = o.out_y0; s.out_x0 = o.out_x0;
         s.residual = o.res; s.res_pix_stride = c.cout; s.up_src = o.up; s.up_h = o.up_h; s.up_w = o.up_w;
-        s.res_mode = o.res_mode; s.relu = relu ? 1 : 0; s.sigmoid_ch = o.sigmoid_ch; s.passes = e->cfg.passes;
+        s.res_mode = o.res_mode; s.relu = k.relu ? 1 : 0; s.sigmoid_ch = o.sigmoid_ch; s.passes = e->cfg.passes;
         s.im_stride = img_stride;
+        op.flops += 2.0 * (double)k.N * Ho * Wo * c.flop_cout * c.flop_cin * (o.ntaps > 0 ? o.ntaps : c.k * c.k);
+        return true;
+    }
+    // one launch of c, or with phase1: one launch of c whose residual is phase1's result (RES_STAGED; c's own residual options are not
+    // used).  When the two need different tile shapes, phase 1 runs as a launch of its own into c's output, which c then adds in place
+    // (RES_TILE on its own output, tile by tile).
+    void conv(int stage, const ConvCall& c, const ConvCall* phase1 = nullptr) {
+        Op op;
         op.stage = stage; op.kind = 0; op.fn = -1;
-        op.flops = 2.0 * (double)N * Ho * Wo * c.flop_cout * c.flop_cin * (o.ntaps > 0 ? o.ntaps : c.k * c.k);
-        if (!conv_build(s, &op.conv)) { ok = false; fprintf(stderr, "[detectorch_b200] engine: conv_build failed for %s\n", wname.c_str()); }
+        ConvSpec s, s1;
+        if (!spec(c, op, 0, s) || (phase1 && !spec(*phase1, op, 1, s1))) { ok = false; return; }
+        if (phase1) {
+            s.res_mode = RES_STAGED; s.phase1 = &s1;
+            if (!conv_staged_ok(s)) {
+                ConvCall p1 = *phase1;
+                p1.y = c.y; p1.ystride = c.ystride;
+                conv(stage, p1);
+                ConvCall p2 = c;
+                p2.o.res_mode = RES_TILE; p2.o.res = c.y;
+                conv(stage, p2);
+                return;
+            }
+        }
+        if (!conv_build(s, &op.conv)) { ok = false; fprintf(stderr, "[detectorch_b200] engine: conv_build failed for %s\n", c.w.c_str()); }
         e->ops.push_back(op);
+    }
+    void conv(int stage, const std::string& wname, const float* x, int N, int H, int W, int xstride, float* y, int ystride, int kpad,
+              int stride, bool relu, const ConvOpt& o = ConvOpt()) {
+        conv(stage, ConvCall{wname, x, N, H, W, xstride, y, ystride, kpad, stride, relu, o});
     }
     void fn(int stage, StageFn f) {
         Op op;
@@ -707,10 +739,10 @@ void add_stem(ProgBuilder& pb, bool f16) {
     op.flops = 2.0 * (double)B * e->H1 * e->W1 * sw.flop_cout * sw.flop_cin;
     bool ok;
     if (f16) {
-        op.matrix = e->matrix_of(sw.w);
-        op.scale_src = e->wvec(sw.scale); op.scale16 = e->scale16_arena() + e->scale16_used; op.scale_n = 64;
+        op.matrix[0] = e->matrix_of(sw.w);
+        op.scale_src[0] = e->wvec(sw.scale); op.scale16[0] = e->scale16_arena() + e->scale16_used; op.scale_n[0] = 64;
         e->scale16_used += 64;
-        ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w), e->wlo16(sw.w), op.scale16, e->wvec(sw.shift),
+        ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->whi16(sw.w), e->wlo16(sw.w), op.scale16[0], e->wvec(sw.shift),
                              e->buf("c1"), c.passes, &op.conv, KIND_F16X3, e->buf<int>("range_flag"));
     } else {
         ok = conv_build_stem(e->buf("stem_x4"), B, e->Hp, e->Wp, e->H1, e->W1, e->wmat(sw.w), e->wlo(sw.w), e->wvec(sw.scale), e->wvec(sw.shift),
@@ -742,13 +774,17 @@ const float* add_layer(ProgBuilder& pb, int stage, const std::string& pre, int l
         // round trip (16 KB read + 16 KB written per k-block) and their issue slots in the epilogue-bound conv3
         ConvOpt o2; o2.planes_in = handover; o2.planes_out = handover;
         pb.conv(stage, wp + "conv2", e->buf(p + ".t1"), N, ho, wo, planes, e->buf(p + ".t2"), planes, 1, 1, true, o2);
-        const float* idt = x;
+        ConvOpt o3; o3.planes_in = handover;
+        const ConvCall c3{wp + "conv3", e->buf(p + ".t2"), N, ho, wo, planes, e->buf(p + ".out"), planes * 4, 0, 1, true, o3};
         if (b == 0) {
-            pb.conv(stage, wp + "downsample.0", x, N, h, w, cin, e->buf(p + ".ds"), planes * 4, 0, stride, false);
-            idt = e->buf(p + ".ds");
+            // the downsample is conv3's phase 1: its result stays on chip as conv3's residual
+            const ConvCall ds{wp + "downsample.0", x, N, h, w, cin, e->buf(p + ".out"), planes * 4, 0, stride, false, ConvOpt()};
+            pb.conv(stage, c3, &ds);
+        } else {
+            ConvCall c3r = c3;
+            c3r.o.res_mode = RES_TILE; c3r.o.res = x;
+            pb.conv(stage, c3r);
         }
-        ConvOpt o3; o3.res_mode = RES_TILE; o3.res = idt; o3.planes_in = handover;
-        pb.conv(stage, wp + "conv3", e->buf(p + ".t2"), N, ho, wo, planes, e->buf(p + ".out"), planes * 4, 0, 1, true, o3);
         x = e->buf(p + ".out");
         h = ho; w = wo;
     }
@@ -858,16 +894,16 @@ void add_mask_head(ProgBuilder& pb) {
         mx = add_layer(pb, ST_MASK_HEAD, "m5", 4, mx, D, h, w, false);
     } else {
         // The mask logits carry the tightest parity bar (1e-4 absolute) and sit behind four K = 2304 convolutions, where the tensor
-        // core's truncating fp32 accumulate is the error floor.  The chains are shortened by SPLITTING K: each 3x3 convolution runs as
-        // two launches over filter taps [0,5) and [5,9); the second adds the first's fp32 result in its epilogue (RES_TILE on the output
-        // buffer itself, round-to-nearest) before the ReLU.
+        // core's truncating fp32 accumulate is the error floor.  The chains are shortened by SPLITTING K: each 3x3 convolution runs
+        // filter taps [0,5) as phase 1 and [5,9) as phase 2 of one launch; phase 2's epilogue adds phase 1's fp32 result
+        // (round-to-nearest) before the ReLU.
         for (int i = 1; i <= 4; ++i) {
             const std::string wn = "mask_head.conv_head.fcn" + std::to_string(i);
             float* my = e->buf("mask_c" + std::to_string(i));
             ConvOpt lo; lo.ntaps = 5;
-            pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, lo);
-            ConvOpt hi; hi.res_mode = RES_TILE; hi.res = my; hi.tap0 = 5; hi.ntaps = 4; hi.zero_shift = true;
-            pb.conv(ST_MASK_HEAD, wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, hi);
+            ConvOpt hi; hi.tap0 = 5; hi.ntaps = 4; hi.zero_shift = true;
+            const ConvCall first{wn, mx, D, 14, 14, 256, my, 256, 1, 1, false, lo};
+            pb.conv(ST_MASK_HEAD, ConvCall{wn, mx, D, 14, 14, 256, my, 256, 1, 1, true, hi}, &first);
             mx = my;
         }
     }
@@ -1051,8 +1087,9 @@ int dt_engine_finalize_weights(dt_engine_t h, dt_stream_t stream) {
                 e->wmat(e->matrices[m].first), (long long)e->matrices[m].second, e->matinfo() + m, e->whi16(e->matrices[m].first),
                 e->wlo16(e->matrices[m].first));
         for (const Op& op : e->ops)
-            if (op.kind == 0 && op.scale16)
-                scale16_kernel<<<(op.scale_n + 255) / 256, 256, 0, st>>>(op.scale_src, e->matinfo() + op.matrix, op.scale16, op.scale_n);
+            for (int m = 0; m < 2; ++m)
+                if (op.kind == 0 && op.scale16[m])
+                    scale16_kernel<<<(op.scale_n[m] + 255) / 256, 256, 0, st>>>(op.scale_src[m], e->matinfo() + op.matrix[m], op.scale16[m], op.scale_n[m]);
         DT_CHECK_CUDA(cudaGetLastError());
     }
     return 1;

@@ -460,6 +460,34 @@ extern "C" int dt_conv2d_nhwc_f16x3(const float* x, int N, int H, int W, int Cin
                             res_mode, up_src, up_h, up_w, relu, sigmoid_ch, passes, force_block_n, range_flag, y, y_pix_stride, stream);
 }
 
+extern "C" int dt_conv2d_nhwc_two_phase(int kind, const dt_conv_operand* phase1, const dt_conv_operand* phase2, const float* residual, int N,
+                                        int Cout, int relu, int passes, int force_block_n, int* range_flag, const float* im_info, int im_stride,
+                                        float* y, dt_stream_t stream) {
+    if (!phase2 || (phase1 && residual) || (kind != KIND_TF32X3 && kind != KIND_F16X3)) {
+        fprintf(stderr, "dt_conv2d_nhwc_two_phase: phase 2 is required, a residual excludes phase 1, kind is 0 or 1\n");
+        return 0;
+    }
+    auto spec = [&](const dt_conv_operand& o) {
+        ConvSpec s;
+        memset(&s, 0, sizeof(s));
+        s.x = o.x; s.N = N; s.H = o.H; s.W = o.W; s.Cin = o.Cin; s.x_pix_stride = o.Cin;
+        s.w_hi = o.w_hi; s.w_lo = o.w_lo; s.kind = kind; s.range_flag = range_flag;
+        s.Cout = Cout; s.kh = o.kh; s.kw = o.kw; s.pad = o.pad; s.stride = o.stride; s.tap0 = o.tap0; s.ntaps = o.ntaps;
+        s.scale = o.scale; s.shift = o.shift; s.passes = passes;
+        s.precise = force_block_n < 0; s.force_block_n = force_block_n < 0 ? 0 : force_block_n;
+        return s;
+    };
+    ConvSpec s = spec(*phase2), s1;
+    s.y = y; s.y_pix_stride = Cout; s.relu = relu; s.im_stride = im_stride;
+    if (phase1) { s1 = spec(*phase1); s.res_mode = RES_STAGED; s.phase1 = &s1; }
+    else if (residual) { s.res_mode = RES_TILE; s.residual = residual; s.res_pix_stride = Cout; }
+    ConvLayer L;
+    if (!conv_build(s, &L)) return 0;
+    L.p.im_info = im_stride > 0 ? im_info : nullptr;
+    DT_CHECK_CUDA(conv_launch(L, (cudaStream_t)stream));
+    return 1;
+}
+
 // ================================================================================== mask paste + COCO RLE (segm_results)
 namespace {
 constexpr int kSegmCharsPerRun = 4;     // staging bytes per run (maskApi's worst case is 7; typical masks need 1-2)

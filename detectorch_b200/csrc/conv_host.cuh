@@ -129,6 +129,10 @@ struct ConvSpec {
     // optional output remap (transposed conv): pixel (n,h,w) is written at y + ((n*Hy + h*ys + yo)*Wy + w*ys + xo)*y_pix_stride
     int out_h, out_w, out_step, out_y0, out_x0;   // out_step==0 -> plain [N,Ho,Wo]
     const float* residual; int res_pix_stride;    // RES_TILE: same geometry as the (plain) output
+    // RES_STAGED: the convolution whose result is the residual, run by the same launch (phase 1; its x, N, H, W, Cin, x_pix_stride,
+    // weights, filter geometry, taps, scale and shift are read; the output, kind and passes are this spec's).  It must give the same
+    // output extents and, by conv_tile, the same tile shape; its input is fp32.
+    const ConvSpec* phase1;
     const float* up_src; int up_h, up_w;          // RES_UPSAMPLE2X
     int res_mode, relu, sigmoid_ch, passes;
     // fp16 hi/lo plane hand-over between two KIND_F16X3 layers (dense channel stride only): x / y then point at the HIGH plane and
@@ -167,6 +171,43 @@ inline void finish_grid(ConvLayer* L, int n_tiles) {
     L->valid = true;
 }
 
+// Tile width and rotating main-term accumulators of a convolution.
+// Tiles are at most 128 channels wide: the main and cross accumulators of a 64 x 128 warpgroup tile are 128 registers per thread,
+// which is what the register file leaves with two MMA warpgroups per SM.  A wider request (256) runs as 128-wide tiles.
+inline void conv_tile(const ConvSpec& s, int* block_n, int* nmain) {
+    int bn = s.force_block_n;
+    if (bn == 0 || bn > 128) bn = s.Cout > 64 ? 128 : 64;
+    // tf32 k-steps are half as long as fp16 ones: a long-K tf32 layer's accumulation chain is twice as long, and the 3xTF32 engine met the
+    // 1e-4 mask-logit bar only with the main term rotated over three accumulators (64-wide tiles)
+    if (s.precise || (s.kind != KIND_F16X3 && s.kh * s.kw * (s.Cin / 32) > 16)) bn = 64;
+    // 64-wide tiles rotate the main term over 3 accumulators (same register budget as one 128-wide pair) -- except at K <= 256, where
+    // one accumulator already is a chain of at most 16 k-blocks
+    const int ntaps = s.ntaps > 0 ? s.ntaps : s.kh * s.kw;
+    *block_n = bn;
+    *nmain = (bn == 64 && (s.precise || ntaps * (s.Cin / 32) > 8)) ? 3 : 1;
+}
+
+// The phase-1 spec of a RES_STAGED launch as a launch of its own into the same output (what conv_build checks it against)
+inline ConvSpec phase1_as_launch(const ConvSpec& s) {
+    ConvSpec t = *s.phase1;
+    t.kind = s.kind; t.range_flag = s.range_flag; t.passes = s.passes; t.force_block_n = s.force_block_n; t.precise = s.precise;
+    t.y = s.y; t.y_pix_stride = s.y_pix_stride; t.y_lo = nullptr; t.out_step = 0;
+    t.res_mode = RES_NONE; t.relu = 0; t.sigmoid_ch = 0; t.im_stride = 0; t.phase1 = nullptr;
+    return t;
+}
+
+// Whether a RES_STAGED launch can serve the spec: phase 1 has the same tile shape and output extents, fp32 input, and phase 2 writes
+// a plain fp32 output.  Equal extents give equal boxes (choose_box) while both strides allow 128-pixel-wide boxes.
+inline bool conv_staged_ok(const ConvSpec& s) {
+    if (!s.phase1 || s.phase1->x_lo || s.y_lo || s.out_step != 0) return false;
+    const ConvSpec t = phase1_as_launch(s);
+    int bn, nm, bn1, nm1;
+    conv_tile(s, &bn, &nm);
+    conv_tile(t, &bn1, &nm1);
+    return bn == bn1 && nm == nm1 && t.Cout == s.Cout && t.N == s.N && (t.H + 2 * t.pad - t.kh) / t.stride == (s.H + 2 * s.pad - s.kh) / s.stride &&
+           (t.W + 2 * t.pad - t.kw) / t.stride == (s.W + 2 * s.pad - s.kw) / s.stride && 256 / t.stride >= 128 && 256 / s.stride >= 128;
+}
+
 inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     memset(&L->p, 0, sizeof(ConvParams));
     ConvParams& p = L->p;
@@ -178,13 +219,8 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     const int Wo = (s.W + 2 * s.pad - s.kw) / s.stride + 1;
     int wbox, hbox, nbox;
     choose_box(Wo, Ho, s.N, 256 / s.stride, &wbox, &hbox, &nbox);
-    // Tiles are at most 128 channels wide: the main and cross accumulators of a 64 x 128 warpgroup tile are 128 registers per thread,
-    // which is what the register file leaves with two MMA warpgroups per SM.  A wider request (256) runs as 128-wide tiles.
-    int bn = s.force_block_n;
-    if (bn == 0 || bn > 128) bn = s.Cout > 64 ? 128 : 64;
-    // tf32 k-steps are half as long as fp16 ones: a long-K tf32 layer's accumulation chain is twice as long, and the 3xTF32 engine met the
-    // 1e-4 mask-logit bar only with the main term rotated over three accumulators (64-wide tiles)
-    if (s.precise || (s.kind != KIND_F16X3 && s.kh * s.kw * (s.Cin / 32) > 16)) bn = 64;
+    int bn, nmain;
+    conv_tile(s, &bn, &nmain);
     if (bn != 64 && bn != 128) { fprintf(stderr, "[detectorch_b200] conv_build: unsupported tile width %d\n", bn); return false; }
     L->block_n = bn;
     const int K = s.kh * s.kw * s.Cin;
@@ -246,9 +282,20 @@ inline bool conv_build(const ConvSpec& s, ConvLayer* L) {
     p.relu = s.relu; p.sigmoid_ch = s.sigmoid_ch; p.res_mode = s.res_mode;
     p.passes = s.passes == 1 ? 1 : 3;
     p.im_stride = s.out_step == 0 ? s.im_stride : 0;
-    // 64-wide tiles rotate the main term over 3 accumulators (same register budget as one 128-wide pair) -- except at K <= 256, where
-    // one accumulator already is a chain of at most 16 k-blocks
-    L->nmain = (bn == 64 && (s.precise || p.ntaps * p.cin_blocks > 8)) ? 3 : 1;
+    L->nmain = nmain;
+    if (s.res_mode == RES_STAGED) {
+        // phase 1 is built as a launch of its own into the same output; its operands then move into this launch
+        ConvLayer L1;
+        if (!conv_staged_ok(s) || !conv_build(phase1_as_launch(s), &L1) || L1.p.wbox != wbox || L1.p.hbox != hbox || L1.p.nbox != nbox) {
+            fprintf(stderr, "[detectorch_b200] conv_build: the two phases need the same output, tile shape and box, fp32 phase-1 input and a "
+                            "plain fp32 output\n");
+            return false;
+        }
+        p.tm_a1 = L1.p.tm_a; p.tm_bhi1 = L1.p.tm_bhi; p.tm_blo1 = L1.p.tm_blo;
+        p.scale1 = L1.p.scale; p.shift1 = L1.p.shift;
+        p.cin_blocks1 = L1.p.cin_blocks; p.kw1 = L1.p.kw; p.tap01 = L1.p.tap0; p.ntaps1 = L1.p.ntaps;
+        p.pad1 = L1.p.pad_w; p.stride1 = L1.p.stride_w;
+    }
     finish_grid(L, ceil_div(s.Cout, bn));
     return true;
 }
@@ -301,24 +348,31 @@ inline bool conv_build_stem(const float* x4, int B, int Hp, int Wp, int H1, int 
     return true;
 }
 
-template <int BN, int NM, int KIND, bool MASK>
+template <int BN, int NM, int KIND, bool MASK, bool STAGED>
 inline cudaError_t conv_launch_cfg(const ConvLayer& L, cudaStream_t stream) {
     using Cfg = ConvCfg<BN, NM, KIND>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e =
+            cudaFuncSetAttribute(conv_wgmma_kernel<BN, NM, KIND, MASK, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    conv_wgmma_kernel<BN, NM, KIND, MASK><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
+    conv_wgmma_kernel<BN, NM, KIND, MASK, STAGED><<<L.grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(L.p);
     return cudaGetLastError();
+}
+
+template <int KIND, bool MASK, bool STAGED>
+inline cudaError_t conv_launch_tile(const ConvLayer& L, cudaStream_t stream) {
+    if (L.block_n == 64)
+        return L.nmain == 3 ? conv_launch_cfg<64, 3, KIND, MASK, STAGED>(L, stream) : conv_launch_cfg<64, 1, KIND, MASK, STAGED>(L, stream);
+    if (L.block_n == 128 && L.nmain == 1) return conv_launch_cfg<128, 1, KIND, MASK, STAGED>(L, stream);
+    return cudaErrorInvalidValue;
 }
 
 template <int KIND, bool MASK>
 inline cudaError_t conv_launch_kind(const ConvLayer& L, cudaStream_t stream) {
-    if (L.block_n == 64) return L.nmain == 3 ? conv_launch_cfg<64, 3, KIND, MASK>(L, stream) : conv_launch_cfg<64, 1, KIND, MASK>(L, stream);
-    if (L.block_n == 128 && L.nmain == 1) return conv_launch_cfg<128, 1, KIND, MASK>(L, stream);
-    return cudaErrorInvalidValue;
+    return L.p.res_mode == RES_STAGED ? conv_launch_tile<KIND, MASK, true>(L, stream) : conv_launch_tile<KIND, MASK, false>(L, stream);
 }
 
 inline cudaError_t conv_launch(const ConvLayer& L, cudaStream_t stream) {

@@ -34,7 +34,10 @@
 //   warpgroups 1-2 MMA + epilogue, rows [0, 64) and [64, 128) of the tile: operand split, wgmma, then scale/shift [+residual]
 //                  [ReLU|sigmoid] -> swizzled staging area -> TMA store.  The producer runs ahead into the next tile while a tile
 //                  drains, and the stores of a tile overlap the main loop of the next.  A RES_TILE layer loads the residual tile into the
-//                  staging area during the main loop, as soon as the previous tile's stores have read it.
+//                  staging area during the main loop, as soon as the previous tile's stores have read it.  A RES_STAGED layer computes
+//                  its residual instead: each work item first runs phase 1, a convolution of its own (a downsample, or the first taps of a
+//                  K-split), whose scale/shift epilogue writes the staging area, then the layer itself, whose epilogue adds the staged tile
+//                  exactly where a RES_TILE launch adds the loaded one.  The residual map never goes through HBM.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -42,7 +45,7 @@
 
 namespace dt {
 
-enum ConvResidualMode { RES_NONE = 0, RES_TILE = 1, RES_UPSAMPLE2X = 2 };
+enum ConvResidualMode { RES_NONE = 0, RES_TILE = 1, RES_UPSAMPLE2X = 2, RES_STAGED = 3 };
 enum ConvKind { KIND_TF32X3 = 0, KIND_F16X3 = 1 };
 
 struct ConvParams {
@@ -53,6 +56,12 @@ struct ConvParams {
     CUtensorMap tm_r;      // 4D residual, same geometry as tm_d (RES_TILE only)
     CUtensorMap tm_a2;     // a_planes: the fp16 LOW plane of the input (tm_a is then the fp16 HIGH plane), SWIZZLE_64B boxes of 32 channels
     CUtensorMap tm_d2;     // out_planes: the fp16 LOW plane of the output (tm_d the HIGH plane), SWIZZLE_64B boxes of 32 channels
+    // RES_STAGED phase 1: fp32 input, weights, scale / shift and filter geometry of the convolution whose result is the residual.  Its A
+    // box is the output box like phase 2's, so a stage carries the same bytes in both phases.
+    CUtensorMap tm_a1, tm_bhi1, tm_blo1;
+    const float* scale1;
+    const float* shift1;
+    int cin_blocks1, kw1, tap01, ntaps1, pad1, stride1;
     const float* scale;    // [Cout] per-channel scale (folded BN gain, or 1)
     const float* shift;    // [Cout] per-channel shift (folded BN bias, or conv bias)
     const float* up_src;   // RES_UPSAMPLE2X: coarser NHWC map [N, up_h, up_w, Cout]
@@ -134,8 +143,9 @@ __device__ __forceinline__ void split_f16x2(float2 v, uint32_t& hi, uint32_t& lo
 }
 
 // MASK: the launch zeroes pixels outside each image (p.im_info non-null); a separate instantiation, so that the epilogue of every other
-// launch is the plain one
-template <int BLOCK_N, int NMAIN, int KIND, bool MASK>
+// launch is the plain one.  STAGED: a RES_STAGED launch (p.res_mode); likewise separate, so that every other launch runs one code
+// instance of the main loop.
+template <int BLOCK_N, int NMAIN, int KIND, bool MASK, bool STAGED>
 __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     using Cfg = ConvCfg<BLOCK_N, NMAIN, KIND>;
     constexpr int STAGES = Cfg::STAGES;
@@ -155,6 +165,7 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
     const int lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
     const int num_kb = p.ntaps * p.cin_blocks;           // pipeline steps per tile: one k-block = 32 channels of one filter tap
+    const int num_kb1 = STAGED ? p.ntaps1 * p.cin_blocks1 : 0;   // RES_STAGED: phase-1 k-blocks, run before those
     const int num_tiles = p.m_tiles * p.n_tiles;
 
     if (threadIdx.x == 0) {
@@ -163,6 +174,11 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
         if (p.passes == 3) tma_prefetch_desc(&p.tm_blo);
         tma_prefetch_desc(&p.tm_d);
         if (p.res_mode == RES_TILE) tma_prefetch_desc(&p.tm_r);
+        if (STAGED) {
+            tma_prefetch_desc(&p.tm_a1);
+            tma_prefetch_desc(&p.tm_bhi1);
+            if (p.passes == 3) tma_prefetch_desc(&p.tm_blo1);
+        }
         if (p.a_planes) tma_prefetch_desc(&p.tm_a2);
         if (p.out_planes) tma_prefetch_desc(&p.tm_d2);
         for (int s = 0; s < STAGES; ++s) {
@@ -192,26 +208,32 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
             for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
                 int w0, h0, n0img, n0;
                 tile_of(item, w0, h0, n0img, n0);
-                for (int kb = 0; kb < num_kb; ++kb, ++it) {
+                // phase-1 k-blocks (RES_STAGED), then the layer's own, on one stage ring
+                for (int kbt = 0; kbt < num_kb1 + num_kb; ++kbt, ++it) {
                     const int s = it % STAGES;
                     mbar_wait(bar_empty(s), ((it / STAGES) & 1u) ^ 1u);
-                    const int tap_l = kb / p.cin_blocks;
-                    const int cb = kb - tap_l * p.cin_blocks;
-                    const int tap = p.tap0 + tap_l;
-                    const int kbg = tap * p.cin_blocks + cb;        // k-block index into the full weight row
-                    const int fy = tap / p.kw, fx = tap - fy * p.kw;
-                    const int xw = w0 * p.stride_w + fx - p.pad_w, xh = h0 * p.stride_h + fy - p.pad_h;
+                    const bool ph1 = STAGED && kbt < num_kb1;
+                    const int kb = ph1 ? kbt : kbt - num_kb1;
+                    const int cin_blocks = ph1 ? p.cin_blocks1 : p.cin_blocks, kw = ph1 ? p.kw1 : p.kw;
+                    const int tap_l = kb / cin_blocks;
+                    const int cb = kb - tap_l * cin_blocks;
+                    const int tap = (ph1 ? p.tap01 : p.tap0) + tap_l;
+                    const int kbg = tap * cin_blocks + cb;        // k-block index into the full weight row
+                    const int fy = tap / kw, fx = tap - fy * kw;
+                    const int xw = ph1 ? w0 * p.stride1 + fx - p.pad1 : w0 * p.stride_w + fx - p.pad_w;
+                    const int xh = ph1 ? h0 * p.stride1 + fy - p.pad1 : h0 * p.stride_h + fy - p.pad_h;
                     const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
                     mbar_arrive_expect_tx(bar_full(s), tx_bytes);
-                    if (KIND == KIND_F16X3 && p.a_planes) {
+                    if (KIND == KIND_F16X3 && !ph1 && p.a_planes) {
                         // fp16 planes: the two operand tiles land where the fp32 tile would have landed
                         tma_load_4d(st, &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
                         tma_load_4d(st + Cfg::A_BYTES / 2, &p.tm_a2, bar_full(s), cb * 32, xw, xh, n0img);
                     } else {
-                        tma_load_4d(st, &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
+                        tma_load_4d(st, ph1 ? &p.tm_a1 : &p.tm_a, bar_full(s), cb * 32, xw, xh, n0img);
                     }
-                    tma_load_2d(st + Cfg::A_STAGE_BYTES, &p.tm_bhi, bar_full(s), kbg * 32, n0);
-                    if (p.passes == 3) tma_load_2d(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES, &p.tm_blo, bar_full(s), kbg * 32, n0);
+                    tma_load_2d(st + Cfg::A_STAGE_BYTES, ph1 ? &p.tm_bhi1 : &p.tm_bhi, bar_full(s), kbg * 32, n0);
+                    if (p.passes == 3)
+                        tma_load_2d(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES, ph1 ? &p.tm_blo1 : &p.tm_blo, bar_full(s), kbg * 32, n0);
                 }
             }
         }
@@ -249,170 +271,209 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
         tile_of(item, w0, h0, n0img, n0);
         int nlive = (p.cout - n0 + 31) / 32;       // chunks past the true Cout are neither computed nor stored
         nlive = nlive > Cfg::NCHUNK ? Cfg::NCHUNK : nlive;
+        // SWIZZLE_128B fp32 staging chunk: 16-byte piece (col % 32) / 4 of the row, XOR (row mod 8)
+        auto off32_of = [](int row, int col) { return row * 128 + ((((col & 31) >> 2) ^ (row & 7)) << 4) + ((col & 3) << 2); };
+        // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1);
+        // its rows are tile rows trow (+ 8).  The scale/shift value of pair i0 = 4 j + 2 hr (channels ch, ch + 1):
+        const int cq = 2 * (lane & 3);
+        auto scaled = [&](int i0, int ch, const float* scale, const float* shift) {
+            float v0 = accx[i0], v1 = accx[i0 + 1];
+            if (p.passes != 3) { v0 = 0.f; v1 = 0.f; }
 #pragma unroll
-        for (int i = 0; i < R; ++i) {
-            accx[i] = 0.f;
-#pragma unroll
-            for (int a = 0; a < NMAIN; ++a) acc[a][i] = 0.f;
-        }
-        // RES_TILE: the residual tile goes to the staging area while the main loop runs, once the previous tile's stores have read it.
-        // Called after the first k-block's MMAs are issued, so that waiting for those stores overlaps tensor-core work.
-        auto prefetch_residual = [&]() {
-            if (p.res_mode == RES_TILE && ct == 0) {
-                tma_store_wait_read0();
-                mbar_arrive_expect_tx(bar_res, (uint32_t)(nlive * p.a_tile_bytes));
-                for (int c = 0; c < nlive; ++c) tma_load_4d(epi_base + c * Cfg::A_BYTES, &p.tm_r, bar_res, n0 + c * 32, w0, h0, n0img);
+            for (int a = 0; a < NMAIN; ++a) { v0 += acc[a][i0]; v1 += acc[a][i0 + 1]; }
+            float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
+            if (ch < p.cout) {                  // cout % 4 == 0 and ch is even: ch + 1 < cout too
+                sc = __ldg(reinterpret_cast<const float2*>(scale + ch));
+                sh = __ldg(reinterpret_cast<const float2*>(shift + ch));
             }
+            return make_float2(fmaf(v0, sc.x, sh.x), fmaf(v1, sc.y, sh.y));
         };
-        int prev_s = -1;
-        if constexpr (KIND == KIND_F16X3) {
-            // one k-block into fragment buffer B: wait for the stage, load A into registers, one uninterrupted batch of wgmmas, then
-            // retire the previous k-block's batch (whose fragment buffer the next k-block rewrites) and hand its stage back
-            auto kblock = [&](auto B, int kb) {
-                constexpr int b = decltype(B)::value;
-                const int s = it % STAGES;
-                mbar_wait(bar_full(s), (it / STAGES) & 1u);
-                const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
-                const uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
-                if (!p.a_planes) {
-                    // fragment register (hr + 2 (j % 2)) of k-step j / 2 = the float2 of channels 8 j + 2 (l % 4) of row trow + 8 hr
-                    float2 v[2][4];
+        // One GEMM phase into the accumulators, from zero and k-block 0 (the NMAIN == 3 rotation restarts as in a launch of its own):
+        // PH 0 = RES_STAGED's phase 1 (fp32 A), PH 1 = the layer.  A code instance per phase keeps the layer's main loop what it was
+        // (one runtime-selected instance does not fit the register budget).
+        auto run_phase = [&](auto PH) {
+            constexpr bool P1 = decltype(PH)::value == 0;
+            const int nkb = P1 ? num_kb1 : num_kb;
+            const bool planes = !P1 && p.a_planes;
 #pragma unroll
-                    for (int hr = 0; hr < 2; ++hr)
+            for (int i = 0; i < R; ++i) {
+                accx[i] = 0.f;
 #pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                            v[hr][j] = *reinterpret_cast<const float2*>(st_gen + a32_off + hr * 1024 + (((2 * j) ^ a32_x) << 4));
-#pragma unroll
-                    for (int hr = 0; hr < 2; ++hr) {
-                        bool b_hr = false;
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            split_f16x2(v[hr][j], fh[b][j >> 1][hr + 2 * (j & 1)], fl[b][j >> 1][hr + 2 * (j & 1)]);
-                            b_hr = b_hr || !(fabsf(v[hr][j].x) < 65504.f) || !(fabsf(v[hr][j].y) < 65504.f);
-                        }
-                        // rows past the TMA box (boxes smaller than 128 pixels) hold stale data: their accumulator rows are never stored,
-                        // and they must not raise the range flag
-                        bad = bad || (b_hr && (hr == 0 ? live0 : live1));
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < Cfg::KSTEPS; ++k) {
-                        const uint32_t a = st + lm_off + ((uint32_t)((2 * k + lm_k) ^ lm_x) << 4);
-                        ldmatrix_x4(fh[b][k], a);
-                        ldmatrix_x4(fl[b][k], a + Cfg::A_BYTES / 2);
-                    }
+                for (int a = 0; a < NMAIN; ++a) acc[a][i] = 0.f;
+            }
+            // RES_TILE: the residual tile goes to the staging area while the main loop runs, once the previous tile's stores have read it.
+            // Called after the first k-block's MMAs are issued, so that waiting for those stores overlaps tensor-core work.
+            auto prefetch_residual = [&]() {
+                if (p.res_mode == RES_TILE && ct == 0) {
+                    tma_store_wait_read0();
+                    mbar_arrive_expect_tx(bar_res, (uint32_t)(nlive * p.a_tile_bytes));
+                    for (int c = 0; c < nlive; ++c) tma_load_4d(epi_base + c * Cfg::A_BYTES, &p.tm_r, bar_res, n0 + c * 32, w0, h0, n0img);
                 }
-                const uint64_t dbh = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES);
-                const uint64_t dbl = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
-                // the same MMA sequence per k-step as the three-term product always ran: cross terms A_l B_h, A_h B_l, then the main term
-                auto batch = [&](float (&am)[R]) {
-                    if (p.passes == 3) {
-                        wgmma_fence();
+            };
+            int prev_s = -1;
+            if constexpr (KIND == KIND_F16X3) {
+                // one k-block into fragment buffer B: wait for the stage, load A into registers, one uninterrupted batch of wgmmas, then
+                // retire the previous k-block's batch (whose fragment buffer the next k-block rewrites) and hand its stage back
+                auto kblock = [&](auto B, int kb) {
+                    constexpr int b = decltype(B)::value;
+                    const int s = it % STAGES;
+                    mbar_wait(bar_full(s), (it / STAGES) & 1u);
+                    const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+                    const uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
+                    if (!planes) {
+                        // fragment register (hr + 2 (j % 2)) of k-step j / 2 = the float2 of channels 8 j + 2 (l % 4) of row trow + 8 hr
+                        float2 v[2][4];
+#pragma unroll
+                        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                            for (int j = 0; j < 4; ++j)
+                                v[hr][j] = *reinterpret_cast<const float2*>(st_gen + a32_off + hr * 1024 + (((2 * j) ^ a32_x) << 4));
+#pragma unroll
+                        for (int hr = 0; hr < 2; ++hr) {
+                            bool b_hr = false;
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                split_f16x2(v[hr][j], fh[b][j >> 1][hr + 2 * (j & 1)], fl[b][j >> 1][hr + 2 * (j & 1)]);
+                                b_hr = b_hr || !(fabsf(v[hr][j].x) < 65504.f) || !(fabsf(v[hr][j].y) < 65504.f);
+                            }
+                            // rows past the TMA box (boxes smaller than 128 pixels) hold stale data: their accumulator rows are never stored,
+                            // and they must not raise the range flag
+                            bad = bad || (b_hr && (hr == 0 ? live0 : live1));
+                        }
+                    } else {
 #pragma unroll
                         for (int k = 0; k < Cfg::KSTEPS; ++k) {
-                            const uint64_t koff = (uint64_t)(k * 32 >> 4);
-                            conv_mma_f16<BLOCK_N>(accx, fl[b][k], dbh + koff);
-                            conv_mma_f16<BLOCK_N>(accx, fh[b][k], dbl + koff);
-                            conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + koff);
+                            const uint32_t a = st + lm_off + ((uint32_t)((2 * k + lm_k) ^ lm_x) << 4);
+                            ldmatrix_x4(fh[b][k], a);
+                            ldmatrix_x4(fl[b][k], a + Cfg::A_BYTES / 2);
                         }
-                        wgmma_commit();
-                    } else {
-                        wgmma_fence();
-#pragma unroll
-                        for (int k = 0; k < Cfg::KSTEPS; ++k) conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + (uint64_t)(k * 32 >> 4));
-                        wgmma_commit();
                     }
-                };
-                // NMAIN == 3 rotates the main term over three accumulators by k-block (see the tf32 loop)
-                if constexpr (NMAIN == 1) {
-                    batch(acc[0]);
-                } else {
-                    const int sel = kb % 3;
-                    if (sel == 0) batch(acc[0]);
-                    else if (sel == 1) batch(acc[NMAIN > 1 ? 1 : 0]);
-                    else batch(acc[NMAIN > 2 ? 2 : 0]);
-                }
-                wgmma_wait<1>();
-                if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
-                prev_s = s;
-                ++it;
-            };
-            for (int kb = 0; kb < num_kb; kb += 2) {
-                kblock(IntC<0>{}, kb);
-                if (kb == 0) prefetch_residual();
-                if (kb + 1 < num_kb) kblock(IntC<1>{}, kb + 1);
-            }
-        } else {
-            for (int kb = 0; kb < num_kb; ++kb, ++it) {
-                const int s = it % STAGES;
-                mbar_wait(bar_full(s), (it / STAGES) & 1u);
-                const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
-                uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
-                if (p.passes == 3) {
-                    // A_lo = A - trunc_tf32(A), element-wise, so the swizzled placement is preserved verbatim
-                    const float4* a = reinterpret_cast<const float4*>(st_gen) + 512 * cw;
-                    float4* alo = reinterpret_cast<float4*>(st_gen + Cfg::A_BYTES) + 512 * cw;
+                    const uint64_t dbh = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES);
+                    const uint64_t dbl = gmma_desc_sw64(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
+                    // the same MMA sequence per k-step as the three-term product always ran: cross terms A_l B_h, A_h B_l, then the main term
+                    auto batch = [&](float (&am)[R]) {
+                        if (p.passes == 3) {
+                            wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float4 v = a[t + i * 128];
-                        float4 o;
-                        o.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                        o.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                        o.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                        o.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                        alo[t + i * 128] = o;
-                    }
-                    fence_proxy_async_smem();
-                    named_bar_sync(2 + cw, 128);
-                }
-                const uint64_t da = gmma_desc_sw128(st + cw * 64 * 128);
-                const uint64_t dal = gmma_desc_sw128(st + Cfg::A_BYTES + cw * 64 * 128);
-                const uint64_t dbh = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES);
-                const uint64_t dbl = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
-                wgmma_fence();
+                            for (int k = 0; k < Cfg::KSTEPS; ++k) {
+                                const uint64_t koff = (uint64_t)(k * 32 >> 4);
+                                conv_mma_f16<BLOCK_N>(accx, fl[b][k], dbh + koff);
+                                conv_mma_f16<BLOCK_N>(accx, fh[b][k], dbl + koff);
+                                conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + koff);
+                            }
+                            wgmma_commit();
+                        } else {
+                            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < Cfg::KSTEPS; ++k) {
-                    const uint64_t koff = (uint64_t)(k * 32 >> 4);
-                    if (p.passes == 3) {
-                        conv_mma_tf32<BLOCK_N>(accx, dal + koff, dbh + koff);
-                        conv_mma_tf32<BLOCK_N>(accx, da + koff, dbl + koff);
-                    }
-                    // The tensor core accumulates in fp32 with truncation, so every accumulate step costs up to 1 ulp of the running sum.
-                    // NMAIN == 3 rotates the main term over three accumulators by k-block (summed with RN adds in the epilogue): shorter chains.
+                            for (int k = 0; k < Cfg::KSTEPS; ++k) conv_mma_f16<BLOCK_N>(am, fh[b][k], dbh + (uint64_t)(k * 32 >> 4));
+                            wgmma_commit();
+                        }
+                    };
+                    // NMAIN == 3 rotates the main term over three accumulators by k-block (see the tf32 loop)
                     if constexpr (NMAIN == 1) {
-                        conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
+                        batch(acc[0]);
                     } else {
                         const int sel = kb % 3;
-                        if (sel == 0) conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
-                        else if (sel == 1) conv_mma_tf32<BLOCK_N>(acc[NMAIN > 1 ? 1 : 0], da + koff, dbh + koff);
-                        else conv_mma_tf32<BLOCK_N>(acc[NMAIN > 2 ? 2 : 0], da + koff, dbh + koff);
+                        if (sel == 0) batch(acc[0]);
+                        else if (sel == 1) batch(acc[NMAIN > 1 ? 1 : 0]);
+                        else batch(acc[NMAIN > 2 ? 2 : 0]);
+                    }
+                    wgmma_wait<1>();
+                    if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
+                    prev_s = s;
+                    ++it;
+                };
+                for (int kb = 0; kb < nkb; kb += 2) {
+                    kblock(IntC<0>{}, kb);
+                    if (kb == 0) prefetch_residual();
+                    if (kb + 1 < nkb) kblock(IntC<1>{}, kb + 1);
+                }
+            } else {
+                for (int kb = 0; kb < nkb; ++kb, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait(bar_full(s), (it / STAGES) & 1u);
+                    const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+                    uint8_t* st_gen = smem_gen + s * Cfg::STAGE_BYTES;
+                    if (p.passes == 3) {
+                        // A_lo = A - trunc_tf32(A), element-wise, so the swizzled placement is preserved verbatim
+                        const float4* a = reinterpret_cast<const float4*>(st_gen) + 512 * cw;
+                        float4* alo = reinterpret_cast<float4*>(st_gen + Cfg::A_BYTES) + 512 * cw;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const float4 v = a[t + i * 128];
+                            float4 o;
+                            o.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
+                            o.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
+                            o.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
+                            o.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
+                            alo[t + i * 128] = o;
+                        }
+                        fence_proxy_async_smem();
+                        named_bar_sync(2 + cw, 128);
+                    }
+                    const uint64_t da = gmma_desc_sw128(st + cw * 64 * 128);
+                    const uint64_t dal = gmma_desc_sw128(st + Cfg::A_BYTES + cw * 64 * 128);
+                    const uint64_t dbh = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES);
+                    const uint64_t dbl = gmma_desc_sw128(st + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < Cfg::KSTEPS; ++k) {
+                        const uint64_t koff = (uint64_t)(k * 32 >> 4);
+                        if (p.passes == 3) {
+                            conv_mma_tf32<BLOCK_N>(accx, dal + koff, dbh + koff);
+                            conv_mma_tf32<BLOCK_N>(accx, da + koff, dbl + koff);
+                        }
+                        // The tensor core accumulates in fp32 with truncation, so every accumulate step costs up to 1 ulp of the running sum.
+                        // NMAIN == 3 rotates the main term over three accumulators by k-block (summed with RN adds in the epilogue): shorter chains.
+                        if constexpr (NMAIN == 1) {
+                            conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
+                        } else {
+                            const int sel = kb % 3;
+                            if (sel == 0) conv_mma_tf32<BLOCK_N>(acc[0], da + koff, dbh + koff);
+                            else if (sel == 1) conv_mma_tf32<BLOCK_N>(acc[NMAIN > 1 ? 1 : 0], da + koff, dbh + koff);
+                            else conv_mma_tf32<BLOCK_N>(acc[NMAIN > 2 ? 2 : 0], da + koff, dbh + koff);
+                        }
+                    }
+                    wgmma_commit();
+                    if (kb == 0) prefetch_residual();
+                    // the MMAs of the previous k-block have retired: its stage goes back to the producer
+                    wgmma_wait<1>();
+                    if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
+                    prev_s = s;
+                }
+            }
+            wgmma_wait<0>();
+            if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
+            reg_fence(accx);
+#pragma unroll
+            for (int a = 0; a < NMAIN; ++a) reg_fence(acc[a]);
+            if constexpr (P1) {
+                // phase 1's scale/shift result into the staging area, in the layout a RES_TILE residual load leaves there, once the
+                // previous tile's stores have read it.  Each thread writes the positions its phase-2 epilogue reads.
+                if (ct == 0) tma_store_wait_read0();
+                named_bar_sync(1, 256);
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 8; ++j) {
+                        const int col = 8 * j + cq;
+                        if ((j >> 2) >= nlive) continue;
+                        *reinterpret_cast<float2*>(epi_gen + (j >> 2) * Cfg::A_BYTES + off32_of(trow + 8 * hr, col)) =
+                            scaled(4 * j + 2 * hr, n0 + col, p.scale1, p.shift1);
                     }
                 }
-                wgmma_commit();
-                if (kb == 0) prefetch_residual();
-                // the MMAs of the previous k-block have retired: its stage goes back to the producer
-                wgmma_wait<1>();
-                if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
-                prev_s = s;
             }
-        }
-        wgmma_wait<0>();
-        if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty(prev_s));
-        reg_fence(accx);
-#pragma unroll
-        for (int a = 0; a < NMAIN; ++a) reg_fence(acc[a]);
+        };
+        if constexpr (STAGED) run_phase(IntC<0>{});
+        run_phase(IntC<1>{});
 
         // ---------------------------------------------------------------- epilogue
         if (ct == 0 && p.res_mode != RES_TILE) tma_store_wait_read0();   // the previous tile's stores have read the staging area
         named_bar_sync(1, 256);
         if (p.res_mode == RES_TILE) mbar_wait(bar_res, tcount & 1u);
-        // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1);
-        // its rows are tile rows trow (+ 8)
-        const int rbase = trow;
-        const int cq = 2 * (lane & 3);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
-            const int row = rbase + 8 * hr;
+            const int row = trow + 8 * hr;
             bool outside = false;           // past its image's extent: the row is written as zeros below, and never raises the range flag
             if constexpr (MASK) {
                 int r = row;
@@ -439,21 +500,11 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
                 const int ch = n0 + col;
                 const int c = j >> 2;               // 32-channel chunk
                 if (c >= nlive) continue;
-                const int i0 = 4 * j + 2 * hr;
-                float v0 = accx[i0], v1 = accx[i0 + 1];
-                if (p.passes != 3) { v0 = 0.f; v1 = 0.f; }
-#pragma unroll
-                for (int a = 0; a < NMAIN; ++a) { v0 += acc[a][i0]; v1 += acc[a][i0 + 1]; }
-                float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
-                if (ch < p.cout) {                  // cout % 4 == 0 and ch is even: ch + 1 < cout too
-                    sc = __ldg(reinterpret_cast<const float2*>(p.scale + ch));
-                    sh = __ldg(reinterpret_cast<const float2*>(p.shift + ch));
-                }
-                float o0 = fmaf(v0, sc.x, sh.x), o1 = fmaf(v1, sc.y, sh.y);
+                const float2 o = scaled(4 * j + 2 * hr, ch, p.scale, p.shift);
+                float o0 = o.x, o1 = o.y;
                 uint8_t* slot = epi_gen + c * Cfg::A_BYTES;
-                // SWIZZLE_128B fp32 chunk: 16-byte piece (col % 32) / 4 of the row, XOR (row mod 8)
-                const int off32 = row * 128 + (((((col & 31) >> 2)) ^ (row & 7)) << 4) + ((col & 3) << 2);
-                if (p.res_mode == RES_TILE) {
+                const int off32 = off32_of(row, col);
+                if (STAGED || p.res_mode == RES_TILE) {
                     const float2 r2 = *reinterpret_cast<const float2*>(slot + off32);
                     o0 += r2.x; o1 += r2.y;
                 } else if (p.res_mode == RES_UPSAMPLE2X) {
@@ -491,7 +542,7 @@ __global__ void __launch_bounds__(384, 1) conv_wgmma_kernel(const __grid_constan
                         *reinterpret_cast<uint32_t*>(slot + off16) = 0u;
                         *reinterpret_cast<uint32_t*>(slot + Cfg::A_BYTES / 2 + off16) = 0u;
                     } else {
-                        *reinterpret_cast<float2*>(slot + row * 128 + (((((col & 31) >> 2)) ^ (row & 7)) << 4) + ((col & 3) << 2)) = make_float2(0.f, 0.f);
+                        *reinterpret_cast<float2*>(slot + off32_of(row, col)) = make_float2(0.f, 0.f);
                     }
                 }
             }

@@ -370,3 +370,49 @@ def conv2d_nhwc(x, w_kmajor, scale, shift, kh, kw, pad, stride, w_lo=None, resid
                                    int(force_block_n), _p(out), Cout, _stream())
     _lib.check(ok, "dt_conv2d_nhwc")
     return out
+
+
+class ConvOperand(ctypes.Structure):
+    """dt_conv_operand of include/detectorch_b200.h"""
+    _fields_ = [("x", ctypes.c_void_p), ("H", ctypes.c_int), ("W", ctypes.c_int), ("Cin", ctypes.c_int), ("w_hi", ctypes.c_void_p),
+                ("w_lo", ctypes.c_void_p), ("kh", ctypes.c_int), ("kw", ctypes.c_int), ("pad", ctypes.c_int), ("stride", ctypes.c_int),
+                ("tap0", ctypes.c_int), ("ntaps", ctypes.c_int), ("scale", ctypes.c_void_p), ("shift", ctypes.c_void_p)]
+
+
+def conv2d_nhwc_two_phase(phase2, phase1=None, residual=None, relu=False, passes=3, force_block_n=0, out=None, kind="tf32", range_flag=None,
+                          im_info=None, im_stride=0):
+    """One launch of y = act(conv(phase2) + conv(phase1)), phase 1's fp32 result staying on chip as phase 2's residual: rounded exactly as
+    phase 1 into a buffer, then phase 2 with residual=that buffer.  A phase is a dict: x [N,H,W,Cin] fp32, w [Cout, kh*kw*Cin],
+    scale, shift [Cout], k (or kh, kw), pad, stride, and optionally the filter taps tap0, ntaps (0 = all).  phase1=None runs phase 2
+    alone (+ residual).  im_info [N,5] with im_stride > 0 zeroes output pixels outside each image."""
+    keep = []
+
+    def operand(ph):
+        x, w = ph["x"], ph["w"]
+        _need_cuda(x, w)
+        kh, kw = ph.get("kh", ph.get("k")), ph.get("kw", ph.get("k"))
+        if kind == "f16":
+            mult = weight_multiplier(w)
+            hi, lo = fp16_split(w, mult)
+            sc = (ph["scale"] / mult).contiguous()
+        else:
+            hi, lo, sc = w.contiguous(), tf32_residual(w.contiguous()), ph["scale"].contiguous()
+        sh = ph["shift"].contiguous()
+        x = x.contiguous()
+        keep.extend([x, hi, lo, sc, sh])
+        return ConvOperand(x.data_ptr(), x.size(1), x.size(2), x.size(3), hi.data_ptr(), lo.data_ptr(), kh, kw, ph["pad"], ph["stride"],
+                           ph.get("tap0", 0), ph.get("ntaps", 0), sc.data_ptr(), sh.data_ptr())
+
+    o2 = operand(phase2)
+    o1 = operand(phase1) if phase1 is not None else None
+    N, H, W, _ = phase2["x"].shape
+    Cout = phase2["w"].size(0)
+    Ho = (H + 2 * o2.pad - o2.kh) // o2.stride + 1
+    Wo = (W + 2 * o2.pad - o2.kw) // o2.stride + 1
+    if out is None:
+        out = torch.empty((N, Ho, Wo, Cout), device=phase2["x"].device, dtype=torch.float32)
+    ok = _lib.lib().dt_conv2d_nhwc_two_phase(1 if kind == "f16" else 0, ctypes.byref(o1) if o1 is not None else None, ctypes.byref(o2),
+                                             _p(residual), N, Cout, int(relu), int(passes), int(force_block_n), _p(range_flag), _p(im_info),
+                                             int(im_stride), _p(out), _stream())
+    _lib.check(ok, "dt_conv2d_nhwc_two_phase")
+    return out

@@ -194,6 +194,26 @@ int dt_conv2d_nhwc(const float* x, int N, int H, int W, int Cin, int x_pix_strid
                    int res_mode, const float* up_src, int up_h, int up_w, int relu, int sigmoid_ch, int passes, int force_block_n,
                    float* y, int y_pix_stride, dt_stream_t stream);
 
+/* One operand of dt_conv2d_nhwc_two_phase: conv(x, w) over filter taps [tap0, tap0 + ntaps) (ntaps 0: all kh*kw), * scale + shift.
+ * x [N,H,W,Cin] fp32, dense; w_hi / w_lo as for dt_conv2d_nhwc (kind 0) or dt_conv2d_nhwc_f16x3 (kind 1). */
+typedef struct dt_conv_operand {
+    const float* x;
+    int H, W, Cin;
+    const void* w_hi;
+    const void* w_lo;
+    int kh, kw, pad, stride, tap0, ntaps;
+    const float* scale;
+    const float* shift;
+} dt_conv_operand;
+/* y [N,Ho,Wo,Cout] = act( phase2 + phase1 ), with phase 1's fp32 result kept on chip as the residual of phase 2 (both GEMMs run in one
+ * launch, tile by tile; what the engine runs for a bottleneck's downsample + conv3 and for the two K-split halves of a mask-head conv).
+ * The sum is rounded exactly as phase 1 written to a buffer and then phase 2 with that buffer as its residual.  The phases must give
+ * the same output extents and tile shape.  phase1 NULL: phase 2 alone, plus `residual` [N,Ho,Wo,Cout] when given.
+ * kind 0 = 3xTF32, 1 = 3xFP16.  im_info [N,5] (may be NULL): output pixels outside image n (its network size at im_stride) are zero. */
+int dt_conv2d_nhwc_two_phase(int kind, const dt_conv_operand* phase1, const dt_conv_operand* phase2, const float* residual, int N, int Cout,
+                             int relu, int passes, int force_block_n, int* range_flag, const float* im_info, int im_stride, float* y,
+                             dt_stream_t stream);
+
 
 /* ---------------------------------------------------------------------------------------------
  * Fused Mask R-CNN (ResNet-50/101 + FPN) inference engine: the whole of
