@@ -70,6 +70,8 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p]),
     "dt_coco_results_write": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_coco_json": (c_int, [c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_void_p, c_void_p, c_void_p]),
     "dt_proposal_recall_smem_bytes": (c_int64, [c_int, c_int64]),
     "dt_proposal_recall": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64,
                                    c_void_p, c_void_p, c_void_p]),

@@ -1,9 +1,10 @@
-// detectorch_b200 -- C-ABI entry points of the COCO evaluation (coco_eval.cuh) and of the proposal recall (proposal_recall.cuh);
-// include/detectorch_b200.h.
+// detectorch_b200 -- C-ABI entry points of the COCO evaluation (coco_eval.cuh), the results json (coco_json.cuh) and the proposal
+// recall (proposal_recall.cuh); include/detectorch_b200.h.
 #include <stdio.h>
 
 #include "../../include/detectorch_b200.h"
 #include "coco_eval.cuh"
+#include "coco_json.cuh"
 #include "common.cuh"
 #include "proposal_recall.cuh"
 
@@ -139,6 +140,24 @@ extern "C" int dt_coco_results_write(int64_t num_records, const float* rec_f, co
     }
     DT_CHECK_CUDA(coco_results_write_launch(bins ? num_records : 0, rec_f, rec_i, num_classes, cls_k, ord_i, num_images, num_cats, cats_per_pair,
                                             bin_cnt, scan, gt_keys, num_gts, det_key, det_f, det_i, pairs, cat_kept, order_off, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int dt_coco_json(int iou_type, int64_t num_dets, const double* det_f, const int64_t* det_key, const int64_t* file_pos, int num_images,
+                            const int64_t* img_ids, const int64_t* cat_ids, const int64_t* det_i, const char* det_chars,
+                            const uint8_t* counts_first, const int64_t* offsets, int64_t* lens, char* text, dt_stream_t stream) {
+    if ((iou_type != 0 && iou_type != 1) || num_dets < 0 || num_images < 0 || (num_dets > 0 && num_images == 0) ||
+        num_dets > (1ll << 31) / 32) {
+        fprintf(stderr, "dt_coco_json: bad sizes\n");
+        return 0;
+    }
+    if (num_dets == 0) return 1;
+    if (!det_f || !det_key || !file_pos || !img_ids || !cat_ids || (iou_type == 1 && (!det_i || !det_chars)) || (offsets ? !text : !lens)) {
+        fprintf(stderr, "dt_coco_json: null argument\n");
+        return 0;
+    }
+    JsonRows R{num_dets, num_images, det_f, det_key, file_pos, img_ids, cat_ids, det_i, det_chars, counts_first};
+    DT_CHECK_CUDA(coco_json_launch(iou_type, R, offsets, lens, text, (cudaStream_t)stream));
     return 1;
 }
 

@@ -1156,6 +1156,130 @@ def _bins_device(gt, acc, iou_type, category_ids, keep_eval_imgs=False, view=Non
     return out
 
 
+# ------------------------------------------------------------------------------------------------------------ results json
+_JSON_CHUNK = 64 << 20          # bytes per pinned staging buffer (two of them) between the device text and the file
+
+
+def _counts_first(all_segms, all_boxes, category_ids, num_images):
+    """The RLE dicts in file order (the loop of _flatten_results) -> uint8 [rows], 1 where 'counts' comes before 'size'.  A dict with
+    a key other than these two, or 'counts' that is not a str (json.dump writes no bytes), is refused."""
+    flags = []
+    for j in range(1, len(category_ids) + 1):
+        if j >= len(all_boxes):
+            break
+        for i in range(num_images):
+            d = all_boxes[j][i]
+            if isinstance(d, list) and len(d) == 0:
+                continue
+            for r in all_segms[j][i][:np.asarray(d).shape[0]]:
+                if set(r) != {'size', 'counts'}:
+                    raise ValueError("class %d image %d: an RLE dict must have exactly the keys 'size' and 'counts'" % (j, i))
+                if not isinstance(r['counts'], str):
+                    raise ValueError("class %d image %d: RLE 'counts' must be a str to be written to json" % (j, i))
+                flags.append(next(iter(r)) == 'counts')
+    return np.array(flags, np.uint8)
+
+
+def write_results(gt, results, iou_type, path, all_segms=None, category_ids=None):
+    """The COCO results json of `results` ('bbox' or 'segm') written to `path` -> bytes written.  The file holds the bytes the
+    reference's _write_coco_bbox_results_file / _write_coco_segms_results_file + json.dump write: records class-major (j = 1, 2, ..),
+    images in sorted-id order, each (class, image)'s detections in their order; bbox [x1, y1, x2 - x1 + 1, y2 - y1 + 1] and the score
+    as float64, printed as float.__repr__ prints them; an RLE dict in its own key order.
+    results, all_segms and category_ids as for evaluate(): per-image tuples, all_boxes [class][image] (+ all_segms), or a
+    DeviceResults.  gt only supplies the sorted image ids and the categories: one without annotations (a test-dev image-info file)
+    will do, for either iou_type.
+    Unlike the reference, a non-finite box or score raises ValueError (json.dump would write NaN / Infinity, which is not json).
+    Input evaluate() refuses is refused here, before anything is written: no file is created and an existing one is left as it
+    was (the text goes to a temporary file in the same directory, renamed over `path` once complete).
+    The records are formatted on the device (csrc/coco_json.cuh): a length pass, a scan, a write pass; the text reaches the file
+    through two pinned buffers of 64 MB."""
+    if iou_type not in ('bbox', 'segm'):
+        raise ValueError("iou_type must be 'bbox' or 'segm'")
+    if not isinstance(gt, CocoGroundTruth):
+        raise TypeError("gt must be a CocoGroundTruth")
+    category_ids = list(gt.category_ids if category_ids is None else category_ids)
+    if any(c not in set(gt.cat_ids) for c in category_ids):
+        raise ValueError("category_ids names a category the ground truth does not have")
+    segm, dev, first = iou_type == 'segm', gt.device, None
+    if isinstance(results, DeviceResults):
+        if all_segms is not None:
+            raise ValueError("a DeviceResults carries its masks; all_segms is for all_boxes input")
+        f = _flatten_device(gt, results, iou_type, category_ids, keep_eval_imgs=True)
+        key, det_f, det_i, chars, pos = f['key'], f['det_f'], f['det_i'], f['chars'], f['det_ids'] - 1
+    else:
+        boxes, segms = _per_class(gt, results, all_segms, iou_type)
+        key, det_f, det_i, chars, det_ids = _flatten_results(gt, boxes, segms, iou_type, category_ids, with_ids=True)
+        if segm and len(key):
+            first = _counts_first(segms, boxes, category_ids, gt.num_images)
+        key, det_f, det_i, pos = (torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (key, det_f, det_i, det_ids - 1))
+        chars = torch.from_numpy(np.frombuffer(chars or b"\0", np.uint8).copy()).to(dev)
+        first = torch.from_numpy(first).to(dev) if first is not None and first.any() else None
+    N = int(key.shape[0])
+    text = np.frombuffer(b"[]", np.uint8)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        if N:
+            ids = [torch.tensor(v, dtype=torch.int64, device=dev) for v in (gt.img_ids, gt.cat_ids)]
+            args = (1 if segm else 0, N, _p(det_f), _p(key), _p(pos), gt.num_images, _p(ids[0]), _p(ids[1]), _p(det_i), _p(chars), _p(first))
+            lens = torch.empty((N,), dtype=torch.int64, device=dev)
+            _lib.check(L.dt_coco_json(*args, None, _p(lens), None, _stream(dev)), "dt_coco_json")
+            lens.cumsum_(0)
+            tail = [lens[-1:]]
+            if segm:
+                # as evaluate() refuses them: runs that do not cover h * w pixels
+                bad = torch.empty((N,), dtype=torch.uint8, device=dev)
+                _lib.check(L.dt_coco_det_check(N, _p(det_i), _p(chars), _p(bad), _stream(dev)), "dt_coco_det_check")
+                tail.append(bad.any().view(1).to(torch.int64))
+            tail = torch.cat(tail).cpu().numpy()            # the one read-back: the file's size, and the RLE check
+            if segm and tail[1]:
+                raise ValueError("results: RLE counts of a result do not sum to h * w")
+            text = torch.empty((int(tail[0]),), dtype=torch.uint8, device=dev)
+            _lib.check(L.dt_coco_json(*args, _p(lens), None, _p(text), _stream(dev)), "dt_coco_json")
+        return _write_text(text, path)
+
+
+def _write_text(text, path):
+    """Device bytes (or a host array) -> path, through a temporary file renamed over it; the device text in chunks through two
+    pinned buffers, the copy of the next chunk under the write of this one."""
+    import os
+    import tempfile
+    total = int(text.shape[0])
+    fd, tmp = tempfile.mkstemp(prefix=".%s." % os.path.basename(path), suffix=".tmp", dir=os.path.dirname(os.path.abspath(path)))
+    try:
+        with os.fdopen(fd, "wb") as fh:
+            if isinstance(text, np.ndarray):
+                fh.write(text.tobytes())
+            else:
+                stage = [torch.empty((min(total, _JSON_CHUNK),), dtype=torch.uint8, pin_memory=True) for _ in range(1 + (total > _JSON_CHUNK))]
+                spans = [(o, min(o + _JSON_CHUNK, total)) for o in range(0, total, _JSON_CHUNK)]
+                events = []
+
+                def copy(c):
+                    a, b = spans[c]
+                    stage[c % 2][:b - a].copy_(text[a:b], non_blocking=True)
+                    events.append(torch.cuda.Event())
+                    events[-1].record()
+                copy(0)
+                for c, (a, b) in enumerate(spans):
+                    if c + 1 < len(spans):
+                        copy(c + 1)             # its buffer's previous chunk is already in the file
+                    events[c].synchronize()
+                    fh.write(memoryview(stage[c % 2].numpy())[:b - a])
+        os.chmod(tmp, 0o666 & ~_umask())
+        os.replace(tmp, path)
+    except BaseException:
+        os.unlink(tmp)
+        raise
+    return total
+
+
+def _umask():
+    import os
+    m = os.umask(0)
+    os.umask(m)
+    return m
+
+
 # ------------------------------------------------------------------------------------------------------------ proposal recall
 # evaluate_box_proposals' area ranges (json_dataset_evaluator.py:247-264), both bounds inclusive
 PROPOSAL_AREAS = {'all': [0 ** 2, 1e5 ** 2], 'small': [0 ** 2, 32 ** 2], 'medium': [32 ** 2, 96 ** 2], 'large': [96 ** 2, 1e5 ** 2],

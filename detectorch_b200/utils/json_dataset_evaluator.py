@@ -4,8 +4,11 @@ switches with one import line:
     from detectorch_b200.utils.json_dataset_evaluator import evaluate_boxes, evaluate_masks
 json_dataset.COCO.dataset supplies the ground truth (built on the device once per json_dataset, kept on it); its classes /
 category_to_id_map give the json category id of each contiguous class, as _write_coco_*_results_file uses them.
-evaluate_box_proposals (:238-320) is the proposal recall of coco_eval.box_proposal_recall, one (area, limit) combination."""
+evaluate_box_proposals (:238-320) is the proposal recall of coco_eval.box_proposal_recall, one (area, limit) combination.
+_write_coco_bbox_results_file / _write_coco_segms_results_file (:67-190) write the reference's results json, byte for byte, with
+coco_eval.write_results (for test-dev, whose evaluation returns None, the file is the only output)."""
 import logging
+import os
 
 import numpy as np
 
@@ -44,6 +47,27 @@ def evaluate_masks(json_dataset, all_boxes, all_segms, output_dir, use_salt=True
 def evaluate_boxes(json_dataset, all_boxes, output_dir, use_salt=True, cleanup=False):
     """-> the evaluation ('bbox'), as evaluate_masks."""
     return _evaluate(json_dataset, all_boxes, None, 'bbox')
+
+
+def _results_ground_truth(json_dataset):
+    """The images (json_dataset.COCO.getImgIds(), sorted) and categories the results files are written for; no annotations."""
+    cats = list(dict.fromkeys(_category_ids(json_dataset)))
+    return coco_eval.CocoGroundTruth({'images': [{'id': i, 'height': 1, 'width': 1} for i in sorted(json_dataset.COCO.getImgIds())],
+                                      'categories': [{'id': c} for c in cats]})
+
+
+def _write_coco_segms_results_file(json_dataset, all_boxes, all_segms, res_file):
+    """The reference's segm results json (all_boxes / all_segms [class][image], or a DeviceResults with all_segms None), byte for
+    byte; a non-finite box or score raises ValueError (see coco_eval.write_results)."""
+    logger.info('Writing segmentation results json to: {}'.format(os.path.abspath(res_file)))
+    coco_eval.write_results(_results_ground_truth(json_dataset), all_boxes, 'segm', res_file, all_segms,
+                            category_ids=_category_ids(json_dataset))
+
+
+def _write_coco_bbox_results_file(json_dataset, all_boxes, res_file):
+    """The reference's bbox results json, as _write_coco_segms_results_file."""
+    logger.info('Writing bbox results json to: {}'.format(os.path.abspath(res_file)))
+    coco_eval.write_results(_results_ground_truth(json_dataset), all_boxes, 'bbox', res_file, category_ids=_category_ids(json_dataset))
 
 
 def _log_detection_eval_metrics(E):

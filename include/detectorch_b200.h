@@ -370,6 +370,19 @@ int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* union_keys, in
                       const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos, uint8_t* gt_ig,
                       dt_stream_t stream);
 
+/* dt_coco_json: the COCO results json of the reference's results writers + json.dump, byte for byte, in two passes over the
+ * flattened results (iou_type 0 bbox, 1 segm; det_f / det_i / det_chars as dt_coco_eval takes them, rows in any order).
+ *   det_key [num_dets] int64        category index * num_images + image index; img_ids [num_images], cat_ids json ids of those indexes
+ *   file_pos [num_dets] int64       each row's record in the file (a permutation of 0..num_dets-1)
+ *   counts_first [num_dets] uint8   segm, by file position: 1 where the RLE dict is written 'counts' first (NULL: 'size' first everywhere)
+ *   offsets == NULL                 length pass: lens [num_dets] int64 = each record's bytes at its file position ("[" / ", " before it,
+ *                                   "]" after the last)
+ *   offsets != NULL                 write pass: offsets [num_dets] the inclusive scan of lens; text [offsets[num_dets - 1]] bytes
+ * bbox runs one thread per record, segm one warp.  Returns 0 on bad sizes or a NULL pointer. */
+int dt_coco_json(int iou_type, int64_t num_dets, const double* det_f, const int64_t* det_key, const int64_t* file_pos, int num_images,
+                 const int64_t* img_ids, const int64_t* cat_ids, const int64_t* det_i, const char* det_chars, const uint8_t* counts_first,
+                 const int64_t* offsets, int64_t* lens, char* text, dt_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Proposal recall (Detectron's evaluate_box_proposals), bit for bit.  One CTA per (image, combination); every combination of
  * (area range, proposal limit) in one launch.
