@@ -496,17 +496,30 @@ size_t segm_smem_bytes(int M, int im_h, int im_w) {
     return (size_t)((S * S + 3) & ~3) * 4 + (size_t)im_h * sizeof(SegmRowCoef) + (size_t)(im_w + 2) * 4 + 40 * 4;
 }
 
-// paste + RLE of `batch` images x `cap` slots, then the scan of the string lengths and the gather into `strings`.  The caller has
-// checked the pointers and the sizes except the shared-memory limit.  workspace: segm_ws_bytes(batch * cap, runs_cap)
+// Byte sizes and offsets of `slots` slots.  The workspace holds the transition positions (uint32 [slots, runs_cap]) from 0, the string
+// staging (`strings` bytes) after them and the string lengths (int [slots]) from the next 16-byte boundary, `scratch` bytes in all
+// (dt_segm_rle).  The batch entry points, whose callers do not take the run lengths, keep them (uint32 [slots, runs_cap]) from
+// `scratch` and their counts (int [slots]) from `num_counts`: `total` bytes.  The packed strings fit in `strings` bytes.
+struct SegmLayout { int64_t strings, str_len, scratch, num_counts, total; };
+SegmLayout segm_layout(int64_t slots, int runs_cap) {
+    SegmLayout l;
+    l.strings = slots * runs_cap * kSegmCharsPerRun;
+    l.str_len = slots * runs_cap * 4 + (l.strings + 15) / 16 * 16;
+    l.scratch = slots * runs_cap * 4 + l.strings + slots * 4 + 256;
+    l.num_counts = l.scratch + slots * runs_cap * 4;
+    l.total = l.num_counts + slots * 4;
+    return l;
+}
+
+// Paste + RLE of `batch` images x `cap` slots with the row / column tables sized for max_h x max_w, then the scan of the string lengths
+// and the gather of the strings into `strings` at str_offsets.  Without a cursor, flags is one int, the overflow, and the strings start
+// at 0.  With one (dt_segm_rle_batch_append), flags is int [3] and the strings are appended at *cursor, committed only if no flag is
+// raised and they fit in `capacity` (segm_offsets_kernel).  counts / num_counts NULL: they go to the batch workspace (segm_layout).  The
+// caller has checked the pointers and the sizes except the shared-memory limit.
 int segm_rle_launch(const char* who, const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,
                     const int* expanded_boxes, const int* num_dets_dev, const int* im_sizes, int batch, int cap, int max_h, int max_w,
-                    float thresh_binarize, uint32_t* counts, int* num_counts, int runs_cap, uint8_t* strings, int64_t* str_offsets,
-                    int* overflow, void* workspace, cudaStream_t st) {
-    const size_t D = (size_t)batch * cap;
-    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
-    uint8_t* staging = ws + D * runs_cap * 4;
-    int* str_len = reinterpret_cast<int*>(staging + ((D * runs_cap * kSegmCharsPerRun + 15) / 16 * 16));
+                    float thresh_binarize, uint32_t* counts, int* num_counts, int runs_cap, uint8_t* strings, int64_t* cursor,
+                    int64_t capacity, int64_t* str_offsets, int* flags, void* workspace, cudaStream_t st) {
     const size_t smem = segm_smem_bytes(mask_size, max_h, max_w);
     if (smem > 200 * 1024) { fprintf(stderr, "%s: image too large for the row/column tables (%zu B)\n", who, smem); return 0; }
     static size_t smem_set = 48 * 1024;
@@ -514,27 +527,34 @@ int segm_rle_launch(const char* who, const float* masks, const int* classes, int
         DT_CHECK_CUDA(cudaFuncSetAttribute(segm_rle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         smem_set = 200 * 1024;
     }
-    DT_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
+    const int64_t D = (int64_t)batch * cap;
+    const SegmLayout l = segm_layout(D, runs_cap);
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
+    uint8_t* staging = ws + D * runs_cap * 4;
+    int* str_len = reinterpret_cast<int*>(ws + l.str_len);
+    if (!counts) {
+        counts = reinterpret_cast<uint32_t*>(ws + l.scratch);
+        num_counts = reinterpret_cast<int*>(ws + l.num_counts);
+    }
+    const int str_cap = runs_cap * kSegmCharsPerRun;
+    DT_CHECK_CUDA(cudaMemsetAsync(flags, 0, (cursor ? 3 : 1) * sizeof(int), st));
     segm_rle_kernel<<<dim3(cap, batch), 256, smem, st>>>(masks, classes, classes ? num_mask_classes : 1, mask_size, ref_boxes, expanded_boxes,
                                                          num_dets_dev, im_sizes, max_h, max_w, thresh_binarize, positions, counts, num_counts,
-                                                         runs_cap, staging, str_len, runs_cap * kSegmCharsPerRun, overflow);
+                                                         runs_cap, staging, str_len, str_cap, flags, cursor ? flags + 1 : nullptr);
     DT_CHECK_CUDA(cudaGetLastError());
     long long* offsets = reinterpret_cast<long long*>(str_offsets);
-    segm_offsets_kernel<<<1, 1024, 0, st>>>(str_len, (int)D, offsets);
+    segm_offsets_kernel<<<1, 1024, 0, st>>>(str_len, (int)D, reinterpret_cast<long long*>(cursor), capacity, flags, offsets);
     DT_CHECK_CUDA(cudaGetLastError());
-    segm_compact_kernel<<<(unsigned)((D + 7) / 8), 256, 0, st>>>(staging, str_len, (int)D, runs_cap * kSegmCharsPerRun, offsets, strings);
+    segm_compact_kernel<<<(unsigned)((D + 7) / 8), 256, 0, st>>>(staging, str_len, (int)D, str_cap, offsets, cursor ? flags : nullptr, strings);
     DT_CHECK_CUDA(cudaGetLastError());
     return 1;
 }
-
-int64_t segm_ws_bytes(int64_t slots, int runs_cap) {
-    return slots * runs_cap * 4 + slots * runs_cap * kSegmCharsPerRun + slots * 4 + 256;
-}
 }  // namespace
 
-extern "C" int64_t dt_segm_workspace_bytes(int max_dets, int runs_cap) { return segm_ws_bytes(max_dets, runs_cap); }
+extern "C" int64_t dt_segm_workspace_bytes(int max_dets, int runs_cap) { return segm_layout(max_dets, runs_cap).scratch; }
 
-extern "C" int64_t dt_segm_strings_bytes(int max_dets, int runs_cap) { return (int64_t)max_dets * runs_cap * kSegmCharsPerRun; }
+extern "C" int64_t dt_segm_strings_bytes(int max_dets, int runs_cap) { return segm_layout(max_dets, runs_cap).strings; }
 
 extern "C" int dt_segm_rle(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,
                            const int* expanded_boxes, const int* num_dets_dev, int max_dets, int im_h, int im_w, float thresh_binarize,
@@ -550,17 +570,13 @@ extern "C" int dt_segm_rle(const float* masks, const int* classes, int num_mask_
         return 0;
     }
     return segm_rle_launch("dt_segm_rle", masks, classes, num_mask_classes, mask_size, ref_boxes, expanded_boxes, num_dets_dev, nullptr, 1,
-                           max_dets, im_h, im_w, thresh_binarize, counts, num_counts, runs_cap, strings, str_offsets, overflow, workspace,
-                           (cudaStream_t)stream);
+                           max_dets, im_h, im_w, thresh_binarize, counts, num_counts, runs_cap, strings, nullptr, 0, str_offsets, overflow,
+                           workspace, (cudaStream_t)stream);
 }
 
-// run lengths and their counts are scratch here: they follow the dt_segm_rle workspace of batch * cap slots
-extern "C" int64_t dt_segm_batch_workspace_bytes(int batch, int cap, int runs_cap) {
-    const int64_t slots = (int64_t)batch * cap;
-    return segm_ws_bytes(slots, runs_cap) + slots * runs_cap * 4 + slots * 4;
-}
+extern "C" int64_t dt_segm_batch_workspace_bytes(int batch, int cap, int runs_cap) { return segm_layout((int64_t)batch * cap, runs_cap).total; }
 
-extern "C" int64_t dt_segm_batch_strings_bytes(int batch, int cap, int runs_cap) { return (int64_t)batch * cap * runs_cap * kSegmCharsPerRun; }
+extern "C" int64_t dt_segm_batch_strings_bytes(int batch, int cap, int runs_cap) { return segm_layout((int64_t)batch * cap, runs_cap).strings; }
 
 extern "C" int dt_segm_rle_batch(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes,
                                  const int* num_dets_dev, const int* im_sizes, int batch, int cap, int max_im_h, int max_im_w,
@@ -577,18 +593,15 @@ extern "C" int dt_segm_rle_batch(const float* masks, const int* classes, int num
                 num_mask_classes, max_im_h, max_im_w, runs_cap, batch, cap);
         return 0;
     }
-    const int64_t slots = (int64_t)batch * cap;
-    uint8_t* scratch = reinterpret_cast<uint8_t*>(workspace) + segm_ws_bytes(slots, runs_cap);
-    uint32_t* counts = reinterpret_cast<uint32_t*>(scratch);
-    int* num_counts = reinterpret_cast<int*>(scratch + slots * runs_cap * 4);
     return segm_rle_launch("dt_segm_rle_batch", masks, classes, num_mask_classes, mask_size, boxes, nullptr, num_dets_dev, im_sizes, batch,
-                           cap, max_im_h, max_im_w, thresh_binarize, counts, num_counts, runs_cap, strings, str_offsets, overflow, workspace,
-                           (cudaStream_t)stream);
+                           cap, max_im_h, max_im_w, thresh_binarize, nullptr, nullptr, runs_cap, strings, nullptr, 0, str_offsets, overflow,
+                           workspace, (cudaStream_t)stream);
 }
 
-// dt_segm_rle_batch without a host-known size or a host read: bounded tables, flags, and the strings appended to an arena at a device
-// cursor.  Only stream operations are issued, so the call can be captured into a CUDA graph.
-static_assert(kSegmMaxSide == DT_SEGM_APPEND_MAX_SIDE, "the header states the table bound of segm_rle_bounded_kernel");
+// dt_segm_rle_batch without a host-known size or a host read: tables for kSegmMaxSide x kSegmMaxSide whatever the batch holds (so one
+// launch, one captured graph node, serves any im_sizes table), flags, and the strings appended to an arena at a device cursor.  Only
+// stream operations are issued, so the call can be captured into a CUDA graph.
+static_assert(kSegmMaxSide == DT_SEGM_APPEND_MAX_SIDE, "the header states the table bound of dt_segm_rle_batch_append");
 extern "C" int dt_segm_rle_batch_append(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* boxes,
                                         const int* num_dets_dev, const int* im_sizes, int batch, int cap, float thresh_binarize, int runs_cap,
                                         uint8_t* arena, int64_t arena_capacity, int64_t* cursor, int64_t* str_offsets, int* flags,
@@ -599,39 +612,15 @@ extern "C" int dt_segm_rle_batch_append(const float* masks, const int* classes, 
         fprintf(stderr, "dt_segm_rle_batch_append: null argument\n");
         return 0;
     }
-    const size_t smem = segm_smem_bytes(mask_size, kSegmMaxSide, kSegmMaxSide);
-    if (mask_size < 1 || smem > 200 * 1024 || (classes && num_mask_classes < 1) || runs_cap < 2 || batch > 65535 ||
-        (int64_t)batch * cap >= (1ll << 31)) {
+    if (mask_size < 1 || segm_smem_bytes(mask_size, kSegmMaxSide, kSegmMaxSide) > 200 * 1024 || (classes && num_mask_classes < 1) ||
+        runs_cap < 2 || batch > 65535 || (int64_t)batch * cap >= (1ll << 31)) {
         fprintf(stderr, "dt_segm_rle_batch_append: unsupported size (mask %d, %d classes, runs_cap %d, %d x %d slots)\n", mask_size,
                 num_mask_classes, runs_cap, batch, cap);
         return 0;
     }
-    static bool smem_set = false;
-    if (!smem_set) {
-        DT_CHECK_CUDA(cudaFuncSetAttribute(segm_rle_bounded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        smem_set = true;
-    }
-    const int64_t D = (int64_t)batch * cap;
-    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    uint32_t* positions = reinterpret_cast<uint32_t*>(ws);
-    uint8_t* staging = ws + D * runs_cap * 4;
-    int* str_len = reinterpret_cast<int*>(staging + ((D * runs_cap * kSegmCharsPerRun + 15) / 16 * 16));
-    uint8_t* scratch = ws + segm_ws_bytes(D, runs_cap);
-    uint32_t* counts = reinterpret_cast<uint32_t*>(scratch);
-    int* num_counts = reinterpret_cast<int*>(scratch + D * runs_cap * 4);
-    cudaStream_t st = (cudaStream_t)stream;
-    DT_CHECK_CUDA(cudaMemsetAsync(flags, 0, 3 * sizeof(int), st));
-    segm_rle_bounded_kernel<<<dim3(cap, batch), 256, smem, st>>>(masks, classes, classes ? num_mask_classes : 1, mask_size, boxes, num_dets_dev,
-                                                                 im_sizes, thresh_binarize, positions, counts, num_counts, runs_cap, staging,
-                                                                 str_len, runs_cap * kSegmCharsPerRun, flags);
-    DT_CHECK_CUDA(cudaGetLastError());
-    long long* offsets = reinterpret_cast<long long*>(str_offsets);
-    segm_arena_offsets_kernel<<<1, 1024, 0, st>>>(str_len, (int)D, reinterpret_cast<long long*>(cursor), arena_capacity, flags, offsets);
-    DT_CHECK_CUDA(cudaGetLastError());
-    segm_arena_compact_kernel<<<(unsigned)((D + 7) / 8), 256, 0, st>>>(staging, str_len, (int)D, runs_cap * kSegmCharsPerRun, offsets, flags,
-                                                                      arena);
-    DT_CHECK_CUDA(cudaGetLastError());
-    return 1;
+    return segm_rle_launch("dt_segm_rle_batch_append", masks, classes, num_mask_classes, mask_size, boxes, nullptr, num_dets_dev, im_sizes,
+                           batch, cap, kSegmMaxSide, kSegmMaxSide, thresh_binarize, nullptr, nullptr, runs_cap, arena, cursor,
+                           arena_capacity, str_offsets, flags, workspace, (cudaStream_t)stream);
 }
 
 extern "C" int dt_segm_paste(const float* masks, const int* classes, int num_mask_classes, int mask_size, const float* ref_boxes,

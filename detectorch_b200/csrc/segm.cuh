@@ -75,6 +75,12 @@ __device__ __forceinline__ float segm_area2(const float* pm, int S, int dx, int 
     return __fmul_rn(sum, 0.25f);
 }
 
+// value of the pasted mask at pixel (dx, dy) of the resized box: the area-fast average when both sides halve (area2), else the vertical
+// pass over h0, h1, the horizontal passes (segm_hrow) of the source rows cy.s and cy.s + 1, with the row weights w0, w1
+__device__ __forceinline__ float segm_pixel(const float* pm, int S, bool area2, int dx, int dy, int w, float h0, float h1, float w0, float w1) {
+    return area2 ? segm_area2(pm, S, dx, dy, w) : __fadd_rn(__fmul_rn(h0, w0), __fmul_rn(h1, w1));
+}
+
 // exclusive scan of a[0..n) in shared memory by the whole block; returns the total.  scratch: 33 ints
 __device__ __forceinline__ int block_exclusive_scan(int* a, int n, int* scratch) {
     const int T = blockDim.x, tid = threadIdx.x;
@@ -129,21 +135,25 @@ __device__ __forceinline__ T block_scan_value(T v, T* scratch, T* total) {
 
 struct SegmRowCoef { int s; float w0, w1; int pad; };
 
-// Image side the tables of segm_rle_bounded_kernel are sized for (dt_segm_rle_batch_append; include/detectorch_b200.h).
+// Image side of the tables of dt_segm_rle_batch_append's launch, whatever its batch holds (include/detectorch_b200.h).
 constexpr int kSegmMaxSide = 8192;
 
 // Grid (cap, B): block (d, b) is detection slot d of image b, i.e. slot s = b * cap + d of the flat per-slot arrays.
 // masks: [B*cap, K, M, M] (class-specific: K classes, cls[s] selects) or [B*cap, M, M] (K == 1 / cls == NULL)
 // im_sizes: int32 [B, 2] (im_h, im_w) of each image's canvas, or NULL (every image is max_h x max_w).  The shared row / column tables
-// are sized for max_h x max_w; an image whose size is not within [1, max] produces empty results.
+// are sized for max_h x max_w; an image whose size is not within [1, max] produces empty results, and raises *size_flag (atomicOr 1)
+// when size_flag is not NULL.
 // num_dets_dev: int32 [B] live slots per image (NULL: all); slots at or past the count produce empty results
-// outputs per slot s: counts[s*runs_cap ..] (uint32 run lengths), num_counts[s], strings (cap str_cap per slot), str_len[s]
-__device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
-                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
-                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes, int max_h, int max_w,
-                                              float thresh, uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
-                                              int* __restrict__ num_counts, int runs_cap, uint8_t* __restrict__ strings,
-                                              int* __restrict__ str_len, int str_cap, int* __restrict__ overflow) {
+// outputs per slot s: counts[s*runs_cap ..] (uint32 run lengths), num_counts[s], strings (cap str_cap per slot), str_len[s];
+// *overflow: atomicMax of the runs a slot needed when runs_cap or str_cap was too small
+static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
+                                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
+                                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
+                                                              int max_h, int max_w, float thresh,
+                                                              uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
+                                                              int* __restrict__ num_counts, int runs_cap,
+                                                              uint8_t* __restrict__ strings, int* __restrict__ str_len, int str_cap,
+                                                              int* __restrict__ overflow, int* __restrict__ size_flag) {
     extern __shared__ __align__(16) uint8_t segm_smem[];
     const int b = blockIdx.y, det = blockIdx.x;
     const size_t d = (size_t)b * gridDim.x + det;
@@ -153,6 +163,7 @@ __device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, c
     int* colcnt = reinterpret_cast<int*>(rows + max_h);                                  // [max_w + 2]
     int* scratch = colcnt + max_w + 2;                                                   // [40]
     const int im_h = im_sizes ? im_sizes[2 * b] : max_h, im_w = im_sizes ? im_sizes[2 * b + 1] : max_w;
+    if (size_flag && det == 0 && threadIdx.x == 0 && (im_h < 1 || im_w < 1 || im_h > max_h || im_w > max_w)) atomicOr(size_flag, 1);
     if ((num_dets_dev && det >= num_dets_dev[b]) || im_h < 1 || im_w < 1 || im_h > max_h || im_w > max_w) {
         if (threadIdx.x == 0) { num_counts[d] = 0; str_len[d] = 0; }
         return;
@@ -174,11 +185,13 @@ __device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, c
     // value of the pasted mask at an in-region pixel
     const bool area2 = g.w * 2 == S && g.h * 2 == S;
     auto bit_at = [&](int x, int y) -> int {
+        // the area-fast value needs no coefficients: returning it before they are read keeps the kernel at 40 registers rather than 48
+        // (CUDA 12.9), one more CTA per SM
         if (area2) return segm_area2(pm, S, x - g.bx0, y - g.by0, g.w) > thresh ? 1 : 0;
         const AxisCoef cx = resize_coef_x(x - g.bx0, scale_x, S);
         const SegmRowCoef rc = rows[y];
         const float h0 = segm_hrow(pm, S, min(max(rc.s, 0), S - 1), cx), h1 = segm_hrow(pm, S, min(max(rc.s + 1, 0), S - 1), cx);
-        return __fadd_rn(__fmul_rn(h0, rc.w0), __fmul_rn(h1, rc.w1)) > thresh ? 1 : 0;
+        return segm_pixel(pm, S, area2, x - g.bx0, y - g.by0, g.w, h0, h1, rc.w0, rc.w1) > thresh ? 1 : 0;
     };
     const bool empty = g.x1 <= g.x0;
     const int xe = empty ? -1 : (g.x1 < im_w ? g.x1 : g.x1 - 1);        // last column that can hold a transition (pseudo column x1)
@@ -205,8 +218,7 @@ __device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, c
                     h0 = segm_hrow(pm, S, min(max(rc.s, 0), S - 1), cx);                                                 \
                     h1 = segm_hrow(pm, S, min(max(rc.s + 1, 0), S - 1), cx);                                             \
                 }                                                                                                        \
-                const float val = area2 ? segm_area2(pm, S, x - g.bx0, y - g.by0, g.w)                                   \
-                                        : __fadd_rn(__fmul_rn(h0, rc.w0), __fmul_rn(h1, rc.w1));                         \
+                const float val = segm_pixel(pm, S, area2, x - g.bx0, y - g.by0, g.w, h0, h1, rc.w0, rc.w1);             \
                 const int cur = val > thresh ? 1 : 0;                                                                    \
                 if (cur != prev) { EMIT((long long)x * im_h + y); prev = cur; }                                          \
             }                                                                                                            \
@@ -282,69 +294,14 @@ __device__ __forceinline__ void segm_rle_slot(const float* __restrict__ masks, c
     if (threadIdx.x == 0) { num_counts[d] = m; str_len[d] = total_chars; }
 }
 
-static __global__ void __launch_bounds__(256) segm_rle_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K, int M,
-                                                              const float* __restrict__ ref_boxes, const int* __restrict__ exp_boxes,
-                                                              const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
-                                                              int max_h, int max_w, float thresh,
-                                                              uint32_t* __restrict__ positions, uint32_t* __restrict__ counts,
-                                                              int* __restrict__ num_counts, int runs_cap,
-                                                              uint8_t* __restrict__ strings, int* __restrict__ str_len, int str_cap,
-                                                              int* __restrict__ overflow) {
-    segm_rle_slot(masks, cls, K, M, ref_boxes, exp_boxes, num_dets_dev, im_sizes, max_h, max_w, thresh, positions, counts, num_counts, runs_cap,
-                  strings, str_len, str_cap, overflow);
-}
-
-// segm_rle_kernel with tables for kSegmMaxSide x kSegmMaxSide whatever the batch holds, so that one launch (one captured graph node)
-// serves any im_sizes table.  flags[0] gets the overflow (atomicMax of the runs a slot needed); an image whose size is outside
-// [1, kSegmMaxSide] sets flags[1] (its slots are still emptied, and the batch is not committed by segm_arena_offsets_kernel).
-static __global__ void __launch_bounds__(256) segm_rle_bounded_kernel(const float* __restrict__ masks, const int* __restrict__ cls, int K,
-                                                                      int M, const float* __restrict__ boxes,
-                                                                      const int* __restrict__ num_dets_dev, const int* __restrict__ im_sizes,
-                                                                      float thresh, uint32_t* __restrict__ positions,
-                                                                      uint32_t* __restrict__ counts, int* __restrict__ num_counts,
-                                                                      int runs_cap, uint8_t* __restrict__ strings, int* __restrict__ str_len,
-                                                                      int str_cap, int* __restrict__ flags) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        const int h = im_sizes[2 * blockIdx.y], w = im_sizes[2 * blockIdx.y + 1];
-        if (h < 1 || w < 1 || h > kSegmMaxSide || w > kSegmMaxSide) atomicOr(flags + 1, 1);
-    }
-    segm_rle_slot(masks, cls, K, M, boxes, nullptr, num_dets_dev, im_sizes, kSegmMaxSide, kSegmMaxSide, thresh, positions, counts, num_counts,
-                  runs_cap, strings, str_len, str_cap, flags);
-}
-
-// offsets[0..D] = exclusive scan of str_len[0..D) (offsets[D] = total), one block: each thread sums a contiguous chunk, a block scan
-// of the chunk sums gives each chunk's start
-static __global__ void __launch_bounds__(1024) segm_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ offsets) {
+// offsets[0..D] = base + exclusive scan of str_len[0..D) (offsets[D] = base + total), one block: each thread sums a contiguous chunk, a
+// block scan of the chunk sums gives each chunk's start.  Without a cursor base is 0.  With one (a batch appended to a char arena) base
+// is *cursor, and the batch is committed, *cursor advanced by the total, only if no slot overflowed (flags[0]), every image was within
+// the tables (flags[1]) and base + total <= capacity; a batch that does not fit sets flags[2] and leaves the cursor.
+static __global__ void __launch_bounds__(1024) segm_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ cursor,
+                                                                   long long capacity, int* __restrict__ flags, long long* __restrict__ offsets) {
     __shared__ long long scratch[33];
-    const int chunk = (D + blockDim.x - 1) / blockDim.x;
-    const int lo = min((int)threadIdx.x * chunk, D), hi = min(lo + chunk, D);
-    long long sum = 0;
-    for (int i = lo; i < hi; ++i) sum += str_len[i];
-    long long total;
-    long long run = block_scan_value(sum, scratch, &total);
-    for (int i = lo; i < hi; ++i) { offsets[i] = run; run += str_len[i]; }
-    if (threadIdx.x == 0) offsets[D] = total;
-}
-
-// gathers the per-slot strings into one contiguous buffer at the scanned offsets; one warp per slot
-static __global__ void __launch_bounds__(256) segm_compact_kernel(const uint8_t* __restrict__ strings, const int* __restrict__ str_len, int D,
-                                                                  int str_cap, const long long* __restrict__ offsets, uint8_t* __restrict__ packed) {
-    const int d = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (d >= D) return;
-    const int n = str_len[d];
-    uint8_t* dst = packed + offsets[d];
-    const uint8_t* src = strings + (size_t)d * str_cap;
-    for (int i = lane; i < n; i += 32) dst[i] = src[i];
-}
-
-// segm_offsets_kernel for a batch appended to a char arena at a device-side cursor: offsets[s] = *cursor + the scan (offsets[D] =
-// *cursor + total).  The batch is committed, *cursor advanced by the total, only if no slot overflowed (flags[0]), every image was
-// within the tables (flags[1]) and cursor + total <= capacity; a batch that does not fit sets flags[2] and leaves the cursor.
-static __global__ void __launch_bounds__(1024) segm_arena_offsets_kernel(const int* __restrict__ str_len, int D, long long* __restrict__ cursor,
-                                                                         long long capacity, int* __restrict__ flags,
-                                                                         long long* __restrict__ offsets) {
-    __shared__ long long scratch[33];
-    const long long base = *cursor;                 // read by every thread before the scan's barriers, written after them
+    const long long base = cursor ? *cursor : 0;    // read by every thread before the scan's barriers, written after them
     const int chunk = (D + blockDim.x - 1) / blockDim.x;
     const int lo = min((int)threadIdx.x * chunk, D), hi = min(lo + chunk, D);
     long long sum = 0;
@@ -354,21 +311,22 @@ static __global__ void __launch_bounds__(1024) segm_arena_offsets_kernel(const i
     for (int i = lo; i < hi; ++i) { offsets[i] = run; run += str_len[i]; }
     if (threadIdx.x == 0) {
         offsets[D] = base + total;
-        if (flags[0] == 0 && flags[1] == 0) {
+        if (cursor && flags[0] == 0 && flags[1] == 0) {
             if (base + total <= capacity) *cursor = base + total;
             else flags[2] = 1;
         }
     }
 }
 
-// segm_compact_kernel into the arena, for a committed batch only (no flag of segm_arena_offsets_kernel raised)
-static __global__ void __launch_bounds__(256) segm_arena_compact_kernel(const uint8_t* __restrict__ strings, const int* __restrict__ str_len,
-                                                                        int D, int str_cap, const long long* __restrict__ offsets,
-                                                                        const int* __restrict__ flags, uint8_t* __restrict__ arena) {
+// gathers the per-slot strings into one contiguous buffer at the scanned offsets; one warp per slot.  Given flags (an arena batch),
+// only a committed batch is written: none of the flags of segm_rle_kernel and segm_offsets_kernel raised.
+static __global__ void __launch_bounds__(256) segm_compact_kernel(const uint8_t* __restrict__ strings, const int* __restrict__ str_len, int D,
+                                                                  int str_cap, const long long* __restrict__ offsets,
+                                                                  const int* __restrict__ flags, uint8_t* __restrict__ packed) {
     const int d = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (d >= D || flags[0] || flags[1] || flags[2]) return;
+    if (d >= D || (flags && (flags[0] || flags[1] || flags[2]))) return;
     const int n = str_len[d];
-    uint8_t* dst = arena + offsets[d];
+    uint8_t* dst = packed + offsets[d];
     const uint8_t* src = strings + (size_t)d * str_cap;
     for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }
@@ -394,6 +352,7 @@ static __global__ void __launch_bounds__(256) segm_paste_kernel(const float* __r
     }
     __syncthreads();
     const double scale_x = 1.0 / ((double)g.w / (double)S), scale_y = 1.0 / ((double)g.h / (double)S);
+    const bool area2 = g.w * 2 == S && g.h * 2 == S;
     for (int y = 0; y < im_h; ++y) {
         const bool inrow = y >= g.y0 && y < g.y1;
         AxisCoef cy; cy.s = 0; cy.w0 = cy.w1 = 0.f;
@@ -403,9 +362,8 @@ static __global__ void __launch_bounds__(256) segm_paste_kernel(const float* __r
             uint8_t v = 0;
             if (inrow && x >= g.x0 && x < g.x1) {
                 const AxisCoef cx = resize_coef_x(x - g.bx0, scale_x, S);
-                const float val = (g.w * 2 == S && g.h * 2 == S)
-                                      ? segm_area2(pm, S, x - g.bx0, y - g.by0, g.w)
-                                      : __fadd_rn(__fmul_rn(segm_hrow(pm, S, r0, cx), cy.w0), __fmul_rn(segm_hrow(pm, S, r1, cx), cy.w1));
+                const float val = segm_pixel(pm, S, area2, x - g.bx0, y - g.by0, g.w, segm_hrow(pm, S, r0, cx), segm_hrow(pm, S, r1, cx),
+                                             cy.w0, cy.w1);
                 v = val > thresh ? 1 : 0;
             }
             o[(size_t)y * im_w + x] = v;

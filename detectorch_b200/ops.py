@@ -140,6 +140,33 @@ def nms(dets, thresh):
     return keep[:int(cnt.item())]
 
 
+def _segm_grow_and_redo(run, runs_cap):
+    """run(runs_cap) -> (the most runs a detection needed beyond runs_cap, or 0; result), redone with a larger runs_cap until it is 0."""
+    while True:
+        need, out = run(runs_cap)
+        if need == 0:
+            return out
+        runs_cap = max(2 * runs_cap, need + 1)     # a detection needed more runs than provisioned: grow and redo
+
+
+def _segm_batch_args(who, masks, classes, boxes, num_dets):
+    """Checks a batch's masks [B,cap,M,M] or [B,cap,K,M,M] (with classes [B,cap]) and boxes [B,cap,4], and converts them and num_dets
+    ([B], None = all cap slots) for the device: -> (B, cap, K, M, masks, classes, boxes, num_dets)."""
+    if masks.dim() not in (4, 5) or boxes.dim() != 3 or boxes.size(2) != 4:
+        raise ValueError("%s: masks must be [B,cap,M,M] or [B,cap,K,M,M] and boxes [B,cap,4]" % who)
+    B, cap, M = masks.size(0), masks.size(1), masks.size(-1)
+    if tuple(boxes.shape[:2]) != (B, cap) or masks.size(-2) != M:
+        raise ValueError("%s: masks %s and boxes %s disagree" % (who, tuple(masks.shape), tuple(boxes.shape)))
+    if (masks.dim() == 5) != (classes is not None) or (classes is not None and tuple(classes.shape) != (B, cap)):
+        raise ValueError("%s: [B,cap,K,M,M] masks need classes [B,cap]; [B,cap,M,M] masks take none" % who)
+    K = masks.size(2) if masks.dim() == 5 else 1
+    masks, boxes = masks.contiguous().float(), boxes.contiguous().float()
+    if classes is not None:
+        classes = classes.contiguous().to(torch.int32)
+    nd = torch.full((B,), cap, dtype=torch.int32, device=masks.device) if num_dets is None else num_dets.contiguous().to(torch.int32)
+    return B, cap, K, M, masks, classes, boxes, nd
+
+
 def segm_rle(masks, classes, boxes, im_h, im_w, thresh=0.5, expanded=False, num_dets=None, runs_cap=4096):
     """Mask paste + COCO RLE on the device (lib/utils/result_utils.py:170-228).
     masks [D,K,M,M] (classes int32 [D] selects the plane) or [D,M,M]; boxes [D,4] fp32 reference boxes, or int32 already
@@ -160,7 +187,8 @@ def segm_rle(masks, classes, boxes, im_h, im_w, thresh=0.5, expanded=False, num_
         classes = classes.contiguous().to(torch.int32)
     L = _lib.lib()
     dev = masks.device
-    while True:
+
+    def run(runs_cap):
         ws = torch.empty((L.dt_segm_workspace_bytes(D, runs_cap),), dtype=torch.uint8, device=dev)
         counts = torch.empty((D, runs_cap), dtype=torch.int32, device=dev)
         ncount = torch.empty((D,), dtype=torch.int32, device=dev)
@@ -171,10 +199,9 @@ def segm_rle(masks, classes, boxes, im_h, im_w, thresh=0.5, expanded=False, num_
                            int(im_h), int(im_w), float(thresh), _p(counts), _p(ncount), runs_cap, _p(strings), _p(offs), _p(over), _p(ws),
                            _stream())
         _lib.check(ok, "dt_segm_rle")
-        need = int(over.item())
-        if need == 0:
-            break
-        runs_cap = max(2 * runs_cap, need + 1)     # a detection needed more runs than provisioned: grow and redo
+        return int(over.item()), (counts, ncount, strings, offs)
+
+    counts, ncount, strings, offs = _segm_grow_and_redo(run, runs_cap)
     offs_h = offs.cpu().numpy()
     str_h = strings[:int(offs_h[-1])].cpu().numpy().tobytes()
     n_h = ncount.cpu().numpy()
@@ -213,26 +240,16 @@ def segm_rle_batch_device(masks, classes, boxes, num_dets, im_sizes, thresh=0.5,
     """The launch half of segm_rle_batch: -> (packed strings on the device, host copies of [offsets int64 [B*cap+1], num_dets [B]] + the
     `extra` device tensors), all read in one synchronisation (after a grow-and-redo, one more per redo)."""
     _need_cuda(masks, classes, boxes, num_dets)
-    if masks.dim() not in (4, 5) or boxes.dim() != 3 or boxes.size(2) != 4:
-        raise ValueError("segm_rle_batch: masks must be [B,cap,M,M] or [B,cap,K,M,M] and boxes [B,cap,4]")
-    B, cap, M = masks.size(0), masks.size(1), masks.size(-1)
-    if tuple(boxes.shape[:2]) != (B, cap) or masks.size(-2) != M:
-        raise ValueError("segm_rle_batch: masks %s and boxes %s disagree" % (tuple(masks.shape), tuple(boxes.shape)))
-    if (masks.dim() == 5) != (classes is not None) or (classes is not None and tuple(classes.shape) != (B, cap)):
-        raise ValueError("segm_rle_batch: [B,cap,K,M,M] masks need classes [B,cap]; [B,cap,M,M] masks take none")
+    B, cap, K, M, masks, classes, boxes, nd = _segm_batch_args("segm_rle_batch", masks, classes, boxes, num_dets)
     sz = segm_image_sizes(im_sizes, B)
-    K = masks.size(2) if masks.dim() == 5 else 1
     dev = masks.device
-    masks, boxes = masks.contiguous().float(), boxes.contiguous().float()
-    if classes is not None:
-        classes = classes.contiguous().to(torch.int32)
-    nd = torch.full((B,), cap, dtype=torch.int32, device=dev) if num_dets is None else num_dets.contiguous().to(torch.int32)
     if B * cap == 0:
         host = to_host(nd, *extra)
         return torch.empty((0,), dtype=torch.uint8, device=dev), [np.zeros((B * cap + 1,), np.int64)] + host
     sizes = torch.from_numpy(sz.astype(np.int32)).to(dev)
     L = _lib.lib()
-    while True:
+
+    def run(runs_cap):
         ws = torch.empty((L.dt_segm_batch_workspace_bytes(B, cap, runs_cap),), dtype=torch.uint8, device=dev)
         strings = torch.empty((L.dt_segm_batch_strings_bytes(B, cap, runs_cap),), dtype=torch.uint8, device=dev)
         offs = torch.empty((B * cap + 1,), dtype=torch.int64, device=dev)
@@ -241,10 +258,9 @@ def segm_rle_batch_device(masks, classes, boxes, num_dets, im_sizes, thresh=0.5,
                                  float(thresh), runs_cap, _p(strings), _p(offs), _p(over), _p(ws), _stream())
         _lib.check(ok, "dt_segm_rle_batch")
         host = to_host(offs, over, nd, *extra)
-        need = int(host[1][0])
-        if need == 0:
-            return strings, [host[0], host[2]] + host[3:]
-        runs_cap = max(2 * runs_cap, need + 1)     # a detection needed more runs than provisioned: grow and redo
+        return int(host[1][0]), (strings, [host[0], host[2]] + host[3:])
+
+    return _segm_grow_and_redo(run, runs_cap)
 
 
 SEGM_APPEND_MAX_SIDE = 8192     # DT_SEGM_APPEND_MAX_SIDE: the largest image side segm_rle_batch_append encodes
@@ -257,23 +273,13 @@ def segm_rle_batch_append(masks, classes, boxes, num_dets, im_sizes, arena, curs
     both on the device: flags [0] the runs a slot needed beyond runs_cap, [1] an image size outside [1, SEGM_APPEND_MAX_SIDE], [2] the
     strings did not fit (cursor + offsets[-1] - offsets[0] > capacity).  With a flag raised, the arena and the cursor are untouched."""
     _need_cuda(masks, classes, boxes, num_dets, im_sizes, arena, cursor)
-    if masks.dim() not in (4, 5) or boxes.dim() != 3 or boxes.size(2) != 4:
-        raise ValueError("segm_rle_batch_append: masks must be [B,cap,M,M] or [B,cap,K,M,M] and boxes [B,cap,4]")
-    B, cap, M = masks.size(0), masks.size(1), masks.size(-1)
-    if tuple(boxes.shape[:2]) != (B, cap) or masks.size(-2) != M:
-        raise ValueError("segm_rle_batch_append: masks %s and boxes %s disagree" % (tuple(masks.shape), tuple(boxes.shape)))
-    if (masks.dim() == 5) != (classes is not None) or (classes is not None and tuple(classes.shape) != (B, cap)):
-        raise ValueError("segm_rle_batch_append: [B,cap,K,M,M] masks need classes [B,cap]; [B,cap,M,M] masks take none")
+    B, cap, K, M, masks, classes, boxes, nd = _segm_batch_args("segm_rle_batch_append", masks, classes, boxes, num_dets)
     if tuple(im_sizes.shape) != (B, 2) or im_sizes.dtype != torch.int32 or cursor.dtype != torch.int64 or cursor.numel() != 1:
         raise ValueError("segm_rle_batch_append: im_sizes must be int32 [%d, 2] and cursor int64 [1]" % B)
     if arena is not None and (arena.dtype != torch.uint8 or arena.dim() != 1 or not arena.is_contiguous()):
         raise ValueError("segm_rle_batch_append: the arena must be a contiguous uint8 vector")
-    K = masks.size(2) if masks.dim() == 5 else 1
     dev = masks.device
-    masks, boxes, im_sizes = masks.contiguous().float(), boxes.contiguous().float(), im_sizes.contiguous()
-    if classes is not None:
-        classes = classes.contiguous().to(torch.int32)
-    nd = torch.full((B,), cap, dtype=torch.int32, device=dev) if num_dets is None else num_dets.contiguous().to(torch.int32)
+    im_sizes = im_sizes.contiguous()
     offs = torch.empty((B * cap + 1,), dtype=torch.int64, device=dev)
     flags = torch.zeros((3,), dtype=torch.int32, device=dev)
     if B * cap == 0:

@@ -9,7 +9,7 @@ in tests/golden/resize_edges_golden.npz).  Importable without the reference.
   fx     (H, W, fx) straight through cv2.resize(fx=fy=fx) after the mean subtraction: both sides odd at fx = 0.5 (no target / max
          size gives that), fx a few ulp either side of 0.5 (1 / fx is then not 2: the bilinear kernel, not the area-fast one), and
          factors other than 1 that keep the size (OpenCV copies the image then)
-  masks  mask paste + RLE (segm_results; segm_rle_slot, segm_paste_kernel, segm_rle_bounded_kernel) for M = 28 and 14, class-specific
+  masks  mask paste + RLE (segm_results; segm_rle_kernel, segm_paste_kernel) for M = 28 and 14, class-specific
          [D, K, M, M] stacks with one class per detection, on images of 1x1, 1xN, Nx1, 2x2, odd sizes (23x37, 31x17, 47x45), 13x1500 and 600x11; boxes of
          every family in `FAMILIES`, clipped to the image (the reference raises on boxes outside it); masks uniform random, in
          multiples of 1/8 (interpolated values land exactly on the 0.5 threshold), constant 0.5, ones, zeros and a checkerboard."""

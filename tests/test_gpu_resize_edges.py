@@ -4,10 +4,10 @@ reference's own blob.py and segm_results computed with the real cv2 (tests/golde
   prep   prep_image_kernel through image_to_blob (fpn_on off and on), prep_im_for_blob, images_to_batch (a ragged batch of the odd-size
          exact 2x down-scales on a fixed canvas) and dt_prep_image at fx a few ulp from 0.5; full-size 1600x2003 @ 800 and 2666x1003
          capped at 1333 (im_scale == 0.5 with an odd side whose half rounds up) against the oracle computed here
-  masks  segm_paste_kernel, segm_rle_kernel and segm_rle_bounded_kernel through segm_paste, segm_rle (counts and strings, class-specific
-         and class-agnostic masks, a runs_cap of 2 that forces the grow-and-redo), segm_rle_batch (every image of a mask size in one
-         launch, per-image sizes, num_dets trimming, regrow) and segm_rle_batch_append into an arena; the table bound of the bounded
-         kernel at 1x8192 and 8192x1 (against the oracle) and 8193 (flag raised, arena and cursor untouched)."""
+  masks  segm_paste_kernel and segm_rle_kernel through segm_paste, segm_rle (counts and strings, class-specific and class-agnostic
+         masks, a runs_cap of 2 that forces the grow-and-redo), segm_rle_batch (every image of a mask size in one launch, per-image
+         sizes, num_dets trimming, regrow) and segm_rle_batch_append into an arena; the 8192-side table bound of the arena launch at
+         1x8192 and 8192x1 (against the oracle) and 8193 (flag raised, arena and cursor untouched)."""
 import ctypes
 import os
 
@@ -180,7 +180,7 @@ def test_segm_batch_and_append(dev, G, M):
 
 
 def test_segm_bounded_table_limits(dev):
-    """segm_rle_bounded_kernel's tables hold a side of 8192: 1x8192 and 8192x1 images encode as the oracle does; a side of 8193 raises
+    """segm_rle_batch_append's tables hold a side of 8192: 1x8192 and 8192x1 images encode as the oracle does; a side of 8193 raises
     flags[1] and leaves the arena and the cursor as they were."""
     from detectorch_b200 import ops
     from oracle import ref
