@@ -60,10 +60,10 @@ SIGNATURES = {
     "dt_coco_eval_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int]),
     "dt_coco_eval": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                              c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                             c_void_p, c_void_p]),
+                             c_void_p, c_void_p, c_void_p]),
     "dt_coco_eval_imgs": (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                  c_void_p, c_void_p]),
+                                  c_void_p, c_void_p, c_void_p]),
     "dt_coco_results_append": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
     "dt_coco_results_count": (c_int, [c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p,
@@ -72,6 +72,14 @@ SIGNATURES = {
                                       c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_coco_json": (c_int, [c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_void_p]),
+    "dt_coco_file_struct_workspace_bytes": (c_int64, [c_int64]),
+    "dt_coco_file_struct": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_coco_file_separators": (c_int, [c_int64, c_void_p, c_void_p, c_void_p]),
+    "dt_coco_file_records": (c_int, [c_int64, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dt_coco_file_finish_workspace_bytes": (c_int64, [c_int64, c_int64, c_int]),
+    "dt_coco_file_finish": (c_int, [c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p,
+                                    c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dt_proposal_recall_smem_bytes": (c_int64, [c_int, c_int64]),
     "dt_proposal_recall": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64,
                                    c_void_p, c_void_p, c_void_p]),

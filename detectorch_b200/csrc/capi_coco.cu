@@ -5,6 +5,7 @@
 #include "../../include/detectorch_b200.h"
 #include "coco_eval.cuh"
 #include "coco_json.cuh"
+#include "coco_results_file.cuh"
 #include "common.cuh"
 #include "proposal_recall.cuh"
 
@@ -49,7 +50,7 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
                             const int64_t* cat_kept, const int64_t* order_off, int64_t num_dets, const double* det_f, const int64_t* det_i,
                             const char* det_chars, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
                             const double* gt_f, const int64_t* gt_i, const uint32_t* gt_counts, const double* params, double* precision,
-                            double* recall, double* scores, double* ious, void* workspace, dt_stream_t stream) {
+                            double* recall, double* scores, double* ious, void* workspace, dt_stream_t stream, const double* det_area) {
     if ((iou_type != 0 && iou_type != 1) || num_images < 0 || num_cats < 0 || num_active < 0 || num_dets < 0 || num_chars < 0 || kept < 0 ||
         num_ious < 0 || num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || (int64_t)num_cats * 120 >= (1ll << 31) ||
         kCocoMaxDets * kept >= (1ll << 31)) {
@@ -65,7 +66,7 @@ extern "C" int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_
     }
     DT_CHECK_CUDA(coco_eval_launch(iou_type, num_images, num_cats, num_active, pairs, cat_gt, cat_kept, order_off, num_dets, det_f, det_i,
                                    det_chars, num_chars, kept, num_ious, num_gts, num_order, gt_f, gt_i, gt_counts, params, precision, recall,
-                                   scores, ious, workspace, (cudaStream_t)stream));
+                                   scores, ious, workspace, (cudaStream_t)stream, det_area));
     return 1;
 }
 
@@ -73,7 +74,7 @@ extern "C" int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* uni
                                  const double* det_f, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
                                  const int64_t* gt_keys, const double* gt_f, const int64_t* gt_i, const double* params, const double* ious,
                                  const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos, uint8_t* gt_ig,
-                                 dt_stream_t stream) {
+                                 dt_stream_t stream, const double* det_area) {
     if ((iou_type != 0 && iou_type != 1) || num_union < 0 || num_active < 0 || num_dets < 0 || num_chars < 0 || kept < 0 || num_ious < 0 ||
         num_gts < 0 || num_order < 0 || kept > num_dets || num_active > num_dets || num_active > num_union) {
         fprintf(stderr, "dt_coco_eval_imgs: bad sizes\n");
@@ -87,7 +88,7 @@ extern "C" int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* uni
     }
     DT_CHECK_CUDA(coco_eval_imgs_launch(iou_type, num_union, union_keys, num_active, pairs, num_dets, num_chars, kept, num_ious, num_gts, num_order,
                                         gt_keys, det_f, gt_f, gt_i, params, ious, workspace, slot_det, dt_gt, dt_ig, gt_dt, gt_pos, gt_ig,
-                                        (cudaStream_t)stream));
+                                        (cudaStream_t)stream, det_area));
     return 1;
 }
 
@@ -158,6 +159,66 @@ extern "C" int dt_coco_json(int iou_type, int64_t num_dets, const double* det_f,
     }
     JsonRows R{num_dets, num_images, det_f, det_key, file_pos, img_ids, cat_ids, det_i, det_chars, counts_first};
     DT_CHECK_CUDA(coco_json_launch(iou_type, R, offsets, lens, text, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int64_t dt_coco_file_struct_workspace_bytes(int64_t num_bytes) {
+    if (num_bytes < 1) return 0;
+    return (int64_t)cf_struct_ws(num_bytes).total;
+}
+
+extern "C" int dt_coco_file_struct(int64_t num_bytes, const uint8_t* text, void* workspace, int64_t* info, dt_stream_t stream) {
+    if (num_bytes < 1) { fprintf(stderr, "dt_coco_file_struct: empty text\n"); return 0; }
+    if (!text || !workspace || !info) { fprintf(stderr, "dt_coco_file_struct: null argument\n"); return 0; }
+    DT_CHECK_CUDA(cf_struct_launch(num_bytes, text, reinterpret_cast<uint8_t*>(workspace), reinterpret_cast<unsigned long long*>(info),
+                                   (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int dt_coco_file_separators(int64_t num_bytes, void* workspace, int64_t* separators, dt_stream_t stream) {
+    if (num_bytes < 1) { fprintf(stderr, "dt_coco_file_separators: empty text\n"); return 0; }
+    if (!workspace || !separators) { fprintf(stderr, "dt_coco_file_separators: null argument\n"); return 0; }
+    DT_CHECK_CUDA(cf_separators_launch(num_bytes, reinterpret_cast<uint8_t*>(workspace), separators, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int dt_coco_file_records(int64_t num_records, int64_t num_bytes, const uint8_t* text, const int64_t* separators, int num_images,
+                                    const int64_t* img_ids, int num_cats, const int64_t* cat_ids, double* rec_f, int64_t* rec_open, int64_t* rec_i,
+                                    int64_t* rec_n, uint8_t* rec_b, int64_t* info, dt_stream_t stream) {
+    if (num_records < 0 || num_bytes < 1 || num_images < 0 || num_cats < 0) { fprintf(stderr, "dt_coco_file_records: bad sizes\n"); return 0; }
+    if (num_records == 0) return 1;
+    if (!text || !separators || (num_images > 0 && !img_ids) || (num_cats > 0 && !cat_ids) || !rec_f || !rec_open || !rec_i || !rec_n || !rec_b ||
+        !info) {
+        fprintf(stderr, "dt_coco_file_records: null argument\n");
+        return 0;
+    }
+    CfArgs a{num_records, text, separators, num_images, num_cats, img_ids, cat_ids, rec_f, rec_open, rec_i, rec_n, rec_b,
+             reinterpret_cast<unsigned long long*>(info)};
+    DT_CHECK_CUDA(cf_records_launch(a, num_bytes, (cudaStream_t)stream));
+    return 1;
+}
+
+extern "C" int64_t dt_coco_file_finish_workspace_bytes(int64_t num_records, int64_t num_chars, int segm) {
+    if (num_records < 1 || num_chars < 0) return 0;
+    return (int64_t)cf_finish_ws(num_records, num_chars, segm).total;
+}
+
+extern "C" int dt_coco_file_finish(int64_t num_records, int segm, const uint8_t* text, const int64_t* rec_i, const int64_t* rec_n,
+                                   const int64_t* offsets, const uint8_t* rec_b, double* rec_f, int num_images, int num_cats, int64_t num_chars,
+                                   char* chars, void* workspace, int64_t num_kept, int64_t* det_key, double* det_f, int64_t* det_i,
+                                   double* det_area, int64_t* det_id, int64_t* info, dt_stream_t stream) {
+    if (num_records < 1 || num_images < 0 || num_cats < 0 || num_chars < 0 || num_kept < 0 || num_kept > num_records) {
+        fprintf(stderr, "dt_coco_file_finish: bad sizes\n");
+        return 0;
+    }
+    if (!text || !rec_i || !rec_n || !offsets || !rec_b || !rec_f || !chars || !workspace || !det_key || !info ||
+        (num_kept > 0 && (!det_f || !det_i || !det_area || !det_id))) {
+        fprintf(stderr, "dt_coco_file_finish: null argument\n");
+        return 0;
+    }
+    DT_CHECK_CUDA(cf_finish_launch(num_records, segm, text, rec_i, rec_n, offsets, rec_b, rec_f, num_images, num_cats, num_chars, chars,
+                                   reinterpret_cast<uint8_t*>(workspace), num_kept, det_key, det_f, det_i, det_area, det_id,
+                                   reinterpret_cast<unsigned long long*>(info), (cudaStream_t)stream));
     return 1;
 }
 

@@ -304,6 +304,7 @@ inline cudaError_t coco_det_check_launch(int64_t n, const int64_t* det_i, const 
 
 struct CocoEvalArgs {
     int segm, num_images;
+    int use_area;             // det_area holds each detection's area (segm: the RLE area; else the caller's), not w h
     const int64_t* pairs;
     const double* det_f; const int64_t* det_i;
     const uint32_t* det_cnts; const int64_t* det_m; const double* det_area; const double* det_rbox;
@@ -381,7 +382,7 @@ __global__ void coco_pair_kernel(CocoEvalArgs p) {
                 gm[m] = 1;
             }
             const int64_t d = p.kept_det[k0 + dr];
-            const double area = p.segm ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
+            const double area = p.use_area ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
             if (!hit && coco_out(area, rng)) dig = true;
             p.state[(k0 + dr) * kCocoStates + c] = (uint8_t)((hit ? 1 : 0) | (dig ? 2 : 0));
         }
@@ -543,21 +544,24 @@ inline cudaError_t coco_eval_launch(int segm, int num_images, int K, int n_activ
                                     const int64_t* cat_kept, const int64_t* order_off, int64_t n_det, const double* det_f,
                                     const int64_t* det_i, const char* det_chars, int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt,
                                     int64_t n_order, const double* gt_f, const int64_t* gt_i, const uint32_t* gt_cnts, const double* par,
-                                    double* precision, double* recall, double* scores, double* ious, void* workspace, cudaStream_t st) {
+                                    double* precision, double* recall, double* scores, double* ious, void* workspace, cudaStream_t st,
+                                    const double* det_area = nullptr) {
     const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order, K);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    double* rle_area = reinterpret_cast<double*>(ws + L.det_area);
     CocoEvalArgs p;
     p.segm = segm; p.num_images = num_images; p.pairs = pairs;
+    p.use_area = segm || det_area != nullptr;
     p.det_f = det_f; p.det_i = det_i;
     p.det_cnts = reinterpret_cast<uint32_t*>(ws + L.det_cnts); p.det_m = reinterpret_cast<int64_t*>(ws + L.det_m);
-    p.det_area = reinterpret_cast<double*>(ws + L.det_area); p.det_rbox = reinterpret_cast<double*>(ws + L.det_rbox);
+    p.det_area = det_area ? det_area : rle_area; p.det_rbox = reinterpret_cast<double*>(ws + L.det_rbox);
     p.gt_f = gt_f; p.gt_i = gt_i; p.gt_cnts = gt_cnts; p.par = par;
     p.kept_det = reinterpret_cast<int*>(ws + L.kept_det); p.kept_rank = reinterpret_cast<int*>(ws + L.kept_rank);
     p.kept_score = reinterpret_cast<double*>(ws + L.kept_score); p.state = ws + L.state;
     p.iou = ious ? ious : reinterpret_cast<double*>(ws + L.iou); p.gtm = ws + L.gtm;
     int* order = reinterpret_cast<int*>(ws + L.order);
     if (segm && n_det > 0) {
-        coco_det_rle_kernel<<<(unsigned)((n_det + 127) / 128), 128, 0, st>>>(n_det, det_i, det_chars, const_cast<uint32_t*>(p.det_cnts), const_cast<int64_t*>(p.det_m), const_cast<double*>(p.det_area), const_cast<double*>(p.det_rbox));
+        coco_det_rle_kernel<<<(unsigned)((n_det + 127) / 128), 128, 0, st>>>(n_det, det_i, det_chars, const_cast<uint32_t*>(p.det_cnts), const_cast<int64_t*>(p.det_m), rle_area, const_cast<double*>(p.det_rbox));
     }
     if (n_active > 0) {
         coco_pair_kernel<<<n_active, 128, 0, st>>>(p);
@@ -780,7 +784,7 @@ inline cudaError_t coco_results_write_launch(int64_t n, const float* rec_f, cons
 //   gt_dt [gts][40]        rank in its pair of the last kept detection that matched the gt (a crowd gt matches several), -1 for none
 //   gt_pos [gts][4]        the gt's position in the area range's ignore-last order;  gt_ig [gts][4] its ignore flag
 struct CocoEvalImgsArgs {
-    int segm;
+    int segm, use_area;       // as CocoEvalArgs
     int64_t n_active, n_gt;
     const int64_t* ukeys; const int64_t* pairs; const int64_t* gt_keys;
     const double* det_f; const double* det_area; const int* kept_det;
@@ -844,7 +848,7 @@ __global__ void coco_eval_imgs_kernel(CocoEvalImgsArgs p) {
                 gm[m * kCocoStates] = (int)dr;
             }
             const int64_t d = p.kept_det[k0 + dr];
-            const double area = p.segm ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
+            const double area = p.use_area ? p.det_area[d] : __dmul_rn(p.det_f[d * kCocoDetF + 3], p.det_f[d * kCocoDetF + 4]);
             if (!hit && coco_out(area, rng)) dig = true;
             p.dt_gt[(k0 + dr) * kCocoStates + c] = (int)m;
             p.dt_ig[(k0 + dr) * kCocoStates + c] = dig;
@@ -857,13 +861,13 @@ inline cudaError_t coco_eval_imgs_launch(int segm, int n_union, const int64_t* u
                                          int64_t n_chars, int64_t kept, int64_t n_iou, int64_t n_gt, int64_t n_order, const int64_t* gt_keys,
                                          const double* det_f, const double* gt_f, const int64_t* gt_i, const double* par, const double* ious,
                                          const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos,
-                                         uint8_t* gt_ig, cudaStream_t st) {
+                                         uint8_t* gt_ig, cudaStream_t st, const double* det_area = nullptr) {
     const CocoEvalWs L = coco_eval_ws(n_det, n_chars, kept, n_iou, n_gt, n_order);
     const uint8_t* ws = reinterpret_cast<const uint8_t*>(workspace);
     CocoEvalImgsArgs p;
-    p.segm = segm; p.n_active = n_active; p.n_gt = n_gt;
+    p.segm = segm; p.use_area = segm || det_area != nullptr; p.n_active = n_active; p.n_gt = n_gt;
     p.ukeys = ukeys; p.pairs = pairs; p.gt_keys = gt_keys;
-    p.det_f = det_f; p.det_area = reinterpret_cast<const double*>(ws + L.det_area); p.kept_det = reinterpret_cast<const int*>(ws + L.kept_det);
+    p.det_f = det_f; p.det_area = det_area ? det_area : reinterpret_cast<const double*>(ws + L.det_area); p.kept_det = reinterpret_cast<const int*>(ws + L.kept_det);
     p.gt_f = gt_f; p.gt_i = gt_i; p.par = par; p.iou = ious;
     p.slot_det = slot_det; p.dt_gt = dt_gt; p.dt_ig = dt_ig; p.gt_dt = gt_dt; p.gt_pos = gt_pos; p.gt_ig = gt_ig;
     if (n_union > 0) coco_eval_imgs_kernel<<<n_union, 64, 0, st>>>(p);

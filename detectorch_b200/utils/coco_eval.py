@@ -9,6 +9,7 @@ file that lib/utils/json_dataset_evaluator.py would write; no file is written.
     p = Params(gt, "bbox"); p.imgIds = ids[:500]; p.useCats = 0; E = evaluate(gt, results, "bbox", params=p)   # subsets, class-agnostic
     E = evaluate(gt, results, "bbox", keep_eval_imgs=True)  # + COCOeval's per-image records:
     E.eval_imgs["dtMatches"], E.evalImgs[n]               # as flat columns, or as COCOeval's list of dicts (built when first read)
+    R = load_results(gt, "segm_results.json"); E = evaluate(gt, R, "segm")   # a results file, parsed on the device (COCO.loadRes)
 
 keep_eval_imgs=True runs one more kernel after the evaluation, on the IoUs it kept; the records' detection ids are the ones loadRes
 gives the rows of the results file (1 + the row's index), their GT ids the annotation ids.
@@ -628,7 +629,8 @@ def _flatten_results(gt, all_boxes, all_segms, iou_type, category_ids, with_ids=
 def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious=False, keep_eval_imgs=False, params=None):
     """COCOeval(gt, loadRes(results file), iou_type).evaluate() + accumulate() on the device -> CocoEvalResult.
     results: detect_images() / batch_results() output (one tuple per image, images in sorted-id order), the notebooks' all_boxes
-    [class][image] (with all_segms [class][image] for 'segm'), or a DeviceResults (flattened on the device, on gt's device).  category_ids: json id of contiguous class j (1-based) at j - 1;
+    [class][image] (with all_segms [class][image] for 'segm'), a DeviceResults (flattened on the device, on gt's device), or a
+    LoadedResults (load_results(gt, results file): the evaluation is COCOeval(G, G.loadRes(file), iou_type)'s).  category_ids: json id of contiguous class j (1-based) at j - 1;
     default: the dataset's category order, as JsonDataset builds its classes.  keep_ious: also return COCOeval's .ious, {(image id,
     category id): [min(D, 100), G] array} for the pairs with detections and GTs.  keep_eval_imgs: also return COCOeval's per-image
     records, as .eval_imgs (columns, see _eval_imgs_columns) and .evalImgs (the list of dicts, built from the columns when first read);
@@ -644,6 +646,11 @@ def evaluate(gt, results, iou_type, all_segms=None, category_ids=None, keep_ious
         raise TypeError("gt must be a CocoGroundTruth")
     if iou_type == 'segm' and not gt.has_masks:
         raise ValueError("segm evaluation: some ground-truth annotations have no segmentation")
+    if isinstance(results, LoadedResults):
+        if all_segms is not None or category_ids is not None:
+            raise ValueError("a LoadedResults carries its masks and json category ids; all_segms and category_ids are for all_boxes input")
+        p = Params(gt, iou_type) if params is None else _normalised_params(gt, params, iou_type)
+        return _evaluate_loaded(gt, results, iou_type, keep_ious, keep_eval_imgs, p)
     category_ids = list(gt.category_ids if category_ids is None else category_ids)
     if any(c not in set(gt.cat_ids) for c in category_ids):
         raise ValueError("category_ids names a category the ground truth does not have")
@@ -699,10 +706,11 @@ def _pair_tables(gt, key):
 
 
 def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_f_d, det_i_d, ch, num_chars, n_kept, n_iou, n_order, keep_ious,
-                     imgs, params):
+                     imgs, params, det_area_d=None):
     """dt_coco_eval on the flattened results, already on gt's device (pairs: their host copy, or None to read it back for keep_ious).
     gt: the CocoGroundTruth, or its _GtView for params.  imgs: (union keys [Q], detection ids [N]) on the device to also run
-    dt_coco_eval_imgs, None to leave it out."""
+    dt_coco_eval_imgs, None to leave it out.  det_area_d: each detection's area for the area ranges (a results file's loadRes area),
+    None for w h of the box ('bbox') or the RLE area ('segm')."""
     I, K, N = gt.num_images, gt.num_cats, int(det_f_d.shape[0])
     dev = gt.device
     T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
@@ -726,7 +734,8 @@ def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_
     ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
     _lib.check(L.dt_coco_eval(1 if iou_type == 'segm' else 0, I, K, int(pairs_d.shape[0]), _p(pairs_d), _p(cat_gt_d), _p(cat_kept_d),
                               _p(order_off_d), N, _p(det_f_d), _p(det_i_d), _p(ch), num_chars, n_kept, n_iou, gt.num_gts, n_order, _p(gt.gt_f),
-                              _p(gt.gt_i), _p(gt.gt_counts), _p(par_d), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev)), "dt_coco_eval")
+                              _p(gt.gt_i), _p(gt.gt_counts), _p(par_d), _p(prec), _p(rec), _p(scr), _p(ious), _p(ws), _stream(dev),
+                              _p(det_area_d)), "dt_coco_eval")
     if imgs is not None:
         ukeys_d, det_ids_d = imgs
         Q, G = int(ukeys_d.shape[0]), gt.num_gts
@@ -738,7 +747,8 @@ def _evaluate_tables(gt, iou_type, pairs, pairs_d, cat_kept_d, order_off_d, det_
         gt_ig = torch.empty((max(G, 1), A), dtype=torch.uint8, device=dev)
         _lib.check(L.dt_coco_eval_imgs(1 if iou_type == 'segm' else 0, Q, _p(ukeys_d), int(pairs_d.shape[0]), _p(pairs_d), N, _p(det_f_d),
                                        num_chars, n_kept, n_iou, G, n_order, _p(gt.keys_d), _p(gt.gt_f), _p(gt.gt_i), _p(par_d), _p(ious), _p(ws),
-                                       _p(slot_det), _p(dt_gt), _p(dt_ig), _p(gt_dt), _p(gt_pos), _p(gt_ig), _stream(dev)), "dt_coco_eval_imgs")
+                                       _p(slot_det), _p(dt_gt), _p(dt_ig), _p(gt_dt), _p(gt_pos), _p(gt_ig), _stream(dev),
+                                       _p(det_area_d)), "dt_coco_eval_imgs")
         # each kept slot's detection id and score, gathered on the device
         sd = slot_det[:n_kept].long()
         slot_id, slot_score = det_ids_d[sd], det_f_d[sd, 0]
@@ -1278,6 +1288,194 @@ def _umask():
     m = os.umask(0)
     os.umask(m)
     return m
+
+
+# ------------------------------------------------------------------------------------------------------------ reading a results file
+# error bits of csrc/coco_results_file.cuh, in the order they are reported
+_FILE_ERRORS = [(1 << 1, "a byte >= 0x80 (a json.dump file is ASCII)"), (1 << 0, "not valid JSON"),
+                (1 << 2, "the top level is not one JSON array"), (1 << 3, "an element of the array is not an object"),
+                (1 << 4, "values nested deeper than 64 levels"), (1 << 5, "a score or bbox number that is not finite as a double"),
+                (1 << 6, "'image_id' missing or not an integer literal in int64"),
+                (1 << 7, "an image_id that is not an image of the ground truth (loadRes asserts)"),
+                (1 << 8, "'category_id' missing or not an integer literal in int64"), (1 << 9, "'score' missing or not a number"),
+                (1 << 10, "a segmentation dict that is not a compressed RLE (string 'counts', 'size' [h, w] integers, 1 <= h w < 2^32)"),
+                (1 << 11, "RLE counts with a character outside '0'..'o', a value longer than 6 characters, or ending inside a value"),
+                (1 << 12, "RLE counts that do not sum to h * w")]
+_NO_BBOX, _BAD_BBOX, _NO_RLE = 1, 2, 4
+_HAS_BBOX, _BBOX_EMPTY, _HAS_CAPTION = 1, 4, 16
+_INFO = 8
+
+
+class LoadedResults:
+    """A COCO results file as pycocotools' COCO.loadRes(file) hands it to COCOeval, held on the device (load_results).
+        branch          'bbox' or 'segm': loadRes's branch, decided by the first record ('bbox' when it has a bbox that is not [])
+        num_records     records in the file;  num_dropped: those of categories the ground truth does not have (COCOeval never
+                        selects them)
+    The detections of the other records are kept in dt_coco_eval's layout, sorted by (category, image), file order inside a pair;
+    their loadRes ids are 1 + their index in the file and their 'area' is loadRes's (bbox branch: w h; segm branch: the RLE area).
+    evaluate(gt, loaded, 'bbox' | 'segm', ...) takes it any number of times, for either iou type."""
+
+    def __init__(self, gt, branch, num_records, num_dropped, key, det_f, det_i, det_area, det_ids, chars, num_chars, summary):
+        self.gt, self.branch, self.num_records, self.num_dropped = gt, branch, num_records, num_dropped
+        self._key, self._det_f, self._det_i, self._det_area, self._det_ids = key, det_f, det_i, det_area, det_ids
+        self._chars, self._num_chars, self._summary = chars, num_chars, summary
+
+    def __len__(self):
+        return len(self._key)
+
+
+def _read_text(source, dev):
+    """A path or a bytes-like object -> its bytes on the device, read into two pinned buffers of 64 MB and copied in chunks (the
+    read of the next chunk under the copy of this one)."""
+    import os
+    if isinstance(source, (str, os.PathLike)):
+        fh = open(source, "rb")
+        total = os.fstat(fh.fileno()).st_size
+    else:
+        try:
+            view = memoryview(source).cast("B")
+        except TypeError:
+            raise ValueError("load_results: source must be a path or a bytes-like object") from None
+        fh, total = None, view.nbytes
+    try:
+        text = torch.empty((max(total, 1),), dtype=torch.uint8, device=dev)
+        if total:
+            stage = [torch.empty((min(total, _JSON_CHUNK),), dtype=torch.uint8, pin_memory=True) for _ in range(1 + (total > _JSON_CHUNK))]
+            events = [None, None]
+            for c, a in enumerate(range(0, total, _JSON_CHUNK)):
+                b = min(a + _JSON_CHUNK, total)
+                if events[c % 2] is not None:
+                    events[c % 2].synchronize()         # the buffer's previous chunk has reached the device
+                buf = stage[c % 2].numpy()[:b - a]
+                if fh is None:
+                    buf[:] = np.frombuffer(view[a:b], np.uint8)
+                elif fh.readinto(memoryview(buf)) != b - a:
+                    raise ValueError("load_results: the file changed size while it was read")
+                text[a:b].copy_(stage[c % 2][:b - a], non_blocking=True)
+                events[c % 2] = torch.cuda.Event()
+                events[c % 2].record()
+            for e in events:
+                if e is not None:
+                    e.synchronize()
+    finally:
+        if fh is not None:
+            fh.close()
+    return text, total
+
+
+def _file_error(info, what):
+    err = int(info[1])
+    for bit, msg in _FILE_ERRORS:
+        if err & bit:
+            at = "" if info[4] == np.iinfo(np.int64).max else " (record %d)" % info[4]
+            raise ValueError("%s: %s%s" % (what, msg, at))
+
+
+def load_results(gt, source):
+    """COCO.loadRes(source) on the device -> LoadedResults for evaluate(gt, loaded, 'bbox' | 'segm').  source: the path of a COCO
+    results json (a list of {"image_id", "category_id", "score", "bbox" and / or "segmentation"} records, as the reference's results
+    writers, detectron2 or mmdetection write them) or a bytes-like object holding one.  The file is copied to the device once and
+    parsed there (csrc/coco_results_file.cuh): numbers become the doubles json.loads gives, the last occurrence of a key wins, keys
+    loadRes does not read are skipped.  Records of categories gt does not have are kept out (COCOeval never selects them).
+    Raises ValueError, before anything is evaluated, for text json.loads rejects and for NaN / Infinity and non-ASCII bytes (json.dump
+    writes neither), a top level that is not an array of objects, an image_id or category_id that is not an integer literal in int64
+    or an image_id that is not an image of gt (loadRes asserts), a missing or non-numeric score, a number that is not finite as a
+    double, a bbox that is not 4 numbers in the bbox branch, a record without a compressed RLE in the segm branch, a segmentation dict
+    that is not a valid compressed RLE (its counts are checked as list input's are), nesting deeper than 64 levels, and a first record
+    with a 'caption' (loadRes's caption branch).
+    Unlike loadRes, which raises IndexError on it, an empty array [] gives results with no detections."""
+    if not isinstance(gt, CocoGroundTruth):
+        raise TypeError("gt must be a CocoGroundTruth")
+    dev, what = gt.device, "results file"
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        text, n = _read_text(source, dev)
+        if n == 0:
+            raise ValueError("%s: empty (not valid JSON)" % what)
+        st = _stream(dev)
+        info = torch.zeros((_INFO,), dtype=torch.int64, device=dev)
+        info[4] = np.iinfo(np.int64).max
+        ws = torch.empty((L.dt_coco_file_struct_workspace_bytes(n),), dtype=torch.uint8, device=dev)
+        _lib.check(L.dt_coco_file_struct(n, _p(text), _p(ws), _p(info), st), "dt_coco_file_struct")
+        h = info.cpu().numpy()
+        _file_error(h, what)
+        if h[5] != 1 or h[0] < 2:
+            raise ValueError("%s: the top level is not one JSON array" % what)
+        sep = torch.empty((int(h[0]),), dtype=torch.int64, device=dev)
+        _lib.check(L.dt_coco_file_separators(n, _p(ws), _p(sep), st), "dt_coco_file_separators")
+        R = int(h[0]) - 1
+        img_d = torch.tensor(gt.img_ids or [0], dtype=torch.int64, device=dev)
+        cat_d = torch.tensor(gt.cat_ids or [0], dtype=torch.int64, device=dev)
+        rec_f = torch.empty((R, 5), dtype=torch.float64, device=dev)
+        rec_open = torch.empty((R, 5), dtype=torch.int64, device=dev)
+        rec_i = torch.empty((R, 6), dtype=torch.int64, device=dev)
+        rec_n = torch.empty((R,), dtype=torch.int64, device=dev)
+        rec_b = torch.empty((R,), dtype=torch.uint8, device=dev)
+        _lib.check(L.dt_coco_file_records(R, n, _p(text), _p(sep), gt.num_images, _p(img_d), gt.num_cats, _p(cat_d), _p(rec_f), _p(rec_open),
+                                          _p(rec_i), _p(rec_n), _p(rec_b), _p(info), st), "dt_coco_file_records")
+        del ws
+        offs = torch.cumsum(rec_n, 0)
+        h = torch.cat([info, offs[-1:], rec_b[:1].to(torch.int64)]).cpu().numpy()
+        _file_error(h, what)
+        empty = bool(h[6])
+        num_chars, first = int(h[_INFO]), int(h[_INFO + 1])
+        if empty:
+            z = torch.zeros
+            return LoadedResults(gt, 'bbox', 0, 0, np.zeros(0, np.int64), z((0, 5), dtype=torch.float64, device=dev),
+                                 z((0, 4), dtype=torch.int64, device=dev), z((0,), dtype=torch.float64, device=dev),
+                                 z((0,), dtype=torch.int64, device=dev), z((1,), dtype=torch.uint8, device=dev), 0, 0)
+        if first & _HAS_CAPTION:
+            raise ValueError("%s: the first record has a 'caption' (loadRes's caption branch is not evaluated here)" % what)
+        branch = 'bbox' if (first & _HAS_BBOX) and not (first & _BBOX_EMPTY) else 'segm'
+        summary = int(h[2])
+        if branch == 'bbox' and summary & _NO_BBOX:
+            raise ValueError("%s: a record without a bbox of 4 numbers (the first record's bbox makes every record's bbox read)" % what)
+        if branch == 'segm' and summary & _NO_RLE:
+            raise ValueError("%s: a record without a compressed RLE segmentation (the first record has no bbox: loadRes reads every "
+                             "record's RLE)" % what)
+        N = R - int(h[3])
+        chars = torch.empty((num_chars + 1,), dtype=torch.uint8, device=dev)
+        ws = torch.empty((L.dt_coco_file_finish_workspace_bytes(R, num_chars, int(branch == 'segm')),), dtype=torch.uint8, device=dev)
+        det_key = torch.empty((R,), dtype=torch.int64, device=dev)
+        det_f = torch.empty((N, 5), dtype=torch.float64, device=dev)
+        det_i = torch.empty((N, 4), dtype=torch.int64, device=dev)
+        det_area = torch.empty((N,), dtype=torch.float64, device=dev)
+        det_ids = torch.empty((N,), dtype=torch.int64, device=dev)
+        _lib.check(L.dt_coco_file_finish(R, int(branch == 'segm'), _p(text), _p(rec_i), _p(rec_n), _p(offs), _p(rec_b), _p(rec_f), gt.num_images,
+                                         gt.num_cats, num_chars, _p(chars), _p(ws), N, _p(det_key), _p(det_f), _p(det_i), _p(det_area),
+                                         _p(det_ids), _p(info), st), "dt_coco_file_finish")
+        _file_error(info.cpu().numpy(), what)
+        key = det_key[:N].cpu().numpy()
+    return LoadedResults(gt, branch, R, R - N, key, det_f, det_i, det_area, det_ids, chars, num_chars, summary)
+
+
+def _evaluate_loaded(gt, res, iou_type, keep_ious, keep_eval_imgs, p):
+    """evaluate() of a LoadedResults: its tables, re-keyed for a Params view, with loadRes's areas."""
+    if res.gt is not gt:
+        raise ValueError("the results were loaded for another ground truth")
+    if iou_type == 'segm' and res._summary & _NO_RLE:
+        raise ValueError("segm evaluation of a results file with records without a compressed RLE (loadRes would make a polygon "
+                         "of their box; not supported)")
+    if iou_type == 'bbox' and res._summary & _BAD_BBOX:
+        raise ValueError("bbox evaluation of a results file with a bbox that is not 4 numbers")
+    view = None if _is_default(gt, p) else _GtView(gt, p)
+    ev = gt if view is None else view
+    key, det_f, det_i, det_area, det_ids = res._key, res._det_f, res._det_i, res._det_area, res._det_ids
+    dev = gt.device
+    if view is not None:
+        rows, fine = view.select(key)
+        rows_d = torch.from_numpy(rows).to(dev)
+        key = fine // view.per
+        det_f, det_i, det_area, det_ids = (x.index_select(0, rows_d) for x in (det_f, det_i, det_area, det_ids))
+    pairs, cat_kept, order_off = _pair_tables(ev, key)
+    kept, gn = np.minimum(pairs[:, 2], MAX_DETS[-1]), pairs[:, 4]
+    n_kept, n_iou, n_order = int(kept.sum()), int((kept * gn).sum()), int(order_off[-1, -1])
+    up = [torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (pairs, cat_kept, order_off)]
+    imgs = None
+    if keep_eval_imgs:
+        imgs = (torch.from_numpy(np.union1d(pairs[:, 0], ev.keys).astype(np.int64)).to(dev), det_ids)
+    return _evaluate_tables(ev, iou_type, pairs, *up, det_f.contiguous(), det_i.contiguous(), res._chars, res._num_chars, n_kept, n_iou,
+                            n_order, keep_ious, imgs, p, det_area.contiguous())
 
 
 # ------------------------------------------------------------------------------------------------------------ proposal recall

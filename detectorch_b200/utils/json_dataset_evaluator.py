@@ -6,7 +6,9 @@ json_dataset.COCO.dataset supplies the ground truth (built on the device once pe
 category_to_id_map give the json category id of each contiguous class, as _write_coco_*_results_file uses them.
 evaluate_box_proposals (:238-320) is the proposal recall of coco_eval.box_proposal_recall, one (area, limit) combination.
 _write_coco_bbox_results_file / _write_coco_segms_results_file (:67-190) write the reference's results json, byte for byte, with
-coco_eval.write_results (for test-dev, whose evaluation returns None, the file is the only output)."""
+coco_eval.write_results (for test-dev, whose evaluation returns None, the file is the only output).
+_do_detection_eval / _do_segmentation_eval (:116-125, :193-202) evaluate a results file, parsed on the device (coco_eval.load_results):
+    E = _do_segmentation_eval(json_dataset, "segmentations_results.json", output_dir)"""
 import logging
 import os
 
@@ -68,6 +70,25 @@ def _write_coco_bbox_results_file(json_dataset, all_boxes, res_file):
     """The reference's bbox results json, as _write_coco_segms_results_file."""
     logger.info('Writing bbox results json to: {}'.format(os.path.abspath(res_file)))
     coco_eval.write_results(_results_ground_truth(json_dataset), all_boxes, 'bbox', res_file, category_ids=_category_ids(json_dataset))
+
+
+def _do_file_eval(json_dataset, res_file, iou_type):
+    gt = _ground_truth(json_dataset)
+    E = coco_eval.evaluate(gt, coco_eval.load_results(gt, str(res_file)), iou_type)
+    _log_detection_eval_metrics(E)
+    return E
+
+
+def _do_segmentation_eval(json_dataset, res_file, output_dir):
+    """COCOeval(json_dataset.COCO, json_dataset.COCO.loadRes(res_file), 'segm') after evaluate() + accumulate(), logged -> the
+    evaluation (coco_eval.load_results + evaluate).  output_dir is accepted for the reference's signature; nothing is written (the
+    reference pickles the COCOeval object there)."""
+    return _do_file_eval(json_dataset, res_file, 'segm')
+
+
+def _do_detection_eval(json_dataset, res_file, output_dir):
+    """The 'bbox' evaluation of a results file, as _do_segmentation_eval."""
+    return _do_file_eval(json_dataset, res_file, 'bbox')
 
 
 def _log_detection_eval_metrics(E):

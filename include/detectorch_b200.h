@@ -321,6 +321,8 @@ int dt_engine_profile(dt_engine_t e, const float* image_nchw, float scaling_fact
  *   precision / scores [10, 101, K, 4, 3], recall [10, K, 4, 3] double
  *   ious                          optional [num_ious] double: each pair's IoU matrix [min(D, 100), G] (detections in score order, gts in
  *                                 annotation order) at its first IoU; NULL keeps them in the workspace
+ *   det_area                      optional [num_dets] double: each detection's area for the area ranges (loadRes's 'area' of a results
+ *                                 file); NULL: w h of its box for bbox, its RLE area for segm
  * dt_coco_det_check: bad [num_dets] uint8, 1 where a segm detection's string (det_i / det_chars as for dt_coco_eval) decodes to
  *   counts that do not sum to h * w.  rleIou never ends on such a mask, so dt_coco_eval must not be given one.
  * dt_coco_results_append / _count / _write: detect() batches kept on the device as records (utils.coco_eval.DeviceResults) and
@@ -357,18 +359,19 @@ int dt_coco_eval(int iou_type, int num_images, int num_cats, int num_active, con
                  const int64_t* order_off, int64_t num_dets, const double* det_f, const int64_t* det_i, const char* det_chars, int64_t num_chars,
                  int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order, const double* gt_f, const int64_t* gt_i,
                  const uint32_t* gt_counts, const double* params, double* precision, double* recall, double* scores, double* ious, void* workspace,
-                 dt_stream_t stream);
+                 dt_stream_t stream, const double* det_area);
 /* dt_coco_eval_imgs: COCOeval's per-image records (evalImgs) of the evaluation dt_coco_eval has just enqueued, from its workspace and
  * IoU matrices (every size argument and table as given to it; ious must not be NULL there).  union_keys [num_union] int64: the sorted
  * pair indices of the pairs with detections or gts; gt_keys [num_gts] each gt's pair index (sorted).  Outputs, state c = area * 10 +
  * threshold:  slot_det [kept] int: detection index of each kept slot;  dt_gt [kept, 40] int: index in its pair of the gt a kept detection
  * matched, -1 none;  dt_ig [kept, 40] uint8: dtIgnore;  gt_dt [num_gts, 40] int: rank in its pair of the last kept detection that matched
- * the gt, -1 none;  gt_pos [num_gts, 4] int: position in the area's ignore-last gt order;  gt_ig [num_gts, 4] uint8: gtIgnore. */
+ * the gt, -1 none;  gt_pos [num_gts, 4] int: position in the area's ignore-last gt order;  gt_ig [num_gts, 4] uint8: gtIgnore.
+ * det_area: the one given to dt_coco_eval. */
 int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* union_keys, int num_active, const int64_t* pairs, int64_t num_dets,
                       const double* det_f, int64_t num_chars, int64_t kept, int64_t num_ious, int64_t num_gts, int64_t num_order,
                       const int64_t* gt_keys, const double* gt_f, const int64_t* gt_i, const double* params, const double* ious,
                       const void* workspace, int* slot_det, int* dt_gt, uint8_t* dt_ig, int* gt_dt, int* gt_pos, uint8_t* gt_ig,
-                      dt_stream_t stream);
+                      dt_stream_t stream, const double* det_area);
 
 /* dt_coco_json: the COCO results json of the reference's results writers + json.dump, byte for byte, in two passes over the
  * flattened results (iou_type 0 bbox, 1 segm; det_f / det_i / det_chars as dt_coco_eval takes them, rows in any order).
@@ -382,6 +385,31 @@ int dt_coco_eval_imgs(int iou_type, int num_union, const int64_t* union_keys, in
 int dt_coco_json(int iou_type, int64_t num_dets, const double* det_f, const int64_t* det_key, const int64_t* file_pos, int num_images,
                  const int64_t* img_ids, const int64_t* cat_ids, const int64_t* det_i, const char* det_chars, const uint8_t* counts_first,
                  const int64_t* offsets, int64_t* lens, char* text, dt_stream_t stream);
+
+/* COCO results json read on the device (COCO.loadRes of a results file; detectorch_b200/csrc/coco_results_file.cuh), in four calls:
+ * dt_coco_file_struct: the structural pass over text [num_bytes] with a workspace of dt_coco_file_struct_workspace_bytes, kept for
+ *   dt_coco_file_separators.  info [8] int64 (zeroed, info[4] = INT64_MAX by the caller): separators, error bits, summary bits, records of
+ *   unknown categories, first record with an error, top-level '[' count, 1 for an empty array.
+ * dt_coco_file_separators: separators [info[0]] int64, the top-level '[', the ',' between records and the closing ']'.
+ * dt_coco_file_records: num_records = separators - 1; img_ids [num_images] / cat_ids [num_cats] the ground truth's sorted json ids;
+ *   rec_f [R, 5] double score, bbox x y w h (rec_open [R, 5] int64 scratch for the numbers decided exactly); rec_i [R, 6] int64 image index, category index (-1: not in the ground truth), raw span of
+ *   'counts' in text, h, w; rec_n [R] int64 decoded counts length; rec_b [R] uint8 flags (coco_results_file.cuh).
+ * dt_coco_file_finish: offsets = the inclusive scan of rec_n, num_chars its total; chars [num_chars + 1]; segm 1 for loadRes's segm
+ *   branch; workspace of dt_coco_file_finish_workspace_bytes.  det_key [num_records] int64: the keys (category index * num_images + image
+ *   index) sorted; the first num_kept rows (the records of known categories) of det_f [.., 5], det_i [.., 4] (dt_coco_eval's layout),
+ *   det_area (loadRes's area) and det_id (1 + the record's index in the file), in key order, stable.
+ * All return 0 on bad sizes or a NULL pointer. */
+int64_t dt_coco_file_struct_workspace_bytes(int64_t num_bytes);
+int dt_coco_file_struct(int64_t num_bytes, const uint8_t* text, void* workspace, int64_t* info, dt_stream_t stream);
+int dt_coco_file_separators(int64_t num_bytes, void* workspace, int64_t* separators, dt_stream_t stream);
+int dt_coco_file_records(int64_t num_records, int64_t num_bytes, const uint8_t* text, const int64_t* separators, int num_images,
+                         const int64_t* img_ids, int num_cats, const int64_t* cat_ids, double* rec_f, int64_t* rec_open, int64_t* rec_i,
+                         int64_t* rec_n, uint8_t* rec_b, int64_t* info, dt_stream_t stream);
+int64_t dt_coco_file_finish_workspace_bytes(int64_t num_records, int64_t num_chars, int segm);
+int dt_coco_file_finish(int64_t num_records, int segm, const uint8_t* text, const int64_t* rec_i, const int64_t* rec_n, const int64_t* offsets,
+                        const uint8_t* rec_b, double* rec_f, int num_images, int num_cats, int64_t num_chars, char* chars, void* workspace,
+                        int64_t num_kept, int64_t* det_key, double* det_f, int64_t* det_i, double* det_area, int64_t* det_id, int64_t* info,
+                        dt_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Proposal recall (Detectron's evaluate_box_proposals), bit for bit.  One CTA per (image, combination); every combination of
